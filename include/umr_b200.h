@@ -16,6 +16,8 @@
  *   umr_chamfer_forward / _backward  replace nnutils/chamfer_python.py:43-64 (`distChamfer`).
  *   umr_texcycle_forward / _backward replace nnutils/loss_utils.py:152-182 (`TexCycle.forward`).
  *   umr_corr_chamfer_forward / _backward replace nnutils/loss_utils.py:218-248 (`CorrLossChamfer.forward`).
+ *   umr_nmr_forward / umr_nmr_backward_textures replace the render of `neural_renderer.Renderer` (driven by
+ *       nnutils/nmr_pytorch.py; the upstream package is not vendored, its contract is DESIGN.md §7).
  *
  * Conventions: plain device pointers + sizes, no torch types.  Every buffer is CALLER-allocated
  * (torch owns all memory); the library keeps no global mutable state and is re-entrant across host
@@ -311,6 +313,42 @@ int umr_dt_barrier(const float* mask, float* dt, void* workspace, int32_t B, int
 size_t umr_p2p_allreduce_flag_bytes(void);
 int umr_p2p_allreduce(const void* peer_buffers_dev, float* out, int64_t n_floats, int64_t flag_offset_bytes,
                       void* local_state, int32_t rank, int32_t world, float scale, void* stream);
+
+/* Hard z-buffer renderer with neural_renderer's conventions: the `Renderer` of nnutils/nmr_pytorch.py:42-43 in UMR's
+ * configuration (look_at camera with the eye on the z axis, orthographic), forward and texture gradient.  The render
+ * contract is DESIGN.md §7.  The vertex / camera gradient is not built (every UMR call site renders detached geometry). */
+typedef struct UmrNmrParams {
+    int32_t batch_size, num_vertices, num_faces; /* B, V, F */
+    int32_t texture_res;       /* T: textures [B/G, F, T, T, T, 3] (>= 2); ignored without textures */
+    int32_t image_size;        /* output side `is`; raster side S = is * (anti_aliasing ? 2 : 1) */
+    int32_t anti_aliasing;     /* 1: rasterise at 2*is, then 2x2 average pool */
+    int32_t fill_back;         /* 1: faces F..2F-1 are faces 0..F-1 with the vertex order reversed */
+    int32_t shared_textures;   /* G: G consecutive renders share one texture (camera hypotheses); 0 or 1: per render */
+    float eye_z;               /* look_at eye = (0, 0, eye_z), eye_z < 0: a translation z - eye_z */
+    float near_plane, far_plane;
+    float light_intensity_ambient, light_intensity_directional;
+    float light_color_ambient[3], light_color_directional[3], light_direction[3];
+    float background_color[3];
+} UmrNmrParams;
+
+size_t umr_sizeof_nmr_params(void);
+/* Bytes of 256-byte aligned device scratch umr_nmr_forward / umr_nmr_backward_textures need. */
+size_t umr_nmr_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t fill_back);
+/* vertices [B,V,3] f32 (what nmr_pytorch.Render hands over: orthographic_proj_withz(..., offset_z=5) with y negated),
+ * faces [B,F,3] int32 (an index outside [0,V) makes that face invisible), textures [B/G,F,T,T,T,3] f32 or NULL.
+ * Outputs, all fully written:
+ *   face_index   [B,S,S] int32  winning face copy per raster pixel (raster row order, not flipped), -1 = background
+ *   raster_depth [B,S,S] f32    its depth, far_plane where no face wins
+ *   rgb          [B,3,is,is]    flipped + pooled image (NULL to skip; needs textures)
+ *   alpha, depth [B,is,is]      flipped + pooled coverage / depth (NULL to skip) */
+int umr_nmr_forward(const float* vertices, const int32_t* faces, const float* textures, int32_t* face_index,
+                    float* raster_depth, float* rgb, float* alpha, float* depth, const UmrNmrParams* params,
+                    void* workspace, void* stream);
+/* Texture gradient of the rgb output: grad_rgb [B,3,is,is] -> grad_textures [B/G,F,T,T,T,3] (zero-filled by the call,
+ * then accumulated).  face_index is the forward's plane; vertices / faces / params are the forward's. */
+int umr_nmr_backward_textures(const float* vertices, const int32_t* faces, const int32_t* face_index,
+                              const float* grad_rgb, float* grad_textures, const UmrNmrParams* params, void* workspace,
+                              void* stream);
 
 #ifdef __cplusplus
 }

@@ -38,6 +38,16 @@ class UmrProjectParams(ctypes.Structure):
                 ("light_direction", ctypes.c_float * 3), ("num_hypotheses", ctypes.c_int32)]
 
 
+class UmrNmrParams(ctypes.Structure):
+    _fields_ = [("batch_size", ctypes.c_int32), ("num_vertices", ctypes.c_int32), ("num_faces", ctypes.c_int32),
+                ("texture_res", ctypes.c_int32), ("image_size", ctypes.c_int32), ("anti_aliasing", ctypes.c_int32),
+                ("fill_back", ctypes.c_int32), ("shared_textures", ctypes.c_int32),
+                ("eye_z", ctypes.c_float), ("near_plane", ctypes.c_float), ("far_plane", ctypes.c_float),
+                ("light_intensity_ambient", ctypes.c_float), ("light_intensity_directional", ctypes.c_float),
+                ("light_color_ambient", ctypes.c_float * 3), ("light_color_directional", ctypes.c_float * 3),
+                ("light_direction", ctypes.c_float * 3), ("background_color", ctypes.c_float * 3)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "umr_error_string": (ctypes.c_char_p, [ctypes.c_int]),
@@ -97,6 +107,11 @@ EXPORTS = {
     "umr_texcycle_forward": (ctypes.c_int, [c_f32p] * 5 + [ctypes.c_int32] * 3 + [ctypes.c_int64,
                                                                                 ctypes.c_void_p]),
     "umr_texcycle_backward": (ctypes.c_int, [c_f32p] * 5 + [ctypes.c_int32] * 3 + [ctypes.c_void_p]),
+    "umr_sizeof_nmr_params": (ctypes.c_size_t, []),
+    "umr_nmr_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 3),
+    "umr_nmr_forward": (ctypes.c_int, [c_f32p] * 8 + [ctypes.POINTER(UmrNmrParams), ctypes.c_void_p, ctypes.c_void_p]),
+    "umr_nmr_backward_textures": (ctypes.c_int, [c_f32p] * 5 + [ctypes.POINTER(UmrNmrParams), ctypes.c_void_p,
+                                                                ctypes.c_void_p]),
 }
 
 _lock = threading.Lock()
@@ -124,7 +139,8 @@ def load():
                 fn.restype = res
                 fn.argtypes = args
             if (lib.umr_sizeof_raster_params() != ctypes.sizeof(UmrRasterParams)
-                    or lib.umr_sizeof_project_params() != ctypes.sizeof(UmrProjectParams)):
+                    or lib.umr_sizeof_project_params() != ctypes.sizeof(UmrProjectParams)
+                    or lib.umr_sizeof_nmr_params() != ctypes.sizeof(UmrNmrParams)):
                 raise UmrLibraryError("libumr_b200.so was built from a different include/umr_b200.h than this binding "
                                       "(parameter struct sizes differ): rebuild with `python -m umr_b200.build --force`")
             _lib = lib

@@ -257,16 +257,42 @@ class MultiMaskLoss(nn.Module):
         return expected_over_hypotheses(per_render, cam_probs), mask_all_hypo
 
 
+class NeuralRenderer(nn.Module):
+    """nmr_pytorch.py:89-128 (`NeuralRenderer`) as MultiTextureLoss(renderer="nmr") uses it: orthographic projection with
+    offset_z = 5, y flip, textured NMR render of detached geometry.  Camera hypotheses are broadcast like SoftRenderer's:
+    vertices / faces / textures [B, ...], cams [B*H, 7] -> B*H renders."""
+
+    def __init__(self, img_size=256):
+        super().__init__()
+        from ..neural_renderer import Renderer
+        self.renderer = Renderer(image_size=img_size, anti_aliasing=True, camera_mode="look_at", perspective=False,
+                                 background_color=[0, 0, 0])
+        self.renderer.eye = [0, 0, -2.732]
+        self.renderer.light_intensity_ambient = 0.8
+        self.offset_z = 5.
+
+    def ambient_light_only(self):
+        self.renderer.light_intensity_ambient = 1
+        self.renderer.light_intensity_directional = 0
+
+    def forward(self, vertices, faces, cams, textures):
+        H = cams.size(0) // vertices.size(0)
+        verts = geom_utils.orthographic_proj_withz(tile_hypotheses(vertices, H), cams, offset_z=self.offset_z)
+        verts[:, :, 1] *= -1  # nmr_pytorch.py:76-77
+        return self.renderer.render_rgb(verts, tile_hypotheses(faces, H), textures)
+
+
 class MultiTextureLoss(nn.Module):
-    """loss_utils.py:277-331, `renderer="smr"`.  `texture_loss_type` defaults to "perceptual" like the
-    reference; that branch needs the reference's LPIPS module (see PerceptualTextureLoss)."""
+    """loss_utils.py:277-331.  `texture_loss_type` defaults to "perceptual" like the reference; that branch needs the
+    reference's LPIPS module (see PerceptualTextureLoss)."""
 
     def __init__(self, samples_per_gpu=32, num_hypo_cams=8, image_size=256, renderer_type="softmax",
                  texture_loss_type="perceptual", renderer="smr"):
         super().__init__()
-        if renderer not in "smr":
-            raise NotImplementedError("only the SoftRas-based renderer ('smr') is on the hot path")
-        self.renderer = SoftRenderer(image_size, renderer_type)
+        if renderer in "smr":   # substring tests, like the reference (:282, :309)
+            self.renderer = SoftRenderer(image_size, renderer_type)
+        else:
+            self.renderer = NeuralRenderer(image_size)
         self.renderer.ambient_light_only()
         self.hard_renderer = SoftRenderer(image_size, "hard")
         if texture_loss_type in "perceptual":   # substring test, like the reference (:289)
@@ -284,8 +310,13 @@ class MultiTextureLoss(nn.Module):
         # textured softmax render of every hypothesis; vertices detached: only the texture learns here (:313)
         # ... and neither is the [B*8,F,T2,3] texture copy of loss_utils.py:305 (70.8 MB at batch 16): the raster kernels
         # read textures[b // 8] and accumulate the 8 hypotheses' texture gradients directly
-        texture_rgba, _, _ = self.renderer.forward(vs.detach(), fs, cams_all_hypo.view(-1, 7), tx)
-        texture_pred = texture_rgba[:, 0:3, :, :]
+        if self.which_renderer in "nmr":
+            # loss_utils.py:310: the 36 texels of a face as a 6x6 image, repeated along the cube's first axis
+            cube = tx.view(tx.size(0), tx.size(1), 6, 6, 3).unsqueeze(2).expand(-1, -1, 6, -1, -1, -1)
+            texture_pred = self.renderer.forward(vs.detach(), fs, cams_all_hypo.view(-1, 7), cube)
+        else:
+            texture_rgba, _, _ = self.renderer.forward(vs.detach(), fs, cams_all_hypo.view(-1, 7), tx)
+            texture_pred = texture_rgba[:, 0:3, :, :]
         per_render = self.texture_loss(texture_pred, tile_hypotheses(rgbs, H), tile_hypotheses(masks_gt, H),
                                        masks_pred, avg=False)
         tex_loss = expected_over_hypotheses(per_render, cam_probs)
