@@ -1,5 +1,5 @@
 """Kernel time (library events) of the visibility passes at a C3-like shape: visible-face bytes (k_visible_faces, face-parallel)
-vs planes (k_raster_fwd3<2>, per pixel).  UMR_VISIBILITY_IMPL=pixel forces the per-pixel kernel for the bytes (A/B)."""
+vs planes (k_raster_fwd3<2>, per pixel)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -17,4 +17,4 @@ for mode in ("faces", "planes"):
         raster.visibility(fv, IS, want_faces=(mode == "faces"), **kw)
     torch.cuda.synchronize(); raster.set_profile_sink(None)
     pr = raster.collect_profile(sink)
-    print("visibility %s: %.3f ms (32 x 2048^2, F=1280), impl=%s" % (mode, sum(pr["fwd"]) / len(pr["fwd"]), os.environ.get("UMR_VISIBILITY_IMPL", "default")))
+    print("visibility %s: %.3f ms (32 x 2048^2, F=1280)" % (mode, sum(pr["fwd"]) / len(pr["fwd"])))

@@ -8,7 +8,7 @@ import os
 import threading
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("UMR_B200_LIB") or os.path.join(_PKG, "libumr_b200.so")  # override: A/B kernel builds only
+LIB_PATH = os.environ.get("UMR_B200_LIB") or os.path.join(_PKG, "libumr_b200.so")  # override: load another build, e.g. to compare two builds' outputs
 
 c_f32p = ctypes.c_void_p  # raw device pointers are passed as integers (tensor.data_ptr())
 

@@ -36,14 +36,8 @@ def _stale(target, deps):
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False, variant=None, extra=()):
-    """variant/extra: A/B builds for kernel experiments -- `libumr_b200_<variant>.so` compiled with extra nvcc
-    flags (e.g. -DUMR_FWD2_CTAS=4), selected at run time with UMR_B200_LIB=<path>."""
+def build(force=False, verbose=False):
     nvcc = os.environ.get("NVCC", "nvcc")
-    global OBJ, LIB
-    if variant:
-        OBJ = os.path.join(PKG, "csrc", "_obj_" + variant)
-        LIB = os.path.join(PKG, "libumr_b200_%s.so" % variant)
     os.makedirs(OBJ, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     headers.append(os.path.join(ROOT, "include", "umr_b200.h"))
@@ -53,7 +47,7 @@ def build(force=False, verbose=False, variant=None, extra=()):
         o = os.path.join(OBJ, src[:-3] + ".o")
         objs.append(o)
         if force or _stale(o, [s] + headers):
-            cmd = [nvcc, *ARCH, *COMMON, *PER_FILE.get(src, []), *extra, "-c", s, "-o", o]
+            cmd = [nvcc, *ARCH, *COMMON, *PER_FILE.get(src, []), "-c", s, "-o", o]
             if verbose:
                 cmd.insert(1, "-Xptxas=-v")
                 print(" ".join(cmd))
@@ -67,8 +61,4 @@ def build(force=False, verbose=False, variant=None, extra=()):
 
 
 if __name__ == "__main__":
-    var = None
-    if "--variant" in sys.argv:
-        var = sys.argv[sys.argv.index("--variant") + 1]
-    extra = [a for a in sys.argv[1:] if a.startswith("-D")]
-    print(build("--force" in sys.argv, "--verbose" in sys.argv, var, extra))
+    print(build("--force" in sys.argv, "--verbose" in sys.argv))

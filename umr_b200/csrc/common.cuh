@@ -69,14 +69,10 @@ __device__ __forceinline__ void red_add_global(float* addr, float v) {
 // (p, p+1) / (p+1, p+2) is 8-byte aligned goes out as one vector RED (REDG.E.ADD.F32x2, sm_90+), the odd one as a scalar.
 // Selected by address parity, no divergence.  The texel REDs are a large part of the streaming backward's memory traffic.
 __device__ __forceinline__ void red_add3_global(float* p, float a, float b, float c) {
-#ifdef UMR_RED_SCALAR
-    red_add_global(p, a); red_add_global(p + 1, b); red_add_global(p + 2, c);
-#else
     const bool mis = (reinterpret_cast<uintptr_t>(p) & 4u) != 0;  // p itself is not 8-byte aligned -> (p+1, p+2) is the pair
     float* pv = p + (mis ? 1 : 0);
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(pv), "f"(mis ? b : a), "f"(mis ? c : b) : "memory");
     asm volatile("red.global.add.f32 [%0], %1;" ::"l"(p + (mis ? 0 : 2)), "f"(mis ? a : c) : "memory");
-#endif
 }
 // four floats of a 16-byte aligned slot in ONE reduction (REDG.E.ADD.F32x4)
 __device__ __forceinline__ void red_add4_global(float* p, float a, float b, float c, float d) {

@@ -1,5 +1,5 @@
 // raster_fwd3.cuh -- forward of the round-2 pipeline, per-pixel formulation (included by raster.cu after
-// raster_stream.cuh).  The pair-parallel forward k_raster_fwd2 spends its gain in lane utilisation on two
+// raster_stream.cuh).  A pair-parallel forward spends its gain in lane utilisation on two
 // extra CTA phases per sub-chunk, so the forward keeps the round-1 inner loop -- thread = pixel, faces walked in ascending
 // index -- and gains: the tile list comes from the coarse bins (no scan of all F cull boxes), untouched tiles take a
 // store-only fast path, a warp skips every face whose cull rectangle misses its 8x4 pixel block, and survivors are
@@ -9,18 +9,15 @@
 
 namespace umr {
 
+// CTAs per SM: same-box A/B at C2: 3 CTAs (80 registers) and 5 CTAs (48 registers, 88 B of spills: 0.461 vs 0.386 ms) both lose
+constexpr int FWD3_CTAS = 4;
+
 // RGB: 0 = hard z-buffer colours, 1 = softmax aggregation, 2 = VISIBILITY ONLY -- the winning face of the hard z-buffer
 // (aggrs planes: depth_min, face_index_min) and nothing else: no distance / sigmoid / alpha / colour arithmetic, no image
 // planes.  That is all `MultiTextureLoss` keeps of its hard render (loss_utils.py:327-329: `_, p2f, aggr = hard_renderer(...)`,
 // and p2f is zero in hard mode, kernel.cu:417-431).  Same winner as RGB = 0, bit for bit.
 template <int RGB, int NC = 3>  // NC colour channels (3, or 4: the part-map render of SURVEY.md 8f-2); planes = NC + 1 (alpha)
-#ifndef UMR_FWD3_POS_TABLE
-#define UMR_FWD3_POS_TABLE 1   // rank table instead of __fns in issue(): same-box A/B 0.385 -> 0.381 ms at C2 (0 restores the intrinsic)
-#endif
-#ifndef UMR_FWD3_CTAS
-#define UMR_FWD3_CTAS 4   // same-box A/B at C2: 3 CTAs (80 registers) and 5 CTAs (48 registers, 88 B of spills: 0.461 vs 0.386 ms) both lose
-#endif
-__global__ void __launch_bounds__(CTA, UMR_FWD3_CTAS) k_raster_fwd3(const float* __restrict__ rec_all, const float4* __restrict__ box_all,
+__global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __restrict__ rec_all, const float4* __restrict__ box_all,
                                                         const uint16_t* __restrict__ clist, const int* __restrict__ ccount,
                                                         const float* __restrict__ textures, float* __restrict__ images,
                                                         float* __restrict__ colors_hi, float* __restrict__ aggrs,
@@ -42,9 +39,7 @@ __global__ void __launch_bounds__(CTA, UMR_FWD3_CTAS) k_raster_fwd3(const float*
     __shared__ uint32_t s_warp_blk[NWARP];
     __shared__ uint32_t s_segbase;
     __shared__ int s_save;
-#if UMR_FWD3_POS_TABLE
     __shared__ uint8_t s_pos[NWARP][WG];      // list offset of the r-th face of the warp's current issue mask
-#endif
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.z;
@@ -297,24 +292,17 @@ __global__ void __launch_bounds__(CTA, UMR_FWD3_CTAS) k_raster_fwd3(const float*
                 const int base = g * WG;
                 m = __ballot_sync(0xffffffffu, lane < WG && base + lane < n && (s_meet[min(base + lane, n - 1)] & wbit));
                 const int cntm = __popc(m);
-#if UMR_FWD3_POS_TABLE
-                // rank -> list offset through a 16-byte per-warp table (the find-n-th-set-bit intrinsic is a software loop)
+                // rank -> list offset through a 16-byte per-warp table (the find-n-th-set-bit intrinsic is a software loop;
+                // same-box A/B 0.385 -> 0.381 ms at C2)
                 if ((m >> lane) & 1u) s_pos[warp][__popc(m & lt)] = (uint8_t)lane;
                 __syncwarp();
-#endif
                 for (int r = lane >> 3; r < cntm; r += 4) {
-#if UMR_FWD3_POS_TABLE
-                    const int e = s_pos[warp][r];
-#else
-                    const int e = __fns(m, 0, r + 1);  // list offset of the r-th face this warp needs
-#endif
+                    const int e = s_pos[warp][r];  // list offset of the r-th face this warp needs
                     const int f = s_list[base + e];
                     cp_async16(wst + ((size_t)(g & 1) * WG + r) * REC_F + (lane & 7) * 4, rec_img + (size_t)f * REC_F + (lane & 7) * 4);
                 }
             }
-#if UMR_FWD3_POS_TABLE
             __syncwarp();  // table reads done before the next issue() rewrites it
-#endif
             cp_async_commit();
             return m;
         };

@@ -18,7 +18,6 @@ namespace umr {
 
 constexpr int T4 = 32;            // tile side
 constexpr int FWD4_CAP = 1536;    // tile-list entries held in shared memory (10 bytes each)
-constexpr int FWD4_MAX_F = 65535; // (any F: longer coarse lists take the windowed slow path)
 constexpr int WG4 = 16;           // list entries per warp group
 
 __host__ __device__ inline size_t fwd4_dyn_smem(int F) { return (size_t)(F < FWD4_CAP ? F : FWD4_CAP) * 10 + 16; }
