@@ -65,7 +65,7 @@ typedef struct UmrRasterParams {
     void* ev_kernel_start;
     void* ev_kernel_stop;
     /* optional PAIR BUFFER (device memory, 256-byte aligned, caller-allocated like every other buffer): when given,
-     * the forward saves one 48-byte record per surviving (pixel, face) pair and the backward streams them instead
+     * the forward saves one 32-byte record per surviving (pixel, face) pair and the backward streams them instead
      * of re-deriving the geometry (the role `faces_info`/`soft_colors` play as saved tensors in the reference,
      * functional/soft_rasterize.py:75).  It must be the SAME memory, untouched, in the matching backward call.
      * Tiles whose records do not fit are recomputed in the backward -- results are identical, only slower -- so any
@@ -105,8 +105,10 @@ int umr_event_elapsed_ms(void* start, void* stop, float* ms); /* synchronises on
 
 /* Bytes of scratch `workspace` umr_raster_forward/backward need (256-byte aligned device memory). */
 size_t umr_raster_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t image_size, int32_t anti_aliasing);
-/* Bytes of a pair buffer (UmrRasterParams.pair_buffer) holding `capacity_blocks` blocks of 32 pair records
- * (1540 bytes each) plus the per-tile headers. */
+/* Bytes of a pair buffer (UmrRasterParams.pair_buffer) holding at least `capacity_blocks` blocks of 32 pair records
+ * plus the per-tile headers.  It reserves 1540 bytes per block while a block takes 1028 (32 records of 32 bytes and a
+ * 4-byte header), so the buffer holds about 1.5x `capacity_blocks`: renders denser than the caller's estimate keep all
+ * their records instead of recomputing tiles in the backward. */
 size_t umr_raster_pair_buffer_bytes(int32_t batch_size, int32_t image_size, int32_t anti_aliasing,
                                     uint64_t capacity_blocks);
 

@@ -52,7 +52,7 @@ constexpr int R_INV = 9;   // 9 : barycentric inverse, row-major
 constexpr int R_SYM = 18;  // 6 : s00 s01 s02 s11 s12 s22   (Gram + 1)
 constexpr int R_BOX = 24;  // 4 : xlo xhi ylo yhi (cull box, already expanded by r)
 constexpr int R_FLG = 28;  // 1 : bit0..2 obtuse corner, bit3 front-facing
-constexpr int R_IZ2 = 29;  // 3 : 1 / (z_k * z_k)  (backward z-gradient factor, saved per pair by the forward)
+constexpr int R_IZ2 = 29;  // 3 : 1 / (z_k * z_k)  (backward z-gradient factor)
 
 struct WorkspaceLayout {
     size_t rec_off, box_off, p2f_off, ubox_off, ccount_off, clist_off, total;
@@ -90,7 +90,8 @@ __device__ __forceinline__ uint32_t ubox_key(float v) {
 __global__ void __launch_bounds__(256) k_prep(const float* __restrict__ fv, float* __restrict__ rec,
                                               float4* __restrict__ box, uint32_t* __restrict__ ubox, int F, float r,
                                               const uint32_t* __restrict__ only_if_nonzero = nullptr) {
-    // backward with a pair buffer: the records are only needed by the recompute fallback -- skip when no tile needs it
+    // texture-only backward with a pair buffer: the records are only needed by the recompute fallback -- skip when no tile
+    // needs it
     if (only_if_nonzero != nullptr && __ldg(only_if_nonzero) == 0u) return;
     const int fidx = blockIdx.x * blockDim.x + threadIdx.x;
     const bool valid = fidx < F;
@@ -1373,11 +1374,11 @@ using namespace umr;
 // k_raster_bwd2 instantiation for the call: texture-only (grad_faces == NULL) and warp-level texel pre-reduction variants
 // exist for the texture-gradient kernels only
 template <int RGBM, bool TG, int TS>
-static void launch_bwd2(dim3 grid, cudaStream_t stream, bool pre, const float* textures, const float* soft_colors,
+static void launch_bwd2(dim3 grid, cudaStream_t stream, bool pre, const float* rec, const float* textures, const float* soft_colors,
                         const float* aggrs_info, const float* grad_images, float* grad_faces, float* grad_textures,
                         const Consts& K, const PairBuf& pb) {
 #define UMR_BWD2_GO(GEOMV, PREV) \
-    k_raster_bwd2<RGBM, TG, TS, 3, GEOMV, PREV><<<grid, BWD2_THREADS, 0, stream>>>(textures, soft_colors, aggrs_info, grad_images, \
+    k_raster_bwd2<RGBM, TG, TS, 3, GEOMV, PREV><<<grid, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images, \
                                                                                     grad_faces, grad_textures, K, pb)
     if constexpr (TG && RGBM == 1) {
         if (pre) { if (grad_faces) UMR_BWD2_GO(true, true); else UMR_BWD2_GO(false, true); }
@@ -1403,10 +1404,16 @@ extern "C" size_t umr_raster_workspace_bytes(int32_t B, int32_t F, int32_t image
     return ws_layout(B, F, image_size * (anti_aliasing ? 2 : 1)).total;
 }
 
+// Reserves PAIR_BLOCK_RESERVE bytes per block where a block takes BLK_F4 * 16 + 4 = 1028: callers size the buffer from
+// an estimate of the blocks a render wants, and the extra capacity keeps renders denser than the estimate off the
+// recompute path without growing the buffer.
+constexpr size_t PAIR_BLOCK_RESERVE = 1540;
 extern "C" size_t umr_raster_pair_buffer_bytes(int32_t B, int32_t image_size, int32_t anti_aliasing,
                                                uint64_t capacity_blocks) {
     if (B <= 0 || image_size <= 0) return 0;
-    return pair_layout(B, image_size * (anti_aliasing ? 2 : 1), (size_t)capacity_blocks).total + 1024;
+    const size_t blk = (size_t)BLK_F4 * sizeof(float4) + sizeof(uint32_t);
+    return pair_layout(B, image_size * (anti_aliasing ? 2 : 1), (size_t)capacity_blocks).total +
+           (size_t)capacity_blocks * (PAIR_BLOCK_RESERVE - blk) + 1024;
 }
 
 // device pointers into the caller's pair buffer (cap == 0: no saving)
@@ -1696,8 +1703,11 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
     if (e != cudaSuccess) return (int)e;
     const bool gen = is_generic(p);
     const PairBuf pb = gen ? PairBuf{nullptr, nullptr, nullptr, nullptr, nullptr, 0u} : make_pairbuf(p, K.S);
-    // (with a pair buffer the records only serve the recompute fallback: k_prep returns at once when no tile needs it)
-    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, r, pb.cap > 0 ? pb.ctrl + 1 : nullptr);
+    // The streamed backward re-derives its z-gradient factors from the records whenever it forms vertex gradients; a
+    // texture-only backward with a pair buffer needs them only for the recompute fallback, so k_prep returns at once there
+    // when no tile is unsaved.
+    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, r,
+                                                         (pb.cap > 0 && !grad_faces) ? pb.ctrl + 1 : nullptr);
     count_launch();
     if (grad_faces) {
         e = cudaMemsetAsync(grad_faces, 0, (size_t)n * 9 * sizeof(float), stream);
@@ -1721,10 +1731,10 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
             if (pb.cap > 0) {                                                                                 \
                 count_launch();                                                                               \
                 if (forward_impl(p->tile_mode) == 4)                                                          \
-                    launch_bwd2<RGBM, TG, 32>(grid32, stream, tex_pre, textures, soft_colors, aggrs_info, grad_images, \
+                    launch_bwd2<RGBM, TG, 32>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, grad_images, \
                                               grad_faces, grad_textures, K, pb);                              \
                 else                                                                                          \
-                    launch_bwd2<RGBM, TG, 16>(grid_pairs, stream, tex_pre, textures, soft_colors, aggrs_info, grad_images, \
+                    launch_bwd2<RGBM, TG, 16>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, aggrs_info, grad_images, \
                                               grad_faces, grad_textures, K, pb);                              \
             }                                                                                                 \
             if (pb.cap > 0)                                                                                   \
@@ -1753,7 +1763,7 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
     if (nc4) {  // 16x16 tiles, softmax, no texture gradient (check_params / above)
         if (pb.cap > 0) {
             count_launch();
-            k_raster_bwd2<1, false, 16, 4><<<grid_pairs, BWD2_THREADS, 0, stream>>>(textures, soft_colors, aggrs_info, grad_images, grad_faces,
+            k_raster_bwd2<1, false, 16, 4><<<grid_pairs, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images, grad_faces,
                                                                             grad_textures, K, pb);
             k_raster_bwd_pairs_list<1, false, 4><<<list_grid, CTA, smem, stream>>>(rec, box, textures, soft_colors, aggrs_info, grad_images,
                                                                                    grad_faces, grad_textures, ubox, K, pb.ctrl + 1,

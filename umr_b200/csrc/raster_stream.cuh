@@ -9,9 +9,10 @@
 //   k_bin_coarse     one CTA per 64x64-pixel bin scans the image's F cull boxes ONCE (TMA-staged, ordered
 //                    ballot compaction) -> ascending face list per bin.  Tiles scan their bin's list
 //                    (~100-200 entries) instead of F (1280 / 5120).
-//   pair records     the forward writes one 48-byte record per surviving pair that passes the depth range
+//   pair records     the forward writes one 32-byte record per surviving pair that passes the depth range
 //                    (32-slot blocks, survivors compacted to the block front, block-SoA so a warp writes
-//                    three fully coalesced 512-byte lines).
+//                    two fully coalesced 512-byte lines).  The z-gradient factors w_clip_k / z_k^2 are not
+//                    saved: the backward re-derives them bit for bit from the face record and the pixel.
 //   k_raster_bwd2    one CTA per tile streams the tile's blocks: no cull boxes, no fragment(), no barrier
 //                    after the per-pixel inputs are staged; a warp owns a contiguous block range, so the 9
 //                    vertex gradients are accumulated privately and flushed (shuffle reduce + 9 RED) once per
@@ -26,14 +27,14 @@ constexpr int CB = 64;             // coarse bin side in pixels (4 x 4 tiles)
 constexpr int LCAP = 512;          // coarse-list window == longest tile-list segment held in shared memory
 constexpr uint32_t SEG_NONE = 0xffffffffu;
 constexpr int32_t TILE_EMPTY = -1, TILE_UNSAVED = -2;
-constexpr int BLK_F4 = 96;         // float4 per block: 3 planes x 32 records
+constexpr int BLK_F4 = 64;         // float4 per block: 2 planes x 32 records
 
 struct PairBuf {
     uint32_t* ctrl;      // [0] block cursor (== blocks wanted, may exceed cap), [1] tiles left unsaved
     int32_t* tile_head;  // [B * tiles]: first segment (block index), TILE_EMPTY or TILE_UNSAVED
     int32_t* ulist;      // [B * tiles]: ids of the unsaved tiles (count = ctrl[1]), walked by the recompute fallback
     uint32_t* blk_hdr;   // [cap]: per block  face | count << 16 ; per segment  [base] = #blocks, [base+1] = next
-    float4* recs;        // [cap][3][32]
+    float4* recs;        // [cap][2][32]
     uint32_t cap;        // blocks
 };
 
@@ -219,13 +220,16 @@ constexpr int BWD2_THREADS = 256, BWD2_WARPS = BWD2_THREADS / 32;  // threads of
 // the same texel of the step's face (found with match.any) are summed by the lowest of them, which issues the only REDs.
 // Pays only when a face covers hundreds of raster pixels per texel (raster.cu: TEXGRAD_PRE_RATIO_*); at UMR's shapes the
 // plain vector REDs are faster.
+// rec_all: the face records of k_prep (GEOM only): the z-gradient factors w_clip_k / z_k^2 are re-derived from them
 template <int RGB, bool TEXGRAD, int TS, int NC = 3, bool GEOM = true, bool PRE = false>  // NC colour channels; pixel planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
-__global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const float* __restrict__ textures, const float* __restrict__ colors_hi,
+__global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const float* __restrict__ rec_all, const float* __restrict__ textures,
+                                                        const float* __restrict__ colors_hi,
                                                         const float* __restrict__ aggrs, const float* __restrict__ grad_images,
                                                         float* __restrict__ grad_faces, float* __restrict__ grad_tex, Consts K,
                                                         PairBuf pb) {
     constexpr int NPL = NC + 1, NV = 2 * NPL + 2;
     __shared__ float s_pix[NV][TS * TS];  // g[NC], g_alpha, C[NC], alpha, ssum, smax (row-major tile pixels)
+    __shared__ float s_xp[TS], s_yp[TS];  // pixel centres, built as the forward builds its tables (same bits)
     constexpr int NP = TS * TS;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.z;
@@ -234,6 +238,10 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
     const int32_t head = __ldg(pb.tile_head + tile_id);
     if (head < 0) return;  // empty, or unsaved (k_raster_bwd_pairs handles it)
     const int x0 = blockIdx.x * TS, y0 = blockIdx.y * TS;
+    if (GEOM) {
+        if (tid < TS) s_xp[tid] = pixel_coord(x0 + tid, S);
+        else if (tid < 2 * TS) s_yp[tid - TS] = pixel_coord(S - 1 - (y0 + tid - TS), S);
+    }
     for (int pi = tid; pi < NP; pi += BWD2_THREADS) {
         const int px = x0 + (pi % TS), py = y0 + (pi / TS);
         const size_t np = (size_t)S * S;
@@ -263,6 +271,12 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
     const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
     float* gtex_img = TEXGRAD ? grad_tex + (size_t)(b / K.tex_div) * K.tex_bs : nullptr;
     float* gf_img = grad_faces + (size_t)b * F * 9;
+    const float* rec_img = GEOM ? rec_all + (size_t)b * F * REC_F : nullptr;
+    // the 128-byte face record of a step is pulled into L1 one step ahead: lanes 1-3 take the 32-byte sectors that hold
+    // R_INV and R_IZ2
+    auto prefetch_face = [&](int f) {
+        if (lane >= 1 && lane < 4) asm volatile("prefetch.global.L1 [%0];" ::"l"(rec_img + (size_t)f * REC_F + 8 * lane));
+    };
 
     float acc[9];
 #pragma unroll
@@ -298,7 +312,7 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
         uint32_t hw = (kbeg + lane < kend) ? __ldg(hdrs + kbeg + lane) : 0u;
         int o = 0;
         // plan(): the next step of the stream -- its face, whether this lane carries a record, and where the record is --
-        // and advance (k, o).  Planning runs one step AHEAD of the arithmetic so that the step's three 16-byte lines per lane
+        // and advance (k, o).  Planning runs one step AHEAD of the arithmetic so that the step's two 16-byte lines per lane
         // can be prefetched into L1 while the previous step is being processed (the kernel is bound by the latency of
         // these loads).
         auto plan = [&](int& f_out, bool& act_out, const float4*& src_out) -> bool {
@@ -347,30 +361,31 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
         };
         // The records of step i + 1 are prefetched into L1 while step i is processed, so the loads' latency is covered by a
         // whole step of arithmetic.
-        auto prefetch3 = [&](bool act, const float4* p) {
+        auto prefetch2 = [&](bool act, const float4* p) {
             if (act) {
                 asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
                 asm volatile("prefetch.global.L1 [%0];" ::"l"(p + 32));
-                asm volatile("prefetch.global.L1 [%0];" ::"l"(p + 64));
             }
         };
         int f_c = 0, f_n = 0;
         bool act_c = false, act_n = false;
         const float4 *src_c = nullptr, *src_n = nullptr;
         bool have = plan(f_c, act_c, src_c);
-        if (have) prefetch3(act_c, src_c);
+        if (have) prefetch2(act_c, src_c);
+        if (GEOM && have) prefetch_face(f_c);
         while (have) {
             const bool have_n = plan(f_n, act_n, src_n);
-            if (have_n) prefetch3(act_n, src_n);
-            const int f = f_c;
+            if (have_n) prefetch2(act_n, src_n);
+            const int f = f_c;  // (warp-uniform, like f_n and have_n)
             if (f != cur_f) { flush(); cur_f = f; }
+            if (GEOM && have_n && f_n != f) prefetch_face(f_n);
             int pre_tix = -1;   // PRE: this lane's texel of face f and its NC gradient terms (set below when it contributes)
             float pre_v[NC];
 #pragma unroll
             for (int c = 0; c < NC; ++c) pre_v[c] = 0.f;
             if (act_c) {
                 const float4* src = src_c;
-                const float4 r0 = __ldg(src), r1 = __ldg(src + 32), r2 = __ldg(src + 64);
+                const float4 r0 = __ldg(src), r1 = __ldg(src + 32);
                 const float D = r0.x, sdx = r0.y, sdy = r0.z, zn = r0.w;  // zn: normalised depth exactly as the forward formed it
                 const uint32_t meta = __float_as_uint(r1.w);
                 const int pix = TS == 16 ? (int)(meta & 0xffu) : (int)(meta & 0x3ffu);
@@ -426,9 +441,17 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
                                 Cxy += __fdividef(Crgb, D);
                                 const float zp = K.far_ - zn * (K.far_ - K.near_);
                                 const float Cz = Crgb * K.r_gamma * K.r_nf * zp * zp;  // :624
-                                acc[2] += Cz * r2.x;
-                                acc[5] += Cz * r2.y;
-                                acc[8] += Cz * r2.z;
+                                // w_clip_k / z_k^2 (kernel.cu:624-627) exactly as the forward forms them: the w of
+                                // fragment(), clip_bary, times the face record's 1 / z_k^2
+                                const float* q = rec_img + (size_t)f * REC_F;
+                                const float xp = s_xp[pix % TS], yp = s_yp[pix / TS];
+                                float k0 = __ldg(q + R_INV + 0) * xp + __ldg(q + R_INV + 1) * yp + __ldg(q + R_INV + 2);
+                                float k1 = __ldg(q + R_INV + 3) * xp + __ldg(q + R_INV + 4) * yp + __ldg(q + R_INV + 5);
+                                float k2 = __ldg(q + R_INV + 6) * xp + __ldg(q + R_INV + 7) * yp + __ldg(q + R_INV + 8);
+                                clip_bary(k0, k1, k2);
+                                acc[2] += Cz * (k0 * __ldg(q + R_IZ2 + 0));
+                                acc[5] += Cz * (k1 * __ldg(q + R_IZ2 + 1));
+                                acc[8] += Cz * (k2 * __ldg(q + R_IZ2 + 2));
                             }
                         }
                     }
