@@ -352,6 +352,21 @@ int umr_nmr_backward_textures(const float* vertices, const int32_t* faces, const
                               const float* grad_rgb, float* grad_textures, const UmrNmrParams* params, void* workspace,
                               void* stream);
 
+/* Mesh voxelisation: SoftRas `functional.voxelization` (functional/voxelization.py:41-58, kernels
+ * cuda/voxelization_cuda_kernel.cu).  faces [B,F,3,3] (float32 or float64 as `dtype` says, contiguous; coordinates are
+ * multiplied by `scale` in that type first: `size`, or 1 for normalize=True) -> voxels [B,vs,vs,vs] int32 (16-byte
+ * aligned, fully written): 1 for surface voxels and every empty voxel not 6-connected through empty voxels to the grid
+ * boundary, 0 elsewhere.  Bit-exact with the reference's `-fmad=false` build; NaN / inf mark nothing.  The contract is
+ * DESIGN.md §8.  workspace: umr_voxelize_workspace_bytes(B, vs) bytes of 256-byte aligned device scratch.  Its first
+ * uint32 is a status word, cleared at the start of every call: non-zero when the fill stopped at its sweep cap, i.e.
+ * when the result is wrong (a library bug, never expected).  One memset and at most three kernels, whatever the mesh;
+ * no allocation, no synchronisation (CUDA-graph capturable).  UMR_ERR_TOO_LARGE when B*vs^3 >= 2^31. */
+#define UMR_DTYPE_FLOAT32 0
+#define UMR_DTYPE_FLOAT64 1
+size_t umr_voxelize_workspace_bytes(int32_t B, int32_t vs);
+int umr_voxelize(const void* faces, int32_t dtype, int32_t* voxels, int32_t B, int32_t F, int32_t vs, double scale,
+                 void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

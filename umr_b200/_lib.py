@@ -112,6 +112,9 @@ EXPORTS = {
     "umr_nmr_forward": (ctypes.c_int, [c_f32p] * 8 + [ctypes.POINTER(UmrNmrParams), ctypes.c_void_p, ctypes.c_void_p]),
     "umr_nmr_backward_textures": (ctypes.c_int, [c_f32p] * 5 + [ctypes.POINTER(UmrNmrParams), ctypes.c_void_p,
                                                                 ctypes.c_void_p]),
+    "umr_voxelize_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_voxelize": (ctypes.c_int, [c_f32p, ctypes.c_int32, c_f32p] + [ctypes.c_int32] * 3 + [ctypes.c_double, ctypes.c_void_p,
+                                                                                           ctypes.c_void_p]),
 }
 
 _lock = threading.Lock()

@@ -15,7 +15,7 @@ extern "C" const char* umr_error_string(int code) {
     return "unknown error";
 }
 
-extern "C" int umr_version(void) { return 203; }  // 200: round-2 ABI (pair buffer, workspace size takes the image size); 201: color_channels, texture-only backward; 202: umr_nmr_*; 203: 32-byte pair records
+extern "C" int umr_version(void) { return 204; }  // 200: round-2 ABI (pair buffer, workspace size takes the image size); 201: color_channels, texture-only backward; 202: umr_nmr_*; 203: 32-byte pair records; 204: umr_voxelize*
 extern "C" size_t umr_sizeof_raster_params(void) { return sizeof(UmrRasterParams); }
 extern "C" size_t umr_sizeof_project_params(void) { return sizeof(UmrProjectParams); }
 

@@ -496,3 +496,44 @@ class CorrChamferFunction(torch.autograd.Function):
 
 def corr_chamfer(verts, cams, selection, targets, part_ends, weights):
     return CorrChamferFunction.apply(verts, cams, selection, *targets, part_ends, weights)
+
+
+_VOXEL_DTYPES = {torch.float32: 0, torch.float64: 1}  # UMR_DTYPE_FLOAT32 / UMR_DTYPE_FLOAT64
+_voxel_status = {}  # device -> the status word of the last voxelize call on that device
+
+
+def voxelize(faces, size, normalize=False):
+    """SoftRas `functional.voxelization` (functional/voxelization.py:41-58): faces [B,F,3,3] float32 or float64 -> int32
+    [B,size,size,size], 1 for surface voxels and enclosed empty voxels.  Coordinates are multiplied by `size` first
+    unless `normalize` (the reference's `normalize` branch leaves them as they are).  `faces` is not modified; the result
+    is on its device.  Contract: DESIGN.md §8."""
+    size = int(size)
+    if size < 1:
+        raise ValueError("voxelize: size must be >= 1, got %d" % size)
+    _need_cuda(faces)
+    if faces.dtype not in _VOXEL_DTYPES:
+        raise TypeError("voxelize: faces must be float32 or float64, got %s" % faces.dtype)
+    if faces.dim() != 4 or faces.shape[2:] != (3, 3):
+        raise ValueError("voxelize: faces must be [B, F, 3, 3], got %s" % (tuple(faces.shape),))
+    lib = _lib.load()
+    f = faces.detach().contiguous()
+    B, F_ = f.shape[0], f.shape[1]
+    dtype, scale = _VOXEL_DTYPES[f.dtype], 1.0 if normalize else float(size)
+    nbytes = lib.umr_voxelize_workspace_bytes(B, size)
+    if nbytes == 0:  # sizes the library refuses: it checks them before the buffers, so let it say which
+        _lib.check(lib.umr_voxelize(_ptr(f), dtype, None, B, F_, size, scale, None, None), "umr_voxelize")
+    with torch.cuda.device(f.device):
+        out = torch.empty((B, size, size, size), dtype=torch.int32, device=f.device)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=f.device)
+        rc = lib.umr_voxelize(_ptr(f), dtype, _ptr(out), B, F_, size, scale, _ptr(ws), _stream_ptr(f.device))
+    _lib.check(rc, "umr_voxelize")
+    _voxel_status[f.device] = ws[:4].view(torch.int32)
+    return out
+
+
+def voxelize_status(device=None):
+    """The status word of the last `voxelize` call on `device` (synchronises): 0, or non-zero when the fill stopped at
+    its sweep cap, which only a library bug can cause."""
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    st = _voxel_status.get(device)
+    return 0 if st is None else int(st.item())

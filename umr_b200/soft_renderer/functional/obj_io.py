@@ -1,9 +1,10 @@
-"""Wavefront OBJ texture I/O of the drop-in package on the H100 kernels (csrc/mesh_ops.cu).
+"""Wavefront OBJ I/O of the drop-in package on the H100 kernels (csrc/mesh_ops.cu).
 
 Reference: SoftRas/functional/save_obj.py:9-33 (`create_texture_image`: face textures -> atlas image through
-cuda/create_texture_image), :36-90 (`save_obj`), functional/load_obj.py:9-101 (`load_mtl`, `load_textures`: atlas image ->
-face textures through cuda/load_textures).  Image files are read / written with PIL (the reference uses skimage, which is
-not a dependency here); everything between the file and the tensors follows the reference.
+cuda/create_texture_image), :36-90 (`save_obj`), :96-104 (`save_voxel`), functional/load_obj.py:9-101 (`load_mtl`,
+`load_textures`: atlas image -> face textures through cuda/load_textures), :104-167 (`load_obj`).  Image files are read /
+written with PIL (the reference uses skimage, which is not a dependency here); everything between the file and the tensors
+follows the reference.
 """
 import os
 
@@ -137,3 +138,56 @@ def load_textures(filename_obj, filename_mtl, texture_res, device="cuda"):
         is_update = torch.from_numpy((names == mname).astype(np.int32)).to(device)
         textures = ops.load_textures(image, faces, textures, is_update)
     return textures
+
+
+def load_obj(filename_obj, normalization=False, load_texture=False, texture_res=4, texture_type="surface"):
+    """functional/load_obj.py:104-167: vertices [V,3] float32 and faces [F,3] int32 (polygons fan-triangulated) on the
+    GPU, plus the textures with `load_texture` (surface: [F, texture_res^2, 3] from the .mtl; vertex: the colours of the
+    `v` lines).  `normalization` centres and scales the vertices into [-1, 1]."""
+    if texture_type not in ("surface", "vertex"):
+        raise ValueError("texture type not applicable")
+    verts, faces = [], []
+    with open(filename_obj) as fh:
+        for line in fh:
+            tok = line.split()
+            if not tok:
+                continue
+            if tok[0] == "v":
+                verts.append([float(x) for x in tok[1:4]])
+            elif tok[0] == "f":
+                ids = [int(x.split("/")[0]) - 1 for x in tok[1:]]
+                faces.extend([ids[0], ids[k], ids[k + 1]] for k in range(1, len(ids) - 1))  # fan triangulation
+    v = torch.tensor(verts, dtype=torch.float32).cuda()
+    f = torch.tensor(faces, dtype=torch.int32).cuda()
+    if normalization:  # centre and scale into [-1, 1]
+        v = v - v.min(0)[0][None, :]
+        v = v / torch.abs(v).max()
+        v = v * 2
+        v = v - v.max(0)[0][None, :] / 2
+    if not load_texture:
+        return v, f
+    if texture_type == "surface":  # :139-146
+        with open(filename_obj) as fh:
+            mtl = [ln.split()[1] for ln in fh if ln.startswith("mtllib")]
+        if not mtl:
+            raise Exception("Failed to load textures.")
+        textures = load_textures(filename_obj, os.path.join(os.path.dirname(filename_obj), mtl[-1]), texture_res)
+    else:  # :147-154: colours ride on the `v` lines
+        with open(filename_obj) as fh:
+            cols = [[float(x) for x in ln.split()[4:7]] for ln in fh if ln.split() and ln.split()[0] == "v"]
+        textures = torch.tensor(cols, dtype=torch.float32).cuda()
+    return v, f, textures
+
+
+def save_voxel(filename, voxel):
+    """save_obj.py:96-104: one OBJ vertex (i/n0, j/n1, k/n2) per voxel equal to 1, in i, j, k order, and no faces.  (The
+    reference hands its own `save_obj` a 1-D empty face tensor, which that function's assertion rejects; this writes the
+    file it means to write, in `save_obj`'s format.)"""
+    vox = voxel.detach().cpu().numpy() if torch.is_tensor(voxel) else np.asarray(voxel)
+    idx = np.argwhere(vox == 1)  # row-major: the reference's i, j, k loop order
+    verts = (idx / np.asarray(vox.shape, dtype=np.float64)).astype(np.float32)  # torch.tensor(list of floats): float32
+    with open(filename, "w") as f:
+        f.write("# %s\n#\n\n" % os.path.basename(filename))
+        for v in verts:
+            f.write("v %.8f %.8f %.8f\n" % (v[0], v[1], v[2]))
+        f.write("\n")

@@ -5,7 +5,6 @@ quantities (`face_vertices`, `surface_normals`, `vertex_normals`) are cached unt
 reassigned.  OBJ loading / saving (incl. the texture atlas kernels) live in functional/obj_io.py.
 """
 import numpy as np
-import os
 
 import torch
 import torch.nn.functional as F
@@ -142,34 +141,15 @@ class Mesh(object):
 
     @classmethod
     def from_obj(cls, filename_obj, normalization=False, load_texture=False, texture_res=1, texture_type="surface"):
-        verts, faces = [], []
-        with open(filename_obj) as fh:
-            for line in fh:
-                tok = line.split()
-                if not tok:
-                    continue
-                if tok[0] == "v":
-                    verts.append([float(x) for x in tok[1:4]])
-                elif tok[0] == "f":
-                    ids = [int(x.split("/")[0]) - 1 for x in tok[1:]]
-                    faces.extend([ids[0], ids[k], ids[k + 1]] for k in range(1, len(ids) - 1))  # fan triangulation
-        v = torch.tensor(verts, dtype=torch.float32).cuda()
-        f = torch.tensor(faces, dtype=torch.int32).cuda()
-        if normalization:  # functional/load_obj.py: centre and scale into [-1, 1]
-            v = v - v.min(0)[0][None, :]
-            v = v / torch.abs(v).max()
-            v = v * 2
-            v = v - v.max(0)[0][None, :] / 2
-        textures = None
-        if load_texture and texture_type == "surface":  # functional/load_obj.py:139-146
-            from .functional.obj_io import load_textures
-            with open(filename_obj) as fh:
-                mtl = [ln.split()[1] for ln in fh if ln.startswith("mtllib")]
-            if not mtl:
-                raise Exception("Failed to load textures.")
-            textures = load_textures(filename_obj, os.path.join(os.path.dirname(filename_obj), mtl[-1]), texture_res)
-        elif load_texture and texture_type == "vertex":  # :147-154: colours ride on the `v` lines
-            with open(filename_obj) as fh:
-                cols = [[float(x) for x in ln.split()[4:7]] for ln in fh if ln.split() and ln.split()[0] == "v"]
-            textures = torch.tensor(cols, dtype=torch.float32).cuda()
-        return cls(v, f, textures, texture_res, texture_type)
+        from .functional.obj_io import load_obj
+        loaded = load_obj(filename_obj, normalization, load_texture, texture_res, texture_type)
+        textures = loaded[2] if load_texture else None
+        return cls(loaded[0], loaded[1], textures, texture_res, texture_type)
+
+    def voxelize(self, voxel_size=32):
+        """SoftRas/mesh.py:177-179: the face vertices mapped by x * vs / (vs - 1) + 0.5, voxelised at vs^3 through the
+        `voxelization` kernels -> int32 [B, vs, vs, vs]."""
+        if voxel_size < 2:
+            raise ValueError("voxel_size must be >= 2 (the reference divides by voxel_size - 1), got %r" % (voxel_size,))
+        face_vertices_norm = self.face_vertices * voxel_size / (voxel_size - 1) + 0.5
+        return srf.voxelization(face_vertices_norm, voxel_size, False)
