@@ -71,6 +71,8 @@ typedef struct UmrRasterParams {
      * Tiles whose records do not fit are recomputed in the backward -- results are identical, only slower -- so any
      * size is valid; umr_raster_pair_buffer_bytes() sizes it.  After the forward, the first uint32 of the buffer
      * holds the number of 32-record blocks the render wanted, the second the number of tiles left unsaved.
+     * A record keeps the sampled texel's index in a bit field of 23 bits with 16x16 tiles and 21 bits with 32x32 tiles;
+     * a texture_size above 2^23 (2^21) saves nothing and the backward recomputes every tile.
      * NULL / 0: nothing is saved (forward-only renders, generic modes). */
     void* pair_buffer;
     uint64_t pair_buffer_bytes;

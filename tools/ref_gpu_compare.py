@@ -19,8 +19,6 @@ import torch.nn.functional as F
 
 from umr_b200 import raster, synth
 
-DIST_EPS_LOG = float(np.log(1.0 / 1e-10 - 1.0))
-
 
 def load(name):
     path = os.path.join(ROOT, "oracle", "_ref", name + ".so")
@@ -32,8 +30,17 @@ def load(name):
     return m
 
 
-def ref_forward(mod, fv, tex, S, rgb):
-    """functional/soft_rasterize.py:41-73 restated with device-side allocations."""
+def _mode_args(sigma_val, dist, dist_eps, gamma_val, rgb, alpha, texture, double_side):
+    # (image_size precedes) near, far, eps, sigma, func_id_dist, dist_eps (log form, soft_rasterize.py:35), gamma,
+    # func_id_rgb, func_id_alpha, texture_sample_type, double_side
+    return (1.0, 100.0, 1e-3, sigma_val, dist, float(np.log(1.0 / dist_eps - 1.0)), gamma_val, rgb, alpha, texture,
+            bool(double_side))
+
+
+def ref_forward(mod, fv, tex, S, rgb, sigma_val=1e-5, dist=2, dist_eps=1e-10, gamma_val=1e-4, alpha=2, texture=0,
+                double_side=True):
+    """functional/soft_rasterize.py:41-73 restated with device-side allocations.  Mode ids as in raster.FUNC_*; the
+    defaults are UMR's configuration."""
     B, Fn = fv.shape[:2]
     dev = fv.device
     faces_info = torch.zeros(B, Fn, 27, device=dev)
@@ -44,16 +51,17 @@ def ref_forward(mod, fv, tex, S, rgb):
     colors[:, :3] = 0.0
     theta = torch.tensor([[1, 0, 0], [0, 1, 0]], dtype=torch.float)
     grid = F.affine_grid(theta.unsqueeze(0), (1, 1, S, S), align_corners=True).view(S, S, 2).to(dev).contiguous()
-    mod.forward_soft_rasterize(fv, tex, faces_info, aggrs, grid, p2f, p2f_sum, colors, S, 1.0, 100.0, 1e-3, 1e-5, 2,
-                               DIST_EPS_LOG, 1e-4, rgb, 2, 0, True)
+    mod.forward_soft_rasterize(fv, tex, faces_info, aggrs, grid, p2f, p2f_sum, colors, S,
+                               *_mode_args(sigma_val, dist, dist_eps, gamma_val, rgb, alpha, texture, double_side))
     return colors, p2f / p2f_sum.clamp_min(1e-12), aggrs, faces_info
 
 
-def ref_backward(mod, fv, tex, colors, faces_info, aggrs, g, S, rgb):
+def ref_backward(mod, fv, tex, colors, faces_info, aggrs, g, S, rgb, sigma_val=1e-5, dist=2, dist_eps=1e-10,
+                 gamma_val=1e-4, alpha=2, texture=0, double_side=True):
     gf = torch.zeros_like(fv)
     gt = torch.zeros_like(tex)
-    mod.backward_soft_rasterize(fv, tex, colors, faces_info, aggrs, gf, gt, g.contiguous(), S, 1.0, 100.0, 1e-3, 1e-5, 2,
-                                DIST_EPS_LOG, 1e-4, rgb, 2, 0, True)
+    mod.backward_soft_rasterize(fv, tex, colors, faces_info, aggrs, gf, gt, g.contiguous(), S,
+                                *_mode_args(sigma_val, dist, dist_eps, gamma_val, rgb, alpha, texture, double_side))
     return gf, gt
 
 

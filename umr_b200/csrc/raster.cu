@@ -1416,11 +1416,19 @@ extern "C" size_t umr_raster_pair_buffer_bytes(int32_t B, int32_t image_size, in
            (size_t)capacity_blocks * (PAIR_BLOCK_RESERVE - blk) + 1024;
 }
 
-// device pointers into the caller's pair buffer (cap == 0: no saving)
+// Texel-index bits of a pair record's meta word: pixel index below, front flag in bit 31.  16x16 tiles (k_raster_fwd3,
+// also the 4-channel render) keep 8 pixel bits, 32x32 tiles (k_raster_fwd4) 10.
+static int pair_texel_bits(const UmrRasterParams* p) {
+    return (p->color_channels != 4 && forward_impl(p->tile_mode) == 4) ? 21 : 23;
+}
+
+// device pointers into the caller's pair buffer (cap == 0: no saving; also when T2 does not fit the record's texel field,
+// so the backward recomputes every tile)
 static PairBuf make_pairbuf(const UmrRasterParams* p, int S) {
     PairBuf pb;
     pb.ctrl = nullptr; pb.tile_head = nullptr; pb.ulist = nullptr; pb.blk_hdr = nullptr; pb.recs = nullptr; pb.cap = 0;
     if (!p->pair_buffer || p->pair_buffer_bytes == 0 || ((uintptr_t)p->pair_buffer & 255) != 0) return pb;
+    if (p->texture_size > (1 << pair_texel_bits(p))) return pb;
     size_t cap = pair_capacity(p->batch_size, S, (size_t)p->pair_buffer_bytes);
     if (cap > 0x7fff0000u) cap = 0x7fff0000u;
     if (cap < 4) return pb;

@@ -403,7 +403,8 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
                         float4* dst = pb.recs + (size_t)blk * BLK_F4 + __popc(m & lt);
                         // closest-point barycentrics as the reference forms them: t_k + w_k (kernel.cu:638-641)
                         const float u0 = fr.t0 + fr.w0, u1 = fr.t1 + fr.w1, u2 = fr.t2 + fr.w2;
-                        const uint32_t meta = (uint32_t)(lrow * TILE + lcol) | (tix << 8) | (front << 24);
+                        // meta: pixel in bits 0-7, texel in bits 8-30 (T2 <= 2^23, make_pairbuf), front in bit 31
+                        const uint32_t meta = (uint32_t)(lrow * TILE + lcol) | (tix << 8) | (front << 31);
                         dst[0] = make_float4(fr.D, fr.sign * fr.dx, fr.sign * fr.dy, zsave);
                         dst[32] = make_float4(u0, u1, u2, __uint_as_float(meta));
                     }

@@ -389,8 +389,8 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
                 const float D = r0.x, sdx = r0.y, sdy = r0.z, zn = r0.w;  // zn: normalised depth exactly as the forward formed it
                 const uint32_t meta = __float_as_uint(r1.w);
                 const int pix = TS == 16 ? (int)(meta & 0xffu) : (int)(meta & 0x3ffu);
-                const int tix = TS == 16 ? (int)((meta >> 8) & 0xffffu) : (int)((meta >> 10) & 0x3fffu);
-                const bool front = (meta >> 24) & 1u;
+                const int tix = TS == 16 ? (int)((meta >> 8) & 0x7fffffu) : (int)((meta >> 10) & 0x1fffffu);
+                const bool front = (meta >> 31) != 0u;
                 const float* sp = &s_pix[0][pix];
                 float Cxy = 0.f;
                 if (GEOM) {
