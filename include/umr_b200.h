@@ -39,7 +39,11 @@ extern "C" {
 #define UMR_OK 0
 #define UMR_ERR_UNSUPPORTED (-1) /* mode combination not built into the sm_90a kernels        */
 #define UMR_ERR_BAD_ARG (-2)     /* null pointer / non-positive size / misaligned buffer       */
-#define UMR_ERR_TOO_LARGE (-3)   /* size beyond a compiled limit (e.g. num_faces > 65535)      */
+#define UMR_ERR_TOO_LARGE (-3)   /* size beyond a compiled limit (e.g. num_faces > UMR_RASTER_MAX_FACES) */
+
+/* Largest num_faces of the soft rasteriser: 2^24.  The hard render's face-index plane holds face ids as float, exact
+ * below 2^24, and the pair-block headers of meshes above 65535 faces keep 24 face bits. */
+#define UMR_RASTER_MAX_FACES 16777216
 
 /* mode ids: same numbering as functional/soft_rasterize.py:22-25 */
 enum { UMR_DIST_HARD = 0, UMR_DIST_BARYCENTRIC = 1, UMR_DIST_EUCLIDEAN = 2 };
@@ -52,7 +56,8 @@ enum { UMR_TEX_SURFACE = 0, UMR_TEX_VERTEX = 1 };
  * receives (functional/soft_rasterize.py:35). */
 typedef struct UmrRasterParams {
     int32_t batch_size;    /* B */
-    int32_t num_faces;     /* F (<= 65535) */
+    int32_t num_faces;     /* F (<= UMR_RASTER_MAX_FACES); F <= 65535 keeps 16-bit face indices, larger meshes take
+                            * the 32-bit-index instantiations of the same kernels */
     int32_t texture_size;  /* T2 = texture_res^2 (surface textures [B,F,T2,3]) */
     int32_t image_size;    /* output image side `is`; raster side S = is * (anti_aliasing ? 2 : 1) */
     int32_t anti_aliasing; /* 1: rasterise at 2*is and 2x2 average-pool (rasterizer.py:43,52-53) */
@@ -105,7 +110,8 @@ int umr_event_destroy(void* event);
 int umr_event_record(void* event, void* stream);
 int umr_event_elapsed_ms(void* start, void* stop, float* ms); /* synchronises on `stop` */
 
-/* Bytes of scratch `workspace` umr_raster_forward/backward need (256-byte aligned device memory). */
+/* Bytes of scratch `workspace` umr_raster_forward/backward need (256-byte aligned device memory).  F > 65535: the
+ * coarse-bin lists share a pool of 8 entries per face (DESIGN.md §3); bins that overflow it stay correct. */
 size_t umr_raster_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t image_size, int32_t anti_aliasing);
 /* Bytes of a pair buffer (UmrRasterParams.pair_buffer) holding at least `capacity_blocks` blocks of 32 pair records
  * plus the per-tile headers.  It reserves 1540 bytes per block while a block takes 1028 (32 records of 32 bytes and a

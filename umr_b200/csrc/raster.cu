@@ -54,23 +54,48 @@ constexpr int R_BOX = 24;  // 4 : xlo xhi ylo yhi (cull box, already expanded by
 constexpr int R_FLG = 28;  // 1 : bit0..2 obtuse corner, bit3 front-facing
 constexpr int R_IZ2 = 29;  // 3 : 1 / (z_k * z_k)  (backward z-gradient factor)
 
+// Face indices.  Meshes of up to NARROW_MAX_FACES faces keep them in 16 bits (coarse-bin lists, tile lists, pair-block
+// headers); larger meshes take the wide instantiations (IdxT = uint32_t) of the same kernels.  The hard render's
+// face-index plane stores face ids as float, exact below 2^24, which bounds F (UMR_RASTER_MAX_FACES).
+constexpr int NARROW_MAX_FACES = 65535;
+// Pair-block header: face | count << HDR_SHIFT (count <= 32).  16 face bits (narrow) or 24 (wide).
+template <typename IdxT>
+__host__ __device__ constexpr int hdr_shift() { return sizeof(IdxT) == 2 ? 16 : 24; }
+// Generic kernels and the recompute backward hold a tile list of window-relative u16 offsets in shared memory: faces are
+// listed and consumed in ascending windows of at most FACE_WINDOW faces (one window when F <= 65535).
+constexpr int FACE_WINDOW = 65536;
+
 struct WorkspaceLayout {
     size_t rec_off, box_off, p2f_off, ubox_off, ccount_off, clist_off, total;
+    size_t clist_cap;  // wide layout: entries of the shared coarse-list pool
 };
 __host__ __device__ inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 constexpr int COARSE_BIN = 64;  // == CB in raster_stream.cuh
+// Wide coarse lists: one pool for all bins, WIDE_BIN_ENTRIES entries (32 bytes) per face; a bin whose list does not fit
+// is marked and its consumers walk every face instead (same result, box tests filter them).
+constexpr size_t WIDE_BIN_ENTRIES = 8;
+constexpr uint32_t BIN_ALL_FACES = 0xffffffffu;
 // S = raster side (0: no coarse-bin lists, e.g. the generic-mode kernels)
 inline WorkspaceLayout ws_layout(int B, int F, int S) {
     WorkspaceLayout L;
     const size_t n = (size_t)B * F;
     const size_t ncb = (size_t)(S + COARSE_BIN - 1) / COARSE_BIN;
+    const size_t nbin = (size_t)B * ncb * ncb;
     L.rec_off = 0;
     L.box_off = align256(n * REC_F * sizeof(float));
     L.p2f_off = L.box_off + align256(n * sizeof(float4));
     L.ubox_off = L.p2f_off + align256(n * 4 * sizeof(float));
     L.ccount_off = L.ubox_off + align256((size_t)B * 4 * sizeof(uint32_t));
-    L.clist_off = L.ccount_off + align256((size_t)B * ncb * ncb * sizeof(int));
-    L.total = L.clist_off + align256((size_t)B * ncb * ncb * F * sizeof(uint16_t));
+    if (F <= NARROW_MAX_FACES) {  // ccount int[nbin], clist u16[nbin][F]
+        L.clist_cap = 0;
+        L.clist_off = L.ccount_off + align256(nbin * sizeof(int));
+        L.total = L.clist_off + align256(nbin * F * sizeof(uint16_t));
+    } else {  // ccount {count, pool offset}[nbin] + the pool cursor (u64), clist u32[clist_cap]
+        L.clist_cap = n * WIDE_BIN_ENTRIES;
+        if (L.clist_cap > 0xfffffff0u) L.clist_cap = 0xfffffff0u;
+        L.clist_off = L.ccount_off + align256(nbin * 2 * sizeof(uint32_t) + sizeof(unsigned long long));
+        L.total = L.clist_off + align256(L.clist_cap * sizeof(uint32_t));
+    }
     return L;
 }
 
@@ -416,9 +441,11 @@ __host__ __device__ inline size_t smem_list_off(int F) {
 // on an mbarrier; the scan then runs out of shared memory.  Each warp owns a contiguous run of the
 // piece (ascending face order = warp-major, round, lane), keeps its ballots in registers, and one
 // barrier per piece turns the per-warp counts into list offsets.  Returns the list length (uniform).
+// `list` == nullptr: count only.
+template <typename IdxT = uint16_t>
 __device__ __forceinline__ int build_tile_list(const float4* __restrict__ box, int F, float tx_first,
                                                float tx_last, float ty_bot, float ty_top, float4* s_box,
-                                               uint16_t* list, int* s_warp_cnt, uint64_t* bar, uint32_t& phase) {
+                                               IdxT* list, int* s_warp_cnt, uint64_t* bar, uint32_t& phase) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     int total = 0;
     for (int base = 0; base < F; base += BOX_PIECE) {
@@ -453,10 +480,12 @@ __device__ __forceinline__ int build_tile_list(const float4* __restrict__ box, i
             total += c;
         }
         const uint32_t lt = (1u << lane) - 1u;
+        if (sizeof(IdxT) == 2 || list != nullptr) {
 #pragma unroll
-        for (int r = 0; r < BOX_PIECE / (NWARP * 32); ++r) {
-            if ((masks[r] >> lane) & 1u) list[off + __popc(masks[r] & lt)] = (uint16_t)(base + warp * per + r * 32 + lane);
-            off += __popc(masks[r]);
+            for (int r = 0; r < BOX_PIECE / (NWARP * 32); ++r) {
+                if ((masks[r] >> lane) & 1u) list[off + __popc(masks[r] & lt)] = (IdxT)(base + warp * per + r * 32 + lane);
+                off += __popc(masks[r]);
+            }
         }
         __syncthreads();  // list visible; s_box / s_warp_cnt reusable
     }
@@ -549,12 +578,9 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
     __syncthreads();
 
     const float4* box = box_all + (size_t)b * F;
-    const float* rec_img = rec_all + (size_t)b * F * REC_F;
     uint32_t bar_phase = 0;
-    const int n = tile_outside_union(ubox, b, s_ext)
-                      ? 0
-                      : build_tile_list(box, F, s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, s_list, s_warp_cnt, &s_bar, bar_phase);
-    // (build_tile_list ends with __syncthreads: the list is visible)
+    const bool outside = tile_outside_union(ubox, b, s_ext);
+    bool any = false;  // some window listed a face (uniform)
 
     // pixel state (kernel.cu:335-348)
     float acc_a = K.alpha == UMR_ALPHA_PROD ? 1.f : 0.f;  // alpha accumulator (kernel.cu:335-336)
@@ -566,17 +592,23 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
     float zmin = 10000000.f;
     int fid = -1;
 
-    const int nchunk = (n + CHUNK - 1) / CHUNK;
-    if (nchunk > 0) {
-        issue_chunk(rec_img, s_list, n, 0, s_rec);
-        issue_chunk(rec_img, s_list, n, 1, s_rec);
-    }
     const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
     // torch-1.1 affine_grid (align_corners=True) coordinates of this pixel: linspace(-1, 1, S)
     const float gstep = 2.f / (float)(S - 1);
     const float gx = (px * 2 < S) ? (-1.f + gstep * px) : (1.f - gstep * (S - 1 - px));
     const float gy = (py * 2 < S) ? (-1.f + gstep * py) : (1.f - gstep * (S - 1 - py));
 
+    for (int wb = 0; wb < F && !outside; wb += FACE_WINDOW) {
+    const int n = build_tile_list(box + wb, min(F - wb, FACE_WINDOW), s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, s_list,
+                                  s_warp_cnt, &s_bar, bar_phase);
+    // (build_tile_list ends with __syncthreads: the list is visible)
+    any = any || n > 0;
+    const float* rec_img = rec_all + ((size_t)b * F + wb) * REC_F;
+    const int nchunk = (n + CHUNK - 1) / CHUNK;
+    if (nchunk > 0) {
+        issue_chunk(rec_img, s_list, n, 0, s_rec);
+        issue_chunk(rec_img, s_list, n, 1, s_rec);
+    }
     for (int c = 0; c < nchunk; ++c) {
         const int st = c % NSTAGE;
         const int cnt = min(CHUNK, n - c * CHUNK);
@@ -608,7 +640,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
                     if (!(zp < K.near_ || zp > K.far_)) {
                         const uint32_t flg = __float_as_uint(rc[R_FLG]);
                         const bool front = (flg & 8u) != 0;
-                        const int f = s_list[c * CHUNK + j];
+                        const int f = wb + s_list[c * CHUNK + j];
                         if (RGB == 0) {
                             const bool inside = fr.w0 <= 1 && fr.w0 >= 0 && fr.w1 <= 1 && fr.w1 >= 0 &&
                                                 fr.w2 <= 1 && fr.w2 >= 0;
@@ -650,13 +682,14 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
             bb = bbn;
         }
         if (RGB == 1 && p2f_acc != nullptr && own_w != 0.f) {  // one global RED per (warp, face, component)
-            float* dst = p2f_acc + ((size_t)b * F + s_list[c * CHUNK + lane]) * 4;
+            float* dst = p2f_acc + ((size_t)b * F + wb + s_list[c * CHUNK + lane]) * 4;
             red_add_global(dst + 0, own_x);
             red_add_global(dst + 1, own_y);
             red_add_global(dst + 2, own_w);
         }
         __syncthreads();  // everyone is done with stage st
         issue_chunk(rec_img, s_list, n, c + NSTAGE, s_rec);  // commits an empty group past the end
+    }
     }
 
     // finalise (kernel.cu:443-475)
@@ -679,7 +712,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
     // pooled values: avg_pool2d(2,2) = ((a00 + a01) + a10) + a11, then /4 (rasterizer.py:52-53)
     float v[4] = {o0, o1, o2, alpha};
     if (K.aa) {
-        if (n > 0) {  // uniform
+        if (any) {  // uniform
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 const float a01 = __shfl_xor_sync(0xffffffffu, v[k], 1);
@@ -802,11 +835,17 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
     for (int i = tid; i < CHUNK * 9; i += CTA) (&s_g[0][0])[i] = 0.f;
     __syncthreads();
     const float4* box = box_all + (size_t)b * F;
-    const float* rec_img = rec_all + (size_t)b * F * REC_F;
     if (tile_outside_union(ubox, b, s_ext)) return;  // uniform
     uint32_t bar_phase = 0;
-    const int n = build_tile_list(box, F, s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, s_list, s_warp_cnt, &s_bar, bar_phase);
-    if (n == 0) return;  // uniform
+    float g0 = 0, g1 = 0, g2 = 0, g3 = 0, C0 = 0, C1 = 0, C2 = 0, C3 = 0, ssum = 1, smax = 0;
+    bool loaded = false;  // per-pixel inputs, read once the first window lists a face
+    const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
+    float* gtex_img = TEXGRAD ? grad_tex + (size_t)(b / K.tex_div) * K.tex_bs : nullptr;
+    for (int wb = 0; wb < F; wb += FACE_WINDOW) {
+    const int n = build_tile_list(box + wb, min(F - wb, FACE_WINDOW), s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, s_list,
+                                  s_warp_cnt, &s_bar, bar_phase);
+    if (n == 0) continue;  // uniform
+    const float* rec_img = rec_all + ((size_t)b * F + wb) * REC_F;
 
     const int nchunk = (n + CHUNK - 1) / CHUNK;
     issue_chunk(rec_img, s_list, n, 0, s_rec);
@@ -814,8 +853,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
 
     // per-pixel inputs
     const size_t np = (size_t)S * S;
-    float g0 = 0, g1 = 0, g2 = 0, g3 = 0, C0 = 0, C1 = 0, C2 = 0, C3 = 0, ssum = 1, smax = 0;
-    if (live) {
+    if (live && !loaded) {
         const size_t p = (size_t)py * S + px;
         if (K.aa) {  // avg_pool2d backward: g / 4
             const size_t nq = (size_t)K.IS * K.IS;
@@ -837,8 +875,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
         ssum = __ldg(aggrs + ((size_t)b * 2 + 0) * np + p);
         smax = __ldg(aggrs + ((size_t)b * 2 + 1) * np + p);
     }
-    const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
-    float* gtex_img = TEXGRAD ? grad_tex + (size_t)(b / K.tex_div) * K.tex_bs : nullptr;
+    loaded = true;
 
     for (int c = 0; c < nchunk; ++c) {
         const int st = c % NSTAGE;
@@ -880,7 +917,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
                         contrib = true;
                         const uint32_t flg = __float_as_uint(rc[R_FLG]);
                         const bool front = (flg & 8u) != 0;
-                        const int f = s_list[c * CHUNK + j];
+                        const int f = wb + s_list[c * CHUNK + j];
                         float gz0 = 0.f, gz1 = 0.f, gz2 = 0.f;
                         if (RGB == 0) {
                             if ((float)f == smax) {  // aggrs[1] = winning face id (:596)
@@ -961,11 +998,12 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
             const float v = (&s_g[0][0])[i];
             if (v != 0.f) {
                 const int j = i / 9, k = i - j * 9;
-                red_add_global(grad_faces + ((size_t)b * F + s_list[c * CHUNK + j]) * 9 + k, v);
+                red_add_global(grad_faces + ((size_t)b * F + wb + s_list[c * CHUNK + j]) * 9 + k, v);
                 (&s_g[0][0])[i] = 0.f;
             }
         }
         issue_chunk(rec_img, s_list, n, c + NSTAGE, s_rec);
+    }
     }
 }
 
@@ -1167,15 +1205,20 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
     __syncthreads();
     if (tile_outside_union(ubox, b, s_ext)) return;  // uniform
     const float4* box = box_all + (size_t)b * F;
-    const float* rec_img = rec_all + (size_t)b * F * REC_F;
-    const int n = build_tile_list(box, F, s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, s_list, s_warp_cnt, &s_bar, bar_phase);
-    if (n == 0) return;  // uniform
+    const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
+    float* gtex_img = TEXGRAD ? grad_tex + (size_t)(b / K.tex_div) * K.tex_bs : nullptr;
+    for (int wb = 0; wb < F; wb += FACE_WINDOW) {
+    const int n = build_tile_list(box + wb, min(F - wb, FACE_WINDOW), s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, s_list,
+                                  s_warp_cnt, &s_bar, bar_phase);
+    if (n == 0) continue;  // uniform
+    const float* rec_img = rec_all + ((size_t)b * F + wb) * REC_F;
 
     const int nchunk = (n + CHUNK - 1) / CHUNK;
     issue_chunk(rec_img, s_list, n, 0, s_rec);
     issue_chunk(rec_img, s_list, n, 1, s_rec);
 
-    // per-pixel inputs -> shared (row-major, PT*PT/CTA pixels per thread, coalesced rows)
+    // per-pixel inputs -> shared (row-major, PT*PT/CTA pixels per thread, coalesced rows); rewritten per window (the
+    // chunk loop's barriers order it against the previous window's readers)
     for (int pi = tid; pi < PT * PT; pi += CTA) {
         const int px = x0 + (pi % PT), py = y0 + (pi / PT);
         const size_t np = (size_t)S * S;
@@ -1202,8 +1245,6 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
         for (int k = 0; k < NV; ++k) s_pix[k][pi] = v[k];
     }
     const int ncol = min(PT, S - x0), nrow = min(PT, S - y0);  // live extent of the tile
-    const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
-    float* gtex_img = TEXGRAD ? grad_tex + (size_t)(b / K.tex_div) * K.tex_bs : nullptr;
 
     for (int c = 0; c < nchunk; ++c) {
         const int st = c % NSTAGE;
@@ -1282,7 +1323,7 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
                 const int cx0 = (int)(geo & 0xff), w = (int)((geo >> 8) & 0xff), ry0 = (int)(geo >> 16);
                 const uint32_t rcpw = s_rcpw[j];
                 const float* rc = chunk + j * REC_F;
-                const int f = (int)s_list[c * CHUNK + j];
+                const int f = wb + (int)s_list[c * CHUNK + j];
                 float acc[9];
 #pragma unroll
                 for (int k = 0; k < 9; ++k) acc[k] = 0.f;
@@ -1310,6 +1351,7 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
         }
         __syncthreads();  // everyone is done with stage st
         issue_chunk(rec_img, s_list, n, c + NSTAGE, s_rec);
+    }
     }
     cp_async_wait<0>();
     __syncthreads();  // shared memory reusable by the next tile of this CTA (list-driven launch)
@@ -1373,12 +1415,12 @@ using namespace umr;
 
 // k_raster_bwd2 instantiation for the call: texture-only (grad_faces == NULL) and warp-level texel pre-reduction variants
 // exist for the texture-gradient kernels only
-template <int RGBM, bool TG, int TS>
+template <int RGBM, bool TG, int TS, typename IdxT>
 static void launch_bwd2(dim3 grid, cudaStream_t stream, bool pre, const float* rec, const float* textures, const float* soft_colors,
                         const float* aggrs_info, const float* grad_images, float* grad_faces, float* grad_textures,
                         const Consts& K, const PairBuf& pb) {
 #define UMR_BWD2_GO(GEOMV, PREV) \
-    k_raster_bwd2<RGBM, TG, TS, 3, GEOMV, PREV><<<grid, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images, \
+    k_raster_bwd2<RGBM, TG, TS, 3, GEOMV, PREV, IdxT><<<grid, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images, \
                                                                                     grad_faces, grad_textures, K, pb)
     if constexpr (TG && RGBM == 1) {
         if (pre) { if (grad_faces) UMR_BWD2_GO(true, true); else UMR_BWD2_GO(false, true); }
@@ -1452,7 +1494,7 @@ static int check_params(const UmrRasterParams* p) {
     if (!p) return UMR_ERR_BAD_ARG;
     if (p->batch_size <= 0 || p->num_faces <= 0 || p->texture_size <= 0 || p->image_size <= 0)
         return UMR_ERR_BAD_ARG;
-    if (p->num_faces > 65535 || p->batch_size > 65535) return UMR_ERR_TOO_LARGE;
+    if (p->num_faces > UMR_RASTER_MAX_FACES || p->batch_size > 65535) return UMR_ERR_TOO_LARGE;
     if (p->func_id_dist < 0 || p->func_id_dist > 2 || p->func_id_alpha < 0 || p->func_id_alpha > 2 ||
         p->texture_sample_type < 0 || p->texture_sample_type > 1)
         return UMR_ERR_UNSUPPORTED;
@@ -1500,7 +1542,7 @@ static Consts make_consts(const UmrRasterParams* p) {
 }
 
 // Opt every raster kernel into the full dynamic shared-memory range ONCE per device (not per call:
-// the call may be inside a CUDA-graph capture).  F = 65535 needs 8 KB + 32 KB + 128 KB.
+// the call may be inside a CUDA-graph capture).  A 65536-face window needs 8 KB + 32 KB + 128 KB.
 static int ensure_smem_attrs() {
     static bool done[64] = {};
     int dev = 0;
@@ -1519,6 +1561,7 @@ static int ensure_smem_attrs() {
     if (e != cudaSuccess) return (int)e;
     UMR_SET((k_raster_fwd<0>)) UMR_SET((k_raster_fwd<1>))
     UMR_SET((k_raster_fwd4<0>)) UMR_SET((k_raster_fwd4<1>))
+    UMR_SET((k_raster_fwd4<0, uint32_t>)) UMR_SET((k_raster_fwd4<1, uint32_t>))
     UMR_SET((k_raster_bwd<0, false>)) UMR_SET((k_raster_bwd<0, true>))
     UMR_SET((k_raster_bwd<1, false>)) UMR_SET((k_raster_bwd<1, true>))
     UMR_SET((k_raster_bwd_pairs<0, false>)) UMR_SET((k_raster_bwd_pairs<0, true>))
@@ -1546,7 +1589,27 @@ static int sm_count(int* sms) {
     return 0;
 }
 
-static size_t raster_dyn_smem(int F) { return smem_list_off(F) + (((size_t)F * 2 + 15) & ~(size_t)15); }
+static size_t raster_dyn_smem(int F) {
+    const int W = F < FACE_WINDOW ? F : FACE_WINDOW;
+    return smem_list_off(F) + (((size_t)W * 2 + 15) & ~(size_t)15);
+}
+
+// Coarse binning for the UMR-configuration kernels: u16 lists of F entries per bin, or (F > 65535) the wide pool, whose
+// cursor is reset first.
+static int launch_bin_coarse(const float4* box, const uint32_t* ubox, void* clist, int* ccount, int B, int F, int S,
+                             const WorkspaceLayout& L, cudaStream_t stream) {
+    const int ncb = (S + CB - 1) / CB;
+    const size_t smem = (size_t)(F < BOX_PIECE ? F : BOX_PIECE) * 16;
+    if (F <= NARROW_MAX_FACES) {
+        k_bin_coarse<uint16_t><<<dim3(ncb, ncb, B), CTA, smem, stream>>>(box, ubox, (uint16_t*)clist, ccount, F, S);
+        return 0;
+    }
+    const size_t nbin = (size_t)B * ncb * ncb;
+    cudaError_t e = cudaMemsetAsync(ccount + 2 * nbin, 0, sizeof(unsigned long long), stream);
+    if (e != cudaSuccess) return (int)e;
+    k_bin_coarse<uint32_t><<<dim3(ncb, ncb, B), CTA, smem, stream>>>(box, ubox, (uint32_t*)clist, ccount, F, S, L.clist_cap);
+    return 0;
+}
 
 extern "C" int umr_raster_forward(const float* face_vertices, const float* textures, float* images,
                                   float* soft_colors, float* aggrs_info, float* p2f_info,
@@ -1569,8 +1632,9 @@ extern "C" int umr_raster_forward(const float* face_vertices, const float* textu
     float* p2f_acc = (float*)(ws + L.p2f_off);
     uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
     int* ccount = (int*)(ws + L.ccount_off);
-    uint16_t* clist = (uint16_t*)(ws + L.clist_off);
-    const int n = B * F;
+    void* clist = ws + L.clist_off;
+    const bool wide = F > NARROW_MAX_FACES;
+    const size_t n = (size_t)B * F;
     const float r = sqrtf(K.thr);  // kernel.cu:355 sqrt(threshold) in float
     {
         cudaError_t e0 = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
@@ -1581,7 +1645,7 @@ extern "C" int umr_raster_forward(const float* face_vertices, const float* textu
     const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
     const bool want_p2f = p2f_info != nullptr;
     if (want_p2f && softmax) {
-        cudaError_t e = cudaMemsetAsync(p2f_acc, 0, (size_t)n * 4 * sizeof(float), stream);
+        cudaError_t e = cudaMemsetAsync(p2f_acc, 0, n * 4 * sizeof(float), stream);
         if (e != cudaSuccess) return (int)e;
     }
     const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
@@ -1597,22 +1661,27 @@ extern "C" int umr_raster_forward(const float* face_vertices, const float* textu
             if (e != cudaSuccess) return (int)e;
         }
         count_launch(2);
-        k_bin_coarse<<<dim3(ncb, ncb, B), CTA, (size_t)(F < BOX_PIECE ? F : BOX_PIECE) * 16, stream>>>(box, ubox, clist, ccount, F, K.S);
+        rc = launch_bin_coarse(box, ubox, clist, ccount, B, F, K.S, L, stream);
+        if (rc) return rc;
         if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
         const bool nc4 = p->color_channels == 4;
         const int impl = nc4 ? 3 : forward_impl(p->tile_mode);
-#define UMR_FWD_ARGS rec, box, clist, ccount, textures, images, soft_colors, aggrs_info, pacc, ubox, K, p->eps, \
+#define UMR_FWD_ARGS(IDX) rec, box, (const IDX*)clist, ccount, textures, images, soft_colors, aggrs_info, pacc, ubox, K, p->eps, \
                      p->background_color[0], p->background_color[1], p->background_color[2], pb, ncb
-        if (nc4) {
-            k_raster_fwd3<1, 4><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS, p->background_extra);
-        } else if (impl == 3) {
-            if (softmax) k_raster_fwd3<1><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS);
-            else k_raster_fwd3<0><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS);
-        } else {
-            const dim3 grid32((K.S + T4 - 1) / T4, (K.S + T4 - 1) / T4, B);
-            if (softmax) k_raster_fwd4<1><<<grid32, CTA, fwd4_dyn_smem(F), stream>>>(UMR_FWD_ARGS);
-            else k_raster_fwd4<0><<<grid32, CTA, fwd4_dyn_smem(F), stream>>>(UMR_FWD_ARGS);
+#define UMR_FWD(IDX)                                                                                                        \
+        if (nc4) {                                                                                                          \
+            k_raster_fwd3<1, 4, IDX><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX), p->background_extra);                     \
+        } else if (impl == 3) {                                                                                             \
+            if (softmax) k_raster_fwd3<1, 3, IDX><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX));                             \
+            else k_raster_fwd3<0, 3, IDX><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX));                                     \
+        } else {                                                                                                            \
+            const dim3 grid32((K.S + T4 - 1) / T4, (K.S + T4 - 1) / T4, B);                                                 \
+            const size_t sm4 = fwd4_dyn_smem(F, sizeof(IDX));                                                               \
+            if (softmax) k_raster_fwd4<1, IDX><<<grid32, CTA, sm4, stream>>>(UMR_FWD_ARGS(IDX));                            \
+            else k_raster_fwd4<0, IDX><<<grid32, CTA, sm4, stream>>>(UMR_FWD_ARGS(IDX));                                    \
         }
+        if (wide) { UMR_FWD(uint32_t) } else { UMR_FWD(uint16_t) }
+#undef UMR_FWD
 #undef UMR_FWD_ARGS
         if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
     } else {
@@ -1629,9 +1698,9 @@ extern "C" int umr_raster_forward(const float* face_vertices, const float* textu
     if (want_p2f) {
         if (softmax) {
             count_launch();
-            k_p2f_finalize<<<(n + 255) / 256, 256, 0, stream>>>(p2f_acc, p2f_info, (size_t)n);
+            k_p2f_finalize<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p2f_acc, p2f_info, n);
         } else {  // hard mode never accumulates p2f (kernel.cu:417-431 is softmax-only) -> zeros
-            cudaError_t e = cudaMemsetAsync(p2f_info, 0, (size_t)n * 2 * sizeof(float), stream);
+            cudaError_t e = cudaMemsetAsync(p2f_info, 0, n * 2 * sizeof(float), stream);
             if (e != cudaSuccess) return (int)e;
         }
     }
@@ -1659,7 +1728,7 @@ extern "C" int umr_raster_visibility(const float* face_vertices, float* aggrs_in
     float4* box = (float4*)(ws + L.box_off);
     uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
     int* ccount = (int*)(ws + L.ccount_off);
-    uint16_t* clist = (uint16_t*)(ws + L.clist_off);
+    void* clist = ws + L.clist_off;
     cudaError_t e0 = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
     if (e0 != cudaSuccess) return (int)e0;
     if (visible_faces) {
@@ -1668,16 +1737,21 @@ extern "C" int umr_raster_visibility(const float* face_vertices, float* aggrs_in
     }
     k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr));
     const int ncb = (K.S + CB - 1) / CB;
-    k_bin_coarse<<<dim3(ncb, ncb, B), CTA, (size_t)(F < BOX_PIECE ? F : BOX_PIECE) * 16, stream>>>(box, ubox, clist, ccount, F, K.S);
+    rc = launch_bin_coarse(box, ubox, clist, ccount, B, F, K.S, L, stream);
+    if (rc) return rc;
     const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
     const PairBuf none{nullptr, nullptr, nullptr, nullptr, nullptr, 0u};
     if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-    if (visible_faces && !aggrs_info)   // only the visible-face bytes: face-parallel z-buffer per 64x64 bin
-        k_visible_faces<<<dim3(ncb, ncb, B), CTA, 0, stream>>>(rec, clist, ccount, visible_faces, K);
-    else
-        k_raster_fwd3<2><<<grid, CTA, 0, stream>>>(rec, box, clist, ccount, /*textures*/ nullptr, /*images*/ nullptr,
-                                                   /*colors_hi*/ nullptr, aggrs_info, /*p2f*/ nullptr, ubox, K, p->eps, 0.f, 0.f, 0.f,
-                                                   none, ncb, 0.f, visible_faces);
+#define UMR_VIS(IDX)                                                                                                          \
+    if (visible_faces && !aggrs_info)   /* only the visible-face bytes: face-parallel z-buffer per 64x64 bin */              \
+        k_visible_faces<IDX><<<dim3(ncb, ncb, B), CTA, 0, stream>>>(rec, (const IDX*)clist, ccount, visible_faces, K);       \
+    else                                                                                                                      \
+        k_raster_fwd3<2, 3, IDX><<<grid, CTA, 0, stream>>>(rec, box, (const IDX*)clist, ccount, /*textures*/ nullptr,        \
+                                                           /*images*/ nullptr, /*colors_hi*/ nullptr, aggrs_info,             \
+                                                           /*p2f*/ nullptr, ubox, K, p->eps, 0.f, 0.f, 0.f, none, ncb, 0.f,   \
+                                                           visible_faces);
+    if (F > NARROW_MAX_FACES) { UMR_VIS(uint32_t) } else { UMR_VIS(uint16_t) }
+#undef UMR_VIS
     if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
     count_launch(3);
     return (int)cudaGetLastError();
@@ -1704,7 +1778,8 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
     float* rec = (float*)(ws + L.rec_off);
     float4* box = (float4*)(ws + L.box_off);
     uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
-    const int n = B * F;
+    const size_t n = (size_t)B * F;
+    const bool wide = F > NARROW_MAX_FACES;
     const float r = sqrtf(K.thr);
     // the workspace is scratch (another render may have used it since forward): rebuild the records
     cudaError_t e = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
@@ -1718,13 +1793,13 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
                                                          (pb.cap > 0 && !grad_faces) ? pb.ctrl + 1 : nullptr);
     count_launch();
     if (grad_faces) {
-        e = cudaMemsetAsync(grad_faces, 0, (size_t)n * 9 * sizeof(float), stream);
+        e = cudaMemsetAsync(grad_faces, 0, n * 9 * sizeof(float), stream);
         if (e != cudaSuccess) return (int)e;
     } else if (gen) {
         return UMR_ERR_UNSUPPORTED;  // texture-only backward: streaming / pair kernels only
     }
     if (grad_textures) {
-        e = cudaMemsetAsync(grad_textures, 0, (size_t)(n / (p->shared_textures > 1 ? p->shared_textures : 1)) * p->texture_size * 3 * sizeof(float), stream);
+        e = cudaMemsetAsync(grad_textures, 0, (n / (p->shared_textures > 1 ? p->shared_textures : 1)) * p->texture_size * 3 * sizeof(float), stream);
         if (e != cudaSuccess) return (int)e;
     }
     const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
@@ -1738,12 +1813,18 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
         else {                                                                                                \
             if (pb.cap > 0) {                                                                                 \
                 count_launch();                                                                               \
-                if (forward_impl(p->tile_mode) == 4)                                                          \
-                    launch_bwd2<RGBM, TG, 32>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, grad_images, \
-                                              grad_faces, grad_textures, K, pb);                              \
+                if (forward_impl(p->tile_mode) == 4 && wide)                                                  \
+                    launch_bwd2<RGBM, TG, 32, uint32_t>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
+                                                        grad_images, grad_faces, grad_textures, K, pb);       \
+                else if (forward_impl(p->tile_mode) == 4)                                                     \
+                    launch_bwd2<RGBM, TG, 32, uint16_t>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
+                                                        grad_images, grad_faces, grad_textures, K, pb);       \
+                else if (wide)                                                                                \
+                    launch_bwd2<RGBM, TG, 16, uint32_t>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
+                                                        grad_images, grad_faces, grad_textures, K, pb);       \
                 else                                                                                          \
-                    launch_bwd2<RGBM, TG, 16>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, aggrs_info, grad_images, \
-                                              grad_faces, grad_textures, K, pb);                              \
+                    launch_bwd2<RGBM, TG, 16, uint16_t>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
+                                                        grad_images, grad_faces, grad_textures, K, pb);       \
             }                                                                                                 \
             if (pb.cap > 0)                                                                                   \
                 k_raster_bwd_pairs_list<RGBM, TG><<<list_grid, CTA, smem, stream>>>(                          \
@@ -1771,8 +1852,12 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
     if (nc4) {  // 16x16 tiles, softmax, no texture gradient (check_params / above)
         if (pb.cap > 0) {
             count_launch();
-            k_raster_bwd2<1, false, 16, 4><<<grid_pairs, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images, grad_faces,
-                                                                            grad_textures, K, pb);
+            if (wide)
+                k_raster_bwd2<1, false, 16, 4, true, false, uint32_t><<<grid_pairs, BWD2_THREADS, 0, stream>>>(
+                    rec, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, K, pb);
+            else
+                k_raster_bwd2<1, false, 16, 4><<<grid_pairs, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images, grad_faces,
+                                                                                grad_textures, K, pb);
             k_raster_bwd_pairs_list<1, false, 4><<<list_grid, CTA, smem, stream>>>(rec, box, textures, soft_colors, aggrs_info, grad_images,
                                                                                    grad_faces, grad_textures, ubox, K, pb.ctrl + 1,
                                                                                    pb.ulist, (int)grid_pairs.x, (int)grid_pairs.y);

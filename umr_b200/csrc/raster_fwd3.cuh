@@ -16,9 +16,10 @@ constexpr int FWD3_CTAS = 4;
 // (aggrs planes: depth_min, face_index_min) and nothing else: no distance / sigmoid / alpha / colour arithmetic, no image
 // planes.  That is all `MultiTextureLoss` keeps of its hard render (loss_utils.py:327-329: `_, p2f, aggr = hard_renderer(...)`,
 // and p2f is zero in hard mode, kernel.cu:417-431).  Same winner as RGB = 0, bit for bit.
-template <int RGB, int NC = 3>  // NC colour channels (3, or 4: the part-map render of SURVEY.md 8f-2); planes = NC + 1 (alpha)
+// IdxT: face-index width of the coarse lists, the tile list and the pair-block headers (uint16_t: F <= 65535)
+template <int RGB, int NC = 3, typename IdxT = uint16_t>  // NC colour channels (3, or 4: the part-map render of SURVEY.md 8f-2); planes = NC + 1 (alpha)
 __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __restrict__ rec_all, const float4* __restrict__ box_all,
-                                                        const uint16_t* __restrict__ clist, const int* __restrict__ ccount,
+                                                        const IdxT* __restrict__ clist, const int* __restrict__ ccount,
                                                         const float* __restrict__ textures, float* __restrict__ images,
                                                         float* __restrict__ colors_hi, float* __restrict__ aggrs,
                                                         float* __restrict__ p2f_acc, const uint32_t* __restrict__ ubox,
@@ -31,7 +32,7 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
     constexpr int WG = 16;                                           // list entries per warp group
     __shared__ __align__(128) float s_wrec[NWARP * 2 * WG * REC_F];  // 32 KB: warp-private record stages; reused by the store epilogue
     float* s_rec = s_wrec;
-    __shared__ uint16_t s_list[LCAP];
+    __shared__ IdxT s_list[LCAP];
     __shared__ uint8_t s_meet[LCAP];          // bit w: the face's cull rectangle meets warp w's 8x4 pixel block
     __shared__ uint32_t s_boff[LCAP + 1];     // exclusive prefix of popc(s_meet): first pair block of the face
     __shared__ float s_xp[TILE], s_yp[TILE], s_ext[4];
@@ -55,7 +56,9 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
 
     const size_t tile_id = ((size_t)b * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
     const size_t cidx = ((size_t)b * ncb + (ty0 / CB)) * ncb + (tx0 / CB);
-    const int nc = tile_outside_union(ubox, b, s_ext) ? 0 : __ldg(ccount + cidx);
+    const bool outside = tile_outside_union(ubox, b, s_ext);
+    const CoarseBin<IdxT> cb = outside ? CoarseBin<IdxT>{0, nullptr} : coarse_bin(clist, ccount, cidx, F);
+    const int nc = cb.n;
 
     if (nc == 0) {
         if (VIS) {
@@ -147,7 +150,6 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
     const bool live = px < S && py < S;
     const float xp = s_xp[lcol], yp = s_yp[lrow];
     const int ncol = min(TILE, S - tx0), nrow = min(TILE, S - ty0);
-    const uint16_t* cl = clist + cidx * F;
     const float4* box = box_all + (size_t)b * F;
     const float* rec_img = rec_all + (size_t)b * F * REC_F;
     const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
@@ -176,7 +178,7 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
         // ---- tile-list segment: ordered compaction of this window's coarse entries that touch the tile ------
         const int nwin = min(LCAP, nc - w0);
         uint32_t masks[LCAP / CTA];
-        uint16_t fids[LCAP / CTA];
+        IdxT fids[LCAP / CTA];
         uint8_t meets[LCAP / CTA];
         int cnt = 0;
 #pragma unroll
@@ -184,9 +186,9 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
             const int i = warp * (LCAP / NWARP) + r * 32 + lane;
             bool hit = false;
             uint32_t meet = 0;
-            uint16_t f = 0;
+            IdxT f = 0;
             if (i < nwin) {
-                f = __ldg(cl + w0 + i);
+                f = (IdxT)bin_face(cb, w0 + i);
                 const float4 bb = __ldg(box + f);
                 hit = !(ext0 > bb.y || ext1 < bb.x || ext2 > bb.w || ext3 < bb.z);
                 if (hit) {
@@ -408,7 +410,7 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
                         dst[0] = make_float4(fr.D, fr.sign * fr.dx, fr.sign * fr.dy, zsave);
                         dst[32] = make_float4(u0, u1, u2, __uint_as_float(meta));
                     }
-                    if (lane == 0) pb.blk_hdr[blk] = (uint32_t)s_list[jl] | ((uint32_t)__popc(m) << 16);
+                    if (lane == 0) pb.blk_hdr[blk] = (uint32_t)s_list[jl] | ((uint32_t)__popc(m) << hdr_shift<IdxT>());
                 }
                 if (RGB == 1 && p2f_acc != nullptr) {
                     // p2f: warp-shuffle reduction (replaces the 4 global atomics per (pixel, face) of kernel.cu:427-430)

@@ -20,11 +20,15 @@ constexpr int T4 = 32;            // tile side
 constexpr int FWD4_CAP = 1536;    // tile-list entries held in shared memory (10 bytes each)
 constexpr int WG4 = 16;           // list entries per warp group
 
-__host__ __device__ inline size_t fwd4_dyn_smem(int F) { return (size_t)(F < FWD4_CAP ? F : FWD4_CAP) * 10 + 16; }
+// bytes per list entry: block offset + meet mask + face index
+__host__ __device__ inline size_t fwd4_dyn_smem(int F, size_t idx_bytes = 2) {
+    return (size_t)(F < FWD4_CAP ? F : FWD4_CAP) * (8 + idx_bytes) + 16;
+}
 
-template <int RGB>
+// IdxT: face-index width of the coarse lists, the tile list and the pair-block headers (uint16_t: F <= 65535)
+template <int RGB, typename IdxT = uint16_t>
 __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict__ rec_all, const float4* __restrict__ box_all,
-                                                        const uint16_t* __restrict__ clist, const int* __restrict__ ccount,
+                                                        const IdxT* __restrict__ clist, const int* __restrict__ ccount,
                                                         const float* __restrict__ textures, float* __restrict__ images,
                                                         float* __restrict__ colors_hi, float* __restrict__ aggrs,
                                                         float* __restrict__ p2f_acc, const uint32_t* __restrict__ ubox,
@@ -35,7 +39,7 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
     const int LC = F < FWD4_CAP ? F : FWD4_CAP;                               // list capacity
     uint32_t* s_boff = reinterpret_cast<uint32_t*>(smem_dyn);                 // [LC + 1]
     uint32_t* s_meet = s_boff + (LC + 1);                                     // [LC]  bit q: rectangle meets pixel block q
-    uint16_t* s_list = reinterpret_cast<uint16_t*>(s_meet + LC);              // [LC]
+    IdxT* s_list = reinterpret_cast<IdxT*>(s_meet + LC);                      // [LC]
     __shared__ __align__(128) float s_wrec[NWARP * 2 * WG4 * REC_F];          // 32 KB: warp-private record stages
     __shared__ float s_xp[T4], s_yp[T4], s_ext[4];
     __shared__ int s_warp_cnt[NWARP];
@@ -57,7 +61,9 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
 
     const size_t tile_id = ((size_t)b * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
     const size_t cidx = ((size_t)b * ncb + (ty0 / CB)) * ncb + (tx0 / CB);
-    const int nc = tile_outside_union(ubox, b, s_ext) ? 0 : __ldg(ccount + cidx);
+    const bool outside = tile_outside_union(ubox, b, s_ext);
+    const CoarseBin<IdxT> cb = outside ? CoarseBin<IdxT>{0, nullptr} : coarse_bin(clist, ccount, cidx, F);
+    const int nc = cb.n;
 
     // the initial pixel state, finalised (kernel.cu:335-348, 443-475): what an untouched pixel stores
     const float ssum0 = expf(eps / K.gamma);
@@ -134,7 +140,6 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
     }
 
     const int ncol = min(T4, S - tx0), nrow = min(T4, S - ty0);
-    const uint16_t* cl = clist + cidx * F;
     const float4* box = box_all + (size_t)b * F;
     const float* rec_img = rec_all + (size_t)b * F * REC_F;
     const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
@@ -148,9 +153,9 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
             const int i = r0 + tid;
             bool hit = false;
             uint32_t meet = 0;
-            uint16_t f = 0;
+            IdxT f = 0;
             if (i < nwin) {
-                f = __ldg(cl + w0 + i);
+                f = (IdxT)bin_face(cb, w0 + i);
                 const float4 bb = __ldg(box + f);
                 hit = !(ext0 > bb.y || ext1 < bb.x || ext2 > bb.w || ext3 < bb.z);
                 if (hit) {
@@ -307,7 +312,7 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
                         dst[0] = make_float4(fr.D, fr.sign * fr.dx, fr.sign * fr.dy, zsave);
                         dst[32] = make_float4(u0, u1, u2, __uint_as_float(meta));
                     }
-                    if (lane == 0) pb.blk_hdr[blk] = (uint32_t)s_list[jl] | ((uint32_t)__popc(m) << 16);
+                    if (lane == 0) pb.blk_hdr[blk] = (uint32_t)s_list[jl] | ((uint32_t)__popc(m) << hdr_shift<IdxT>());
                 }
                 if (RGB == 1 && p2f_acc != nullptr) {
                     // p2f: warp-shuffle reduction (replaces the 4 global atomics per (pixel, face) of kernel.cu:427-430)

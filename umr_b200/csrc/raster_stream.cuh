@@ -33,7 +33,7 @@ struct PairBuf {
     uint32_t* ctrl;      // [0] block cursor (== blocks wanted, may exceed cap), [1] tiles left unsaved
     int32_t* tile_head;  // [B * tiles]: first segment (block index), TILE_EMPTY or TILE_UNSAVED
     int32_t* ulist;      // [B * tiles]: ids of the unsaved tiles (count = ctrl[1]), walked by the recompute fallback
-    uint32_t* blk_hdr;   // [cap]: per block  face | count << 16 ; per segment  [base] = #blocks, [base+1] = next
+    uint32_t* blk_hdr;   // [cap]: per block  face | count << hdr_shift (16 narrow, 24 wide) ; per segment  [base] = #blocks, [base+1] = next
     float4* recs;        // [cap][2][32]
     uint32_t cap;        // blocks
 };
@@ -62,10 +62,38 @@ inline size_t pair_capacity(int B, int S, size_t bytes) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// coarse binning: grid (ncb, ncb, B).  clist[(b, cy, cx)][F] u16, ccount[(b, cy, cx)]
+// coarse binning: grid (ncb, ncb, B).
+//   narrow (u16): clist[(b, cy, cx)][F], ccount[(b, cy, cx)] = list length
+//   wide (u32):   ccount[(b, cy, cx)] = {length, offset of the list in the clist pool}; each bin counts its faces, reserves
+//                 that many pool entries with one atomic on the pool cursor (ccount's tail) and fills them.  A bin that
+//                 does not fit gets offset BIN_ALL_FACES: its consumers walk all F faces, which their own cull tests
+//                 reduce to the same ascending list.
 // ---------------------------------------------------------------------------------------------
+template <typename IdxT>
+struct CoarseBin {
+    int n;           // entries
+    const IdxT* cl;  // nullptr (wide only): entry i is face i
+};
+template <typename IdxT>
+__device__ __forceinline__ CoarseBin<IdxT> coarse_bin(const IdxT* clist, const int* ccount, size_t cidx, int F) {
+    if constexpr (sizeof(IdxT) == 2) {
+        return {__ldg(ccount + cidx), clist + cidx * F};
+    } else {
+        const uint2 c = __ldg(reinterpret_cast<const uint2*>(ccount) + cidx);
+        if (c.y == BIN_ALL_FACES) return {F, nullptr};
+        return {(int)c.x, clist + c.y};
+    }
+}
+template <typename IdxT>
+__device__ __forceinline__ int bin_face(const CoarseBin<IdxT>& cb, int i) {
+    if constexpr (sizeof(IdxT) == 2) return __ldg(cb.cl + i);
+    else return cb.cl ? (int)__ldg(cb.cl + i) : i;
+}
+
+template <typename IdxT>
 __global__ void __launch_bounds__(CTA) k_bin_coarse(const float4* __restrict__ box_all, const uint32_t* __restrict__ ubox,
-                                                    uint16_t* __restrict__ clist, int* __restrict__ ccount, int F, int S) {
+                                                    IdxT* __restrict__ clist, int* __restrict__ ccount, int F, int S,
+                                                    size_t pool_cap = 0) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float4* s_box = reinterpret_cast<float4*>(smem_raw);
     __shared__ uint64_t s_bar;
@@ -81,10 +109,33 @@ __global__ void __launch_bounds__(CTA) k_bin_coarse(const float4* __restrict__ b
     const size_t cidx = ((size_t)b * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
     int n = 0;
     uint32_t bar_phase = 0;
-    if (!tile_outside_union(ubox, b, s_ext))
-        n = build_tile_list(box_all + (size_t)b * F, F, s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, clist + cidx * F,
-                            s_warp_cnt, &s_bar, bar_phase);
-    if (threadIdx.x == 0) ccount[cidx] = n;
+    const float4* box = box_all + (size_t)b * F;
+    if constexpr (sizeof(IdxT) == 2) {
+        if (!tile_outside_union(ubox, b, s_ext))
+            n = build_tile_list(box, F, s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, clist + cidx * F, s_warp_cnt, &s_bar,
+                                bar_phase);
+        if (threadIdx.x == 0) ccount[cidx] = n;
+    } else {
+        __shared__ uint32_t s_off;
+        if (!tile_outside_union(ubox, b, s_ext))
+            n = build_tile_list<IdxT>(box, F, s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, nullptr, s_warp_cnt, &s_bar,
+                                      bar_phase);
+        if (threadIdx.x == 0) {
+            const size_t nbin = (size_t)gridDim.x * gridDim.y * gridDim.z;
+            unsigned long long* cursor = reinterpret_cast<unsigned long long*>(ccount + 2 * nbin);
+            uint32_t off = 0;
+            if (n > 0) {
+                const unsigned long long base = atomicAdd(cursor, (unsigned long long)n);
+                off = base + (unsigned long long)n <= (unsigned long long)pool_cap ? (uint32_t)base : BIN_ALL_FACES;
+            }
+            s_off = off;
+            reinterpret_cast<uint2*>(ccount)[cidx] = make_uint2((uint32_t)n, off);
+        }
+        __syncthreads();
+        if (n > 0 && s_off != BIN_ALL_FACES)  // uniform: the second scan writes the list into the reserved entries
+            build_tile_list<IdxT>(box, F, s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, clist + s_off, s_warp_cnt, &s_bar,
+                                  bar_phase);
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -95,7 +146,8 @@ __global__ void __launch_bounds__(CTA) k_bin_coarse(const float4* __restrict__ b
 // nearest (lowest face index on ties, like the ascending strict-'<' walk).  No plane is written.  Work ~ sum of bounding
 // boxes instead of pixels x candidate faces of k_raster_fwd3<2>.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(CTA) k_visible_faces(const float* __restrict__ rec_all, const uint16_t* __restrict__ clist,
+template <typename IdxT>
+__global__ void __launch_bounds__(CTA) k_visible_faces(const float* __restrict__ rec_all, const IdxT* __restrict__ clist,
                                                        const int* __restrict__ ccount, uint8_t* __restrict__ vis, Consts K) {
     __shared__ unsigned long long s_z[CB * CB];   // 32 KB
     __shared__ float s_xp[CB], s_yp[CB];
@@ -105,7 +157,8 @@ __global__ void __launch_bounds__(CTA) k_visible_faces(const float* __restrict__
     const int x0 = blockIdx.x * CB, y0 = blockIdx.y * CB;
     const int ncol = min(CB, S - x0), nrow = min(CB, S - y0);
     const size_t cidx = ((size_t)b * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-    const int nc = __ldg(ccount + cidx);
+    const CoarseBin<IdxT> cb = coarse_bin(clist, ccount, cidx, F);
+    const int nc = cb.n;
     uint8_t* vb = vis + (size_t)b * F;
     if (nc == 0) {  // all background: face id -1, which the reference's indexing turns into face F-1 (see k_visible)
         if (tid == 0 && *reinterpret_cast<volatile uint8_t*>(vb + F - 1) == 0) vb[F - 1] = 1;
@@ -116,13 +169,12 @@ __global__ void __launch_bounds__(CTA) k_visible_faces(const float* __restrict__
     else if (tid < 2 * CB) s_yp[tid - CB] = pixel_coord(S - 1 - (y0 + tid - CB), S);
     if (tid == 0) { s_bg = 0; s_next = NWARP; }
     __syncthreads();
-    const uint16_t* cl = clist + cidx * F;
     const float* rec_img = rec_all + (size_t)b * F * REC_F;
     auto scan_face = [&](int i) {
-        const int f = __ldg(cl + i);
+        const int f = bin_face(cb, i);
         const float* rc = rec_img + (size_t)f * REC_F;
         if (lane == 0 && i + NWARP < nc)   // the warp's next face: pull its 128-byte record into L1 while this one is scanned
-            asm volatile("prefetch.global.L1 [%0];" ::"l"(rec_img + (size_t)__ldg(cl + i + NWARP) * REC_F));
+            asm volatile("prefetch.global.L1 [%0];" ::"l"(rec_img + (size_t)bin_face(cb, i + NWARP) * REC_F));
         const uint32_t flg = __float_as_uint(__ldg(rc + R_FLG));
         if (!(K.double_side || (flg & 8u))) return;   // back face of a single-sided render never wins (warp-uniform)
         // pixel rectangle to test: bounding box of the vertices widened by 2 pixels (an inside pixel lies in the box; the
@@ -221,7 +273,8 @@ constexpr int BWD2_THREADS = 256, BWD2_WARPS = BWD2_THREADS / 32;  // threads of
 // Pays only when a face covers hundreds of raster pixels per texel (raster.cu: TEXGRAD_PRE_RATIO_*); at UMR's shapes the
 // plain vector REDs are faster.
 // rec_all: the face records of k_prep (GEOM only): the z-gradient factors w_clip_k / z_k^2 are re-derived from them
-template <int RGB, bool TEXGRAD, int TS, int NC = 3, bool GEOM = true, bool PRE = false>  // NC colour channels; pixel planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
+// IdxT: face-index width of the block headers (hdr_shift)
+template <int RGB, bool TEXGRAD, int TS, int NC = 3, bool GEOM = true, bool PRE = false, typename IdxT = uint16_t>  // NC colour channels; pixel planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
 __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const float* __restrict__ rec_all, const float* __restrict__ textures,
                                                         const float* __restrict__ colors_hi,
                                                         const float* __restrict__ aggrs, const float* __restrict__ grad_images,
@@ -325,16 +378,18 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
                 const int rel = (int)(k - kwin);
                 const uint32_t h0 = __shfl_sync(0xffffffffu, hw, rel), h1 = __shfl_sync(0xffffffffu, hw, (rel + 1) & 31);
                 const uint32_t h2 = __shfl_sync(0xffffffffu, hw, (rel + 2) & 31), h3 = __shfl_sync(0xffffffffu, hw, (rel + 3) & 31);
-                const int a0 = (int)(h0 >> 16) - o;
+                constexpr int HS = hdr_shift<IdxT>();
+                constexpr uint32_t HM = (1u << HS) - 1u;
+                const int a0 = (int)(h0 >> HS) - o;
                 if (a0 <= 0) { ++k; o = 0; continue; }  // block exhausted / empty (warp-uniform)
-                const int f = (int)(h0 & 0xffffu);
+                const int f = (int)(h0 & HM);
                 // records available in the following blocks while they belong to the same face (an empty block is transparent)
                 int a1 = 0, a2 = 0, a3 = 0, nchain = 1;
-                if (k + 1 < wend && ((h1 >> 16) == 0 || (int)(h1 & 0xffffu) == f)) {
-                    a1 = (int)(h1 >> 16); nchain = 2;
-                    if (k + 2 < wend && ((h2 >> 16) == 0 || (int)(h2 & 0xffffu) == f)) {
-                        a2 = (int)(h2 >> 16); nchain = 3;
-                        if (k + 3 < wend && ((h3 >> 16) == 0 || (int)(h3 & 0xffffu) == f)) { a3 = (int)(h3 >> 16); nchain = 4; }
+                if (k + 1 < wend && ((h1 >> HS) == 0 || (int)(h1 & HM) == f)) {
+                    a1 = (int)(h1 >> HS); nchain = 2;
+                    if (k + 2 < wend && ((h2 >> HS) == 0 || (int)(h2 & HM) == f)) {
+                        a2 = (int)(h2 >> HS); nchain = 3;
+                        if (k + 3 < wend && ((h3 >> HS) == 0 || (int)(h3 & HM) == f)) { a3 = (int)(h3 >> HS); nchain = 4; }
                     }
                 }
                 const int p1 = a0, p2 = a0 + a1, p3 = p2 + a2, p4 = p3 + a3;
