@@ -155,6 +155,26 @@ int umr_raster_backward(const float* face_vertices, const float* textures, const
                         float* grad_textures, const UmrRasterParams* params, void* workspace,
                         void* stream);
 
+/* Deterministic mode (DESIGN.md §3).  Same arguments and outputs as umr_raster_forward / umr_raster_backward, but every
+ * output is bitwise identical for identical inputs on the same device type and library build, whatever the stream, host
+ * thread, concurrent work or CUDA-graph replay: p2f sums are exact fixed point (integer REDs), and the backward is a
+ * face-parallel gather in which every gradient element has exactly one writer.  The pair buffer and tile_mode are ignored
+ * (the 16x16-tile forward always runs, and the backward recomputes every pair).  No host synchronisation; constant launch
+ * count.  Every mode check_params accepts (all distance, alpha and texture modes, softmax or hard, 3 or 4 channels, shared
+ * textures, any F up to UMR_RASTER_MAX_FACES, grad_faces == NULL for a texture-only backward); a raster side S above
+ * 65535 * 16 returns UMR_ERR_TOO_LARGE.  A face covering most of the raster is walked by one warp (DESIGN.md §3).  The workspace must hold
+ * umr_raster_workspace_bytes_deterministic() bytes: umr_raster_workspace_bytes() plus 104 bytes per (image, face) for the
+ * fixed-point accumulators (rounded up to 256). */
+size_t umr_raster_workspace_bytes_deterministic(int32_t batch_size, int32_t num_faces, int32_t image_size,
+                                                int32_t anti_aliasing);
+int umr_raster_forward_deterministic(const float* face_vertices, const float* textures, float* images,
+                                     float* soft_colors, float* aggrs_info, float* p2f_info,
+                                     const UmrRasterParams* params, void* workspace, void* stream);
+int umr_raster_backward_deterministic(const float* face_vertices, const float* textures, const float* soft_colors,
+                                      const float* aggrs_info, const float* grad_images, float* grad_faces,
+                                      float* grad_textures, const UmrRasterParams* params, void* workspace,
+                                      void* stream);
+
 /* Fused vertex pipeline (SURVEY.md §8f-1): 7-dof orthographic camera projection with z
  * (nnutils/geom_utils.py:74-91,119-165), y flip (nnutils/smr.py:36), look_at with the eye on the z axis
  * + orthogonal scale (SoftRas/functional/look_at.py:48-60, orthogonal.py:13-16), the face gather

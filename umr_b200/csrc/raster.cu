@@ -364,6 +364,70 @@ struct Consts {
 };
 
 // ---------------------------------------------------------------------------------------------
+// Deterministic mode (umr_raster_*_deterministic, DESIGN.md §3): the forward adds its per-(warp, face) p2f partials as
+// exact fixed point.  A partial v (|v| <= 32: a warp sum of 32 pixel terms of magnitude <= 1) becomes the integer
+// round(|v| * 2^P2F_FRAC_BITS) < 2^102, split into P2F_LIMBS limbs of P2F_LIMB_BITS bits, each added into its own int64
+// word with an integer RED.  Integer addition is associative, so the words do not depend on the order of the REDs, and a
+// limb word holds at most (8x4 pixel blocks of the raster) * 2^26 < 2^63 for every raster the kernels can launch.
+// ---------------------------------------------------------------------------------------------
+constexpr int P2F_LIMBS = 4;
+constexpr int P2F_LIMB_BITS = 26;
+constexpr int P2F_FRAC_BITS = 96;
+constexpr int P2F_DET_WORDS = 3 * P2F_LIMBS + 1;  // x, y, w limbs, then a word set when a partial was not finite
+
+__device__ __forceinline__ void red_add_u64(unsigned long long* addr, unsigned long long v) {
+    asm volatile("red.global.add.u64 [%0], %1;" ::"l"(addr), "l"(v) : "memory");
+}
+
+__device__ __forceinline__ void red_fixed(unsigned long long* limbs, unsigned long long* bad, float v) {
+    const uint32_t u = __float_as_uint(v);
+    const int e = (int)((u >> 23) & 0xffu);
+    const int s = (e ? e : 1) - (150 - P2F_FRAC_BITS);  // |v| * 2^96 = m * 2^s
+    if (e == 0xff || s > P2F_LIMBS * P2F_LIMB_BITS - 24) {  // NaN / inf (|v| <= 32 otherwise)
+        atomicOr(bad, 1ull);
+        return;
+    }
+    const uint32_t m = (u & 0x7fffffu) | (e ? 0x800000u : 0u);
+    unsigned __int128 q;
+    if (s >= 0) q = (unsigned __int128)m << s;
+    else if (s > -32) q = ((unsigned long long)m + (1ull << (-s - 1))) >> (-s);  // round half away from zero
+    else return;
+    const bool neg = (u >> 31) != 0;
+#pragma unroll
+    for (int k = 0; k < P2F_LIMBS; ++k) {
+        const unsigned long long l = (unsigned long long)(q >> (k * P2F_LIMB_BITS)) & ((1ull << P2F_LIMB_BITS) - 1ull);
+        if (l != 0ull) red_add_u64(limbs + k, neg ? 0ull - l : l);
+    }
+}
+
+// one (warp, face) p2f partial into the face's P2F_DET_WORDS accumulator words
+__device__ __forceinline__ void red_p2f_fixed(unsigned long long* acc, float x, float y, float w) {
+    red_fixed(acc, acc + 3 * P2F_LIMBS, x);
+    red_fixed(acc + P2F_LIMBS, acc + 3 * P2F_LIMBS, y);
+    red_fixed(acc + 2 * P2F_LIMBS, acc + 3 * P2F_LIMBS, w);
+}
+
+// Texel-gradient sinks of bwd_pair_acc: the recompute backward adds a pair's texel gradient with REDs; the deterministic
+// gather takes it out (address and values) and combines the warp's lanes in a fixed order instead.
+struct TexRedSink {
+    __device__ __forceinline__ void add3(float* p, float a, float b, float c) const { red_add3_global(p, a, b, c); }
+    __device__ __forceinline__ void add(float* p, float v) const { red_add_global(p, v); }
+};
+// A pair adds to at most 9 consecutive floats (a surface texel's 3 channels, or a vertex texture's 3 corner colours) at
+// ascending addresses: *addr = the first, val[k] = the value for *addr + k.
+struct TexTakeSink {
+    float** addr;
+    float* val;
+    __device__ __forceinline__ void add3(float* p, float a, float b, float c) const {
+        *addr = p; val[0] = a; val[1] = b; val[2] = c;
+    }
+    __device__ __forceinline__ void add(float* p, float v) const {
+        if (*addr == nullptr) *addr = p;
+        val[p - *addr] = v;
+    }
+};
+
+// ---------------------------------------------------------------------------------------------
 // Modes UMR does not exercise (SURVEY.md §8f-3): hard / barycentric distance, hard / sum alpha, per-vertex
 // textures.  They run through the generic per-pixel kernels k_raster_fwd / k_raster_bwd, which read the mode
 // ids from Consts at run time; the UMR configuration (euclidean, prod, surface) has its own kernels.
@@ -405,20 +469,21 @@ __device__ __forceinline__ void sample_texture(const float* __restrict__ tx, flo
 
 // texture gradient of one pair: adds wgt * (g0,g1,g2) to the sampled texel (surface) or w_j * wgt * g to the
 // three corner colours (vertex), kernel.cu:597-601 / 610-616 with the intended texel semantics (App. B-1)
+template <class Sink = TexRedSink>
 __device__ __forceinline__ void add_texture_grad(float* __restrict__ gt, float c0, float c1, float c2, const Consts& K,
-                                                 float wgt, float g0, float g1, float g2, bool weighted) {
+                                                 float wgt, float g0, float g1, float g2, bool weighted, Sink sink = Sink()) {
     if (K.tex == UMR_TEX_SURFACE) {
         float* t = gt + (size_t)texel_index(c0, c1, K.R) * 3;
-        red_add_global(t + 0, weighted ? wgt * g0 : g0);
-        red_add_global(t + 1, weighted ? wgt * g1 : g1);
-        red_add_global(t + 2, weighted ? wgt * g2 : g2);
+        sink.add(t + 0, weighted ? wgt * g0 : g0);
+        sink.add(t + 1, weighted ? wgt * g1 : g1);
+        sink.add(t + 2, weighted ? wgt * g2 : g2);
     } else {
         const float w[3] = {c0, c1, c2};
 #pragma unroll
         for (int j = 0; j < 3; ++j) {
-            red_add_global(gt + 3 * j + 0, weighted ? wgt * (w[j] * g0) : w[j] * g0);
-            red_add_global(gt + 3 * j + 1, weighted ? wgt * (w[j] * g1) : w[j] * g1);
-            red_add_global(gt + 3 * j + 2, weighted ? wgt * (w[j] * g2) : w[j] * g2);
+            sink.add(gt + 3 * j + 0, weighted ? wgt * (w[j] * g0) : w[j] * g0);
+            sink.add(gt + 3 * j + 1, weighted ? wgt * (w[j] * g1) : w[j] * g1);
+            sink.add(gt + 3 * j + 2, weighted ? wgt * (w[j] * g2) : w[j] * g2);
         }
     }
 }
@@ -546,7 +611,8 @@ __device__ __forceinline__ void tile_extents(int S, float* s_ext, int tile = TIL
 // =============================================================================================
 // forward
 // =============================================================================================
-template <int RGB>  // RGB: 1 softmax, 0 hard; dist/alpha/texture modes read at run time
+// RGB: 1 softmax, 0 hard; dist/alpha/texture modes read at run time.  DET: fixed-point p2f (red_p2f_fixed).
+template <int RGB, bool DET = false>
 __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__ rec_all,
                                                        const float4* __restrict__ box_all,
                                                        const float* __restrict__ textures,
@@ -682,10 +748,15 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
             bb = bbn;
         }
         if (RGB == 1 && p2f_acc != nullptr && own_w != 0.f) {  // one global RED per (warp, face, component)
+            if constexpr (DET) {
+                red_p2f_fixed(reinterpret_cast<unsigned long long*>(p2f_acc) + ((size_t)b * F + wb + s_list[c * CHUNK + lane]) * P2F_DET_WORDS,
+                              own_x, own_y, own_w);
+            } else {
             float* dst = p2f_acc + ((size_t)b * F + wb + s_list[c * CHUNK + lane]) * 4;
             red_add_global(dst + 0, own_x);
             red_add_global(dst + 1, own_y);
             red_add_global(dst + 2, own_w);
+            }
         }
         __syncthreads();  // everyone is done with stage st
         issue_chunk(rec_img, s_list, n, c + NSTAGE, s_rec);  // commits an empty group past the end
@@ -801,6 +872,98 @@ __global__ void k_p2f_finalize(const float* __restrict__ acc, float* __restrict_
 // =============================================================================================
 // backward
 // =============================================================================================
+// One (pixel, face) pair of the generic-mode backward for the deterministic gather (k_raster_bwd_det<..., GEN>): the
+// per-pair body of k_raster_bwd (kernel.cu:577-654) statement for statement, with the texture gradient going to `sink`;
+// writes the 9 vertex gradients to gv (zeroed by the caller) and sets `contrib` for a pair inside the depth range.
+// k_raster_bwd keeps its inline copy: calling this function from it changes that kernel's SASS (its scheduling), and the
+// default kernels stay bit-for-bit what they were.  The GPU tests hold both to oracle B.
+// face_of() yields the face index (read where k_raster_bwd always read it: only for pairs inside the depth range).
+template <int RGB, bool TEXGRAD, class Sink = TexRedSink, class FaceOf>
+__device__ __forceinline__ void bwd_pair_generic(const float* __restrict__ rc, float xp, float yp, const Consts& K, FaceOf face_of,
+                                                 float g0, float g1, float g2, float g3, float C0, float C1, float C2,
+                                                 float C3, float ssum, float smax, const float* __restrict__ tex_img,
+                                                 float* __restrict__ gtex_img, float* gv, bool& contrib, Sink sink = Sink()) {
+    Frag fr;
+    if (fragment_any(rc, xp, yp, K, fr)) {
+        // alpha: kernel.cu:577-585 (hard alpha passes the raw gradient through, as the reference does)
+        const float one_m_a = 1 - C3;
+        float Cxy;
+        if (K.alpha == UMR_ALPHA_PROD) {
+            Cxy = (one_m_a == 0.f || g3 == 0.f)
+                      ? g3 * one_m_a
+                      : (float)((double)g3 * ((double)one_m_a / fmax((double)(1 - fr.D), 1e-6)));
+        } else if (K.alpha == UMR_ALPHA_SUM) {
+            Cxy = g3 / K.F;
+        } else {
+            Cxy = g3;
+        }
+        float k0 = fr.w0, k1 = fr.w1, k2 = fr.w2;
+        clip_bary(k0, k1, k2);
+        const float zp = depth_of(rc, k0, k1, k2);
+        if (!(zp < K.near_ || zp > K.far_)) {  // :592 drops the alpha gradient as well
+            contrib = true;
+            const uint32_t flg = __float_as_uint(rc[R_FLG]);
+            const bool front = (flg & 8u) != 0;
+            const int f = face_of();
+            float gz0 = 0.f, gz1 = 0.f, gz2 = 0.f;
+            if (RGB == 0) {
+                if ((float)f == smax) {  // aggrs[1] = winning face id (:596)
+                    if (TEXGRAD)
+                        add_texture_grad(gtex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, 1.f, g0, g1, g2, false, sink);
+                }
+            } else if ((front || K.double_side) && (g0 != 0.f || g1 != 0.f || g2 != 0.f)) {
+                const float zn = (K.far_ - zp) / (K.far_ - K.near_);
+                const float s = fr.D * expf((zn - smax) / K.gamma) / ssum;  // :608
+                if (s != 0.f) {
+                    if (TEXGRAD)
+                        add_texture_grad(gtex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, s, g0, g1, g2, true, sink);
+                    float t0, t1, t2;
+                    sample_texture(tex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, t0, t1, t2);
+                    float Crgb = 0.f;
+                    Crgb += g0 * (t0 - C0);
+                    Crgb += g1 * (t1 - C1);
+                    Crgb += g2 * (t2 - C2);
+                    Crgb *= s;
+                    if (Crgb != 0.f) {
+                        Cxy += Crgb / fr.D;
+                        const float Cz = Crgb / K.gamma / (K.near_ - K.far_) * zp * zp;  // :624
+                        gz0 = Cz * k0 / rc[2] / rc[2];
+                        gz1 = Cz * k1 / rc[5] / rc[5];
+                        gz2 = Cz * k2 / rc[8] / rc[8];
+                    }
+                }
+            }
+            Cxy *= fr.D * (1 - fr.D) / K.sigma;  // :632
+            gv[2] = gz0; gv[5] = gz1; gv[8] = gz2;
+            if (K.dist == UMR_DIST_EUCLIDEAN) {
+                const float q = 2 * fr.sign * Cxy;  // :640
+                gv[0] = q * (fr.t0 + fr.w0) * fr.dx;
+                gv[1] = q * (fr.t0 + fr.w0) * fr.dy;
+                gv[3] = q * (fr.t1 + fr.w1) * fr.dx;
+                gv[4] = q * (fr.t1 + fr.w1) * fr.dy;
+                gv[6] = q * (fr.t2 + fr.w2) * fr.dx;
+                gv[7] = q * (fr.t2 + fr.w2) * fr.dy;
+            } else if (K.dist == UMR_DIST_BARYCENTRIC) {  // kernel.cu:162-176
+                const float w0 = fr.t0, w1 = fr.t1, w2 = fr.t2;  // unclipped barycentrics
+                const int pidx = w0 > w1 ? (w1 > w2 ? 2 : 1) : (w0 > w2 ? 2 : 0);
+                const double scale = fr.dis > 0 ? (2. * (double)sqrtf(fr.dis)) : (2. * (double)sqrtf(-fr.dis));
+#pragma unroll
+                for (int l = 0; l < 2; ++l) {
+                    const float ip = rc[R_INV + 3 * pidx + l];
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        float gkl = 0.f;
+                        gkl += -ip * rc[R_INV + 3 * k + 0] * xp;
+                        gkl += -ip * rc[R_INV + 3 * k + 1] * yp;
+                        gkl += -ip * rc[R_INV + 3 * k + 2] * 1.f;
+                        gv[3 * k + l] = (float)((double)(gkl * Cxy) * scale);
+                    }
+                }
+            }
+        }
+    }
+}
+
 template <int RGB, bool TEXGRAD>
 __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__ rec_all,
                                                        const float4* __restrict__ box_all,
@@ -1097,10 +1260,10 @@ __device__ __forceinline__ bool bwd_pair(const float* __restrict__ rc, float xp,
 // Register-lean variant used by the pair-parallel kernel: the 10 per-pixel inputs stay in shared memory
 // (sp = &s_pix[0][pix], plane stride PT*PT) and are fetched where they are consumed, and the 9 gradients are
 // added straight into the caller's accumulators -- this keeps the kernel at <= 64 registers (4 CTAs/SM).
-template <int RGB, bool TEXGRAD, int NC = 3>
+template <int RGB, bool TEXGRAD, int NC = 3, class Sink = TexRedSink>
 __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float xp, float yp, const Consts& K,
                                              const float* __restrict__ sp, int f, const float* __restrict__ tex_img,
-                                             float* __restrict__ gtex_img, float* acc) {
+                                             float* __restrict__ gtex_img, float* acc, Sink sink = Sink()) {
     Frag fr;
     if (!fragment(rc, xp, yp, K.thr, K.sigma, fr)) return false;
     constexpr int NP = PT * PT, NPL = NC + 1, NV = 2 * NPL + 2;  // planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
@@ -1120,7 +1283,7 @@ __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float
             if (TEXGRAD) {
                 float* gt = gtex_img + ((size_t)f * K.T2 + texel_index(k0, k1, K.R)) * NC;
                 if (NC == 3) {
-                    red_add3_global(gt, sp[0], sp[NP], sp[2 * NP]);
+                    sink.add3(gt, sp[0], sp[NP], sp[2 * NP]);
                 } else {
 #pragma unroll
                     for (int c = 0; c < NC; ++c) red_add_global(gt + c, sp[c * NP]);
@@ -1139,7 +1302,7 @@ __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float
                 const size_t to = ((size_t)f * K.T2 + texel_index(k0, k1, K.R)) * NC;
                 if (TEXGRAD) {
                     if (NC == 3) {
-                        red_add3_global(gtex_img + to, s * g[0], s * g[1], s * g[2]);
+                        sink.add3(gtex_img + to, s * g[0], s * g[1], s * g[2]);
                     } else {
 #pragma unroll
                         for (int c = 0; c < NC; ++c) red_add_global(gtex_img + to + c, s * g[c]);
@@ -1402,6 +1565,159 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd_pairs_list(const float* _
     }
 }
 
+// =============================================================================================
+// deterministic mode (DESIGN.md §3)
+// =============================================================================================
+__device__ __forceinline__ double fixed_value(const unsigned long long* l) {
+    double v = 0.0;
+#pragma unroll
+    for (int k = P2F_LIMBS - 1; k >= 0; --k) v += ldexp((double)(long long)l[k], k * P2F_LIMB_BITS - P2F_FRAC_BITS);
+    return v;
+}
+
+// k_p2f_finalize over the fixed-point accumulators: the same clamp and divisions
+__global__ void k_p2f_finalize_det(const unsigned long long* __restrict__ acc, float* __restrict__ p2f, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned long long* a = acc + i * P2F_DET_WORDS;
+    if (a[3 * P2F_LIMBS] != 0ull) {
+        reinterpret_cast<float2*>(p2f)[i] = make_float2(__int_as_float(0x7fffffff), __int_as_float(0x7fffffff));
+        return;
+    }
+    const float x = (float)fixed_value(a), y = (float)fixed_value(a + P2F_LIMBS), w = (float)fixed_value(a + 2 * P2F_LIMBS);
+    const float d = fmaxf(w, 1e-12f);  // soft_rasterize.py:73 clamp_min(1e-12)
+    reinterpret_cast<float2*>(p2f)[i] = make_float2(x / d, y / d);
+}
+
+// Conservative index range [i0, i1] of the pixels whose centre coordinate pixel_coord(i, S) lies in [lo, hi] (monotone in i;
+// one index of slack on each side, the exact test runs per pixel).  NaN bounds keep every index, as the tile tests do.
+__device__ __forceinline__ void det_span(float lo, float hi, int S, int& i0, int& i1) {
+    const double a = ((double)lo * S + (S - 1)) * 0.5, c = ((double)hi * S + (S - 1)) * 0.5;
+    i0 = a > 0.0 ? (a < (double)S ? (int)a - 1 : S) : 0;
+    i1 = c < (double)(S - 1) ? (c >= 0.0 ? (int)c + 1 : -1) : S - 1;
+    i0 = max(i0, 0);
+    i1 = min(i1, S - 1);
+}
+
+// Face-parallel backward without atomics.  A (pixel, face) pair's gradient depends only on per-pixel constants and the face
+// record, so every output gets exactly one writer: one warp owns a (texture group, face) pair and walks the group's images in
+// ascending order and, in each, the face's cull box row by row (lanes across a row segment of 32 pixels), evaluating each pair
+// with bwd_pair_acc -- the recompute backward's arithmetic.  Vertex gradients: a fixed shuffle tree, one plain store per image.
+// Texel gradients: lanes that hit the same texel are summed in ascending lane order, and the lowest of them adds the sum into the
+// warp-owned texels of the face (plain load / store; __syncwarp orders the steps).  GEN: the generic modes (distance, alpha
+// and texture mode read at run time), evaluated with bwd_pair_generic -- k_raster_bwd's arithmetic; a vertex-texture pair adds
+// to the face's 9 corner colours, which the warp sums the same way.
+constexpr int DET_WARPS = CTA / 32;
+template <int RGB, bool TEXGRAD, int NC = 3, bool GEN = false>
+__global__ void __launch_bounds__(CTA) k_raster_bwd_det(const float* __restrict__ rec_all, const float* __restrict__ textures,
+                                                        const float* __restrict__ colors_hi, const float* __restrict__ aggrs,
+                                                        const float* __restrict__ grad_images, float* __restrict__ grad_faces,
+                                                        float* __restrict__ grad_tex, Consts K) {
+    constexpr int NPL = NC + 1, NV = 2 * NPL + 2, NP = PT * PT;
+    static_assert(NP == CTA, "bwd_pair_acc reads the per-pixel planes with stride PT * PT: one slot per thread");
+    __shared__ float s_pix[NV][NP];
+    __shared__ __align__(16) float s_rc[DET_WARPS][REC_F];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int f = blockIdx.x * DET_WARPS + warp;
+    if (f >= K.F) return;  // warp-uniform; the warps share no memory
+    const int grp = blockIdx.y, S = K.S, F = K.F;
+    const float* tex_img = textures + (size_t)grp * K.tex_bs;
+    float* gtex_img = TEXGRAD ? grad_tex + (size_t)grp * K.tex_bs : nullptr;
+    float* sp = &s_pix[0][threadIdx.x];
+    const float* rc = s_rc[warp];
+    const size_t np = (size_t)S * S;
+    for (int i = 0; i < K.tex_div; ++i) {
+        const int b = grp * K.tex_div + i;
+        __syncwarp();
+        s_rc[warp][lane] = __ldg(rec_all + ((size_t)b * F + f) * REC_F + lane);
+        __syncwarp();
+        const float4 bb = *reinterpret_cast<const float4*>(rc + R_BOX);
+        int c0, c1, j0, j1;
+        det_span(bb.x, bb.y, S, c0, c1);
+        det_span(bb.z, bb.w, S, j0, j1);  // j = S - 1 - row
+        float acc[9];
+#pragma unroll
+        for (int k = 0; k < 9; ++k) acc[k] = 0.f;
+        for (int py = S - 1 - j1; py <= S - 1 - j0; ++py) {
+            const float yp = pixel_coord(S - 1 - py, S);
+            if (yp > bb.w || yp < bb.z) continue;  // uniform
+            for (int x0 = c0; x0 <= c1; x0 += 32) {
+                const int px = x0 + lane;
+                const float xp = pixel_coord(px, S);
+                float* taddr = nullptr;
+                float tval[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+                if (px <= c1 && !(xp > bb.y || xp < bb.x)) {
+                    const size_t p = (size_t)py * S + px;
+                    if (K.aa) {  // avg_pool2d backward: g / 4
+                        const size_t nq = (size_t)K.IS * K.IS;
+                        const size_t q = (size_t)(py >> 1) * K.IS + (px >> 1);
+#pragma unroll
+                        for (int k = 0; k < NPL; ++k) sp[k * NP] = __ldg(grad_images + ((size_t)b * NPL + k) * nq + q) * 0.25f;
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < NPL; ++k) sp[k * NP] = __ldg(grad_images + ((size_t)b * NPL + k) * np + p);
+                    }
+#pragma unroll
+                    for (int k = 0; k < NPL; ++k) sp[(NPL + k) * NP] = __ldg(colors_hi + ((size_t)b * NPL + k) * np + p);
+                    sp[(NV - 2) * NP] = __ldg(aggrs + ((size_t)b * 2 + 0) * np + p);
+                    sp[(NV - 1) * NP] = __ldg(aggrs + ((size_t)b * 2 + 1) * np + p);
+                    if constexpr (GEN) {
+                        float gv[9];
+#pragma unroll
+                        for (int k = 0; k < 9; ++k) gv[k] = 0.f;
+                        bool hit = false;
+                        bwd_pair_generic<RGB, TEXGRAD, TexTakeSink>(rc, xp, yp, K, [=] { return f; }, sp[0], sp[NP], sp[2 * NP], sp[3 * NP],
+                                                                    sp[4 * NP], sp[5 * NP], sp[6 * NP], sp[7 * NP], sp[8 * NP],
+                                                                    sp[9 * NP], tex_img, gtex_img, gv, hit, TexTakeSink{&taddr, tval});
+                        if (hit) {
+#pragma unroll
+                            for (int k = 0; k < 9; ++k) acc[k] += gv[k];
+                        }
+                    } else {
+                        bwd_pair_acc<RGB, TEXGRAD, NC, TexTakeSink>(rc, xp, yp, K, sp, f, tex_img, gtex_img, acc,
+                                                                     TexTakeSink{&taddr, tval});
+                    }
+                }
+                if (TEXGRAD) {
+                    const bool has = taddr != nullptr;
+                    uint32_t rem = __ballot_sync(0xffffffffu, has);
+                    if (rem) {  // uniform
+                        const uint32_t peers = __match_any_sync(0xffffffffu, (unsigned long long)(uintptr_t)taddr);
+                        const bool vtx = GEN && K.tex != UMR_TEX_SURFACE;  // 9 corner-colour values instead of 3 texel channels
+                        float sum[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+                        while (rem) {  // ascending lane order
+                            const int o = __ffs(rem) - 1;
+                            rem &= rem - 1u;
+                            const bool mine = (peers >> o) & 1u;
+#pragma unroll
+                            for (int k = 0; k < 9; ++k) {
+                                if (k < 3 || vtx) {
+                                    const float v = __shfl_sync(0xffffffffu, tval[k], o);
+                                    if (mine) sum[k] += v;
+                                }
+                            }
+                        }
+                        if (has && lane == __ffs(peers) - 1) {
+#pragma unroll
+                            for (int k = 0; k < 9; ++k)
+                                if (k < 3 || vtx) taddr[k] = taddr[k] + sum[k];
+                        }
+                        __syncwarp();
+                    }
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < 9; ++k) acc[k] = warp_sum(acc[k]);
+        if (grad_faces != nullptr && lane < 9) {
+            float v = acc[0];
+#pragma unroll
+            for (int k = 1; k < 9; ++k) v = (lane == k) ? acc[k] : v;
+            grad_faces[((size_t)b * F + f) * 9 + lane] = v;
+        }
+    }
+}
+
 }  // namespace umr
 
 #include "raster_stream.cuh"
@@ -1559,7 +1875,7 @@ static int ensure_smem_attrs() {
     e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize,                         \
                              optin - (int)fa.sharedSizeBytes);                                       \
     if (e != cudaSuccess) return (int)e;
-    UMR_SET((k_raster_fwd<0>)) UMR_SET((k_raster_fwd<1>))
+    UMR_SET((k_raster_fwd<0>)) UMR_SET((k_raster_fwd<1>)) UMR_SET((k_raster_fwd<1, true>))
     UMR_SET((k_raster_fwd4<0>)) UMR_SET((k_raster_fwd4<1>))
     UMR_SET((k_raster_fwd4<0, uint32_t>)) UMR_SET((k_raster_fwd4<1, uint32_t>))
     UMR_SET((k_raster_bwd<0, false>)) UMR_SET((k_raster_bwd<0, true>))
@@ -1611,11 +1927,24 @@ static int launch_bin_coarse(const float4* box, const uint32_t* ubox, void* clis
     return 0;
 }
 
-extern "C" int umr_raster_forward(const float* face_vertices, const float* textures, float* images,
-                                  float* soft_colors, float* aggrs_info, float* p2f_info,
-                                  const UmrRasterParams* p, void* workspace, void* stream_) {
+// Deterministic-mode workspace: the default layout, then the fixed-point p2f accumulators (P2F_DET_WORDS int64 per face).
+static size_t det_acc_bytes(int B, int F) { return align256((size_t)B * F * P2F_DET_WORDS * sizeof(unsigned long long)); }
+// Rasters past the launch limit of the 16x16-tile grid (gridDim.y <= 65535) are refused; the p2f limb bound holds below it.
+constexpr int DET_MAX_RASTER = 65535 * TILE;
+
+extern "C" size_t umr_raster_workspace_bytes_deterministic(int32_t B, int32_t F, int32_t image_size, int32_t anti_aliasing) {
+    if (B <= 0 || F <= 0 || image_size <= 0) return 0;
+    return umr_raster_workspace_bytes(B, F, image_size, anti_aliasing) + det_acc_bytes(B, F);
+}
+
+// det: the deterministic mode (UMR's configuration only): 16x16-tile forward whatever tile_mode says, no pair buffer,
+// fixed-point p2f accumulators after the default workspace layout
+static int raster_forward(const float* face_vertices, const float* textures, float* images, float* soft_colors,
+                          float* aggrs_info, float* p2f_info, const UmrRasterParams* p, void* workspace, void* stream_,
+                          bool det) {
     int rc = check_params(p);
     if (rc) return rc;
+    if (det && (int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;
     if (!face_vertices || !textures || !images || !aggrs_info || !workspace) return UMR_ERR_BAD_ARG;
     if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -1644,8 +1973,10 @@ extern "C" int umr_raster_forward(const float* face_vertices, const float* textu
     count_launch();
     const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
     const bool want_p2f = p2f_info != nullptr;
+    if (det) p2f_acc = (float*)(ws + L.total);
     if (want_p2f && softmax) {
-        cudaError_t e = cudaMemsetAsync(p2f_acc, 0, n * 4 * sizeof(float), stream);
+        cudaError_t e = cudaMemsetAsync(p2f_acc, 0, det ? n * P2F_DET_WORDS * sizeof(unsigned long long) : n * 4 * sizeof(float),
+                                        stream);
         if (e != cudaSuccess) return (int)e;
     }
     const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
@@ -1655,7 +1986,7 @@ extern "C" int umr_raster_forward(const float* face_vertices, const float* textu
     if (!gen) {
         // round-2 pipeline: coarse bins -> tiled forward (saves pair records when a pair buffer is given)
         const int ncb = (K.S + CB - 1) / CB;
-        const PairBuf pb = make_pairbuf(p, K.S);
+        const PairBuf pb = det ? PairBuf{nullptr, nullptr, nullptr, nullptr, nullptr, 0u} : make_pairbuf(p, K.S);
         if (pb.cap > 0) {
             cudaError_t e = cudaMemsetAsync(pb.ctrl, 0, 16, stream);
             if (e != cudaSuccess) return (int)e;
@@ -1665,11 +1996,15 @@ extern "C" int umr_raster_forward(const float* face_vertices, const float* textu
         if (rc) return rc;
         if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
         const bool nc4 = p->color_channels == 4;
-        const int impl = nc4 ? 3 : forward_impl(p->tile_mode);
+        const int impl = (nc4 || det) ? 3 : forward_impl(p->tile_mode);
 #define UMR_FWD_ARGS(IDX) rec, box, (const IDX*)clist, ccount, textures, images, soft_colors, aggrs_info, pacc, ubox, K, p->eps, \
                      p->background_color[0], p->background_color[1], p->background_color[2], pb, ncb
 #define UMR_FWD(IDX)                                                                                                        \
-        if (nc4) {                                                                                                          \
+        if (det && nc4) {                                                                                                   \
+            k_raster_fwd3<1, 4, IDX, true><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX), p->background_extra);               \
+        } else if (det && softmax) {                                                                                        \
+            k_raster_fwd3<1, 3, IDX, true><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX));                                    \
+        } else if (nc4) {                                                                                                   \
             k_raster_fwd3<1, 4, IDX><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX), p->background_extra);                     \
         } else if (impl == 3) {                                                                                             \
             if (softmax) k_raster_fwd3<1, 3, IDX><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX));                             \
@@ -1688,7 +2023,10 @@ extern "C" int umr_raster_forward(const float* face_vertices, const float* textu
     if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
     count_launch();
 #define UMR_LAUNCH_FWD(RGBM)                                                                                 \
-    k_raster_fwd<RGBM><<<grid, CTA, smem, stream>>>(rec, box, textures, images, soft_colors, aggrs_info, pacc, ubox, \
+    if (det && RGBM == 1) k_raster_fwd<1, true><<<grid, CTA, smem, stream>>>(rec, box, textures, images, soft_colors,      \
+                                                    aggrs_info, pacc, ubox, K, p->eps, p->background_color[0],       \
+                                                    p->background_color[1], p->background_color[2]);                 \
+    else k_raster_fwd<RGBM><<<grid, CTA, smem, stream>>>(rec, box, textures, images, soft_colors, aggrs_info, pacc, ubox, \
                                                     K, p->eps, p->background_color[0], p->background_color[1],       \
                                                     p->background_color[2])
     if (softmax) UMR_LAUNCH_FWD(1); else UMR_LAUNCH_FWD(0);
@@ -1698,13 +2036,28 @@ extern "C" int umr_raster_forward(const float* face_vertices, const float* textu
     if (want_p2f) {
         if (softmax) {
             count_launch();
-            k_p2f_finalize<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p2f_acc, p2f_info, n);
+            if (det)
+                k_p2f_finalize_det<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>((const unsigned long long*)p2f_acc, p2f_info, n);
+            else
+                k_p2f_finalize<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p2f_acc, p2f_info, n);
         } else {  // hard mode never accumulates p2f (kernel.cu:417-431 is softmax-only) -> zeros
             cudaError_t e = cudaMemsetAsync(p2f_info, 0, n * 2 * sizeof(float), stream);
             if (e != cudaSuccess) return (int)e;
         }
     }
     return (int)cudaGetLastError();
+}
+
+extern "C" int umr_raster_forward(const float* face_vertices, const float* textures, float* images,
+                                  float* soft_colors, float* aggrs_info, float* p2f_info,
+                                  const UmrRasterParams* p, void* workspace, void* stream_) {
+    return raster_forward(face_vertices, textures, images, soft_colors, aggrs_info, p2f_info, p, workspace, stream_, false);
+}
+
+extern "C" int umr_raster_forward_deterministic(const float* face_vertices, const float* textures, float* images,
+                                                float* soft_colors, float* aggrs_info, float* p2f_info,
+                                                const UmrRasterParams* p, void* workspace, void* stream_) {
+    return raster_forward(face_vertices, textures, images, soft_colors, aggrs_info, p2f_info, p, workspace, stream_, true);
 }
 
 // Visibility only: the hard z-buffer's winner per raster pixel (see k_raster_fwd3<2>).  aggrs_info [B,2,S,S] =
@@ -1872,5 +2225,56 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
     }
 #undef UMR_LAUNCH_BWD
     if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+    return (int)cudaGetLastError();
+}
+
+// Deterministic backward: k_prep, then the face-parallel gather k_raster_bwd_det (no pair buffer, no atomics).  Same inputs
+// and outputs as umr_raster_backward; grad_faces == NULL (texture-only) is accepted.
+extern "C" int umr_raster_backward_deterministic(const float* face_vertices, const float* textures,
+                                                 const float* soft_colors, const float* aggrs_info,
+                                                 const float* grad_images, float* grad_faces, float* grad_textures,
+                                                 const UmrRasterParams* p, void* workspace, void* stream_) {
+    int rc = check_params(p);
+    if (rc) return rc;
+    if (!face_vertices || !textures || !soft_colors || !aggrs_info || !grad_images || !workspace) return UMR_ERR_BAD_ARG;
+    if (!grad_faces && !grad_textures) return UMR_ERR_BAD_ARG;
+    if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
+    if ((int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;
+    const bool gen = is_generic(p);
+    const bool nc4 = p->color_channels == 4;
+    if (nc4 && grad_textures) return UMR_ERR_UNSUPPORTED;  // part maps are constants (loss_utils.py:367-381)
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const int B = p->batch_size, F = p->num_faces;
+    const Consts K = make_consts(p);
+    const WorkspaceLayout L = ws_layout(B, F, K.S);
+    char* ws = (char*)workspace;
+    float* rec = (float*)(ws + L.rec_off);
+    float4* box = (float4*)(ws + L.box_off);
+    uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
+    const size_t n = (size_t)B * F;
+    cudaError_t e = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
+    if (e != cudaSuccess) return (int)e;
+    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr));
+    if (grad_textures) {
+        e = cudaMemsetAsync(grad_textures, 0, (n / K.tex_div) * p->texture_size * 3 * sizeof(float), stream);
+        if (e != cudaSuccess) return (int)e;
+    }
+    const dim3 grid((unsigned)((F + DET_WARPS - 1) / DET_WARPS), (unsigned)(B / K.tex_div));
+    const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
+    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
+#define UMR_BWD_DET(RGBM, TG, NCH)                                                                                        \
+    do {                                                                                                                    \
+        if (gen) k_raster_bwd_det<RGBM, TG, NCH, true><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info,     \
+                                                                               grad_images, grad_faces, grad_textures, K); \
+        else k_raster_bwd_det<RGBM, TG, NCH><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images,  \
+                                                                        grad_faces, grad_textures, K);                     \
+    } while (0)
+    if (nc4) k_raster_bwd_det<1, false, 4><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images,
+                                                                      grad_faces, grad_textures, K);
+    else if (softmax) { if (grad_textures) UMR_BWD_DET(1, true, 3); else UMR_BWD_DET(1, false, 3); }
+    else { if (grad_textures) UMR_BWD_DET(0, true, 3); else UMR_BWD_DET(0, false, 3); }
+#undef UMR_BWD_DET
+    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+    count_launch(2);
     return (int)cudaGetLastError();
 }

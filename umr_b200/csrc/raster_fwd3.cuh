@@ -17,7 +17,8 @@ constexpr int FWD3_CTAS = 4;
 // planes.  That is all `MultiTextureLoss` keeps of its hard render (loss_utils.py:327-329: `_, p2f, aggr = hard_renderer(...)`,
 // and p2f is zero in hard mode, kernel.cu:417-431).  Same winner as RGB = 0, bit for bit.
 // IdxT: face-index width of the coarse lists, the tile list and the pair-block headers (uint16_t: F <= 65535)
-template <int RGB, int NC = 3, typename IdxT = uint16_t>  // NC colour channels (3, or 4: the part-map render of SURVEY.md 8f-2); planes = NC + 1 (alpha)
+// DET: p2f partials go to the fixed-point accumulators of the deterministic mode (red_p2f_fixed) instead of float REDs
+template <int RGB, int NC = 3, typename IdxT = uint16_t, bool DET = false>  // NC colour channels (3, or 4: the part-map render of SURVEY.md 8f-2); planes = NC + 1 (alpha)
 __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __restrict__ rec_all, const float4* __restrict__ box_all,
                                                         const IdxT* __restrict__ clist, const int* __restrict__ ccount,
                                                         const float* __restrict__ textures, float* __restrict__ images,
@@ -423,8 +424,13 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
             if (RGB == 1 && p2f_acc != nullptr) {  // one global RED per (warp, face, component)
                 if (own_w != 0.f) {  // lane r owns the r-th staged face of the group
                     const int e = __fns(m_cur, 0, lane + 1);
+                    if constexpr (DET) {
+                        red_p2f_fixed(reinterpret_cast<unsigned long long*>(p2f_acc) + ((size_t)b * F + s_list[base + e]) * P2F_DET_WORDS,
+                                      own_x, own_y, own_w);
+                    } else {
                     float* dst = p2f_acc + ((size_t)b * F + s_list[base + e]) * 4;
                     red_add4_global(dst, own_x, own_y, own_w, 0.f);  // the accumulator slots are 16-byte aligned (ws_layout)
+                    }
                 }
             }
             __syncwarp();  // every lane is done with stage g & 1 before issue(g + 2) overwrites it

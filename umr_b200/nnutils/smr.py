@@ -53,6 +53,12 @@ class SoftRenderer(torch.nn.Module):
     fuse_vertex_pipeline = True  # class-level switch (tests compare both paths)
 
     def _fusable(self, vertices):
+        """True when forward() takes the fused vertex kernel.  Not under torch.use_deterministic_algorithms(True): its
+        backward scatters with float atomics, while the generic torch chain computes the same forward and differentiates
+        deterministically (its look_at matmul needs CUBLAS_WORKSPACE_CONFIG, README)."""
+        return self._projectable(vertices) and not torch.are_deterministic_algorithms_enabled()
+
+    def _projectable(self, vertices):
         """The fused vertex kernel covers exactly the configuration this wrapper sets up (smr.py:56-66):
         look_at camera with the eye on the z axis, orthographic, surface lighting with at most the one
         default directional light.  Anything else takes the generic torch path below."""
@@ -99,7 +105,7 @@ class SoftRenderer(torch.nn.Module):
         runs the visibility-only kernel (z-buffer winner per pixel; p2f_info is zero in hard mode, kernel.cu:417-431);
         every other configuration renders normally and drops the image."""
         r = self.renderer
-        if self._fusable(vertices) and r.rasterizer.supports_visibility():
+        if self._projectable(vertices) and r.rasterizer.supports_visibility():
             tr = r.transform.transformer
             fv, _ = project_faces(vertices.detach(), cams.detach(), faces, offset_z=self.offset_z, eye_z=float(tr._eye[2]),
                                   viewing_scale=tr.viewing_scale, flip_y=True, light=None)
@@ -113,7 +119,7 @@ class SoftRenderer(torch.nn.Module):
         (loss_utils.py:161-166), computed by the visibility kernel itself so that no plane is written or re-read.
         None when this renderer / device has no visibility kernel (callers then use `visibility` / `forward`)."""
         r = self.renderer
-        if not (self._fusable(vertices) and r.rasterizer.supports_visibility()):
+        if not (self._projectable(vertices) and r.rasterizer.supports_visibility()):
             return None
         tr = r.transform.transformer
         fv, _ = project_faces(vertices.detach(), cams.detach(), faces, offset_z=self.offset_z, eye_z=float(tr._eye[2]),

@@ -220,6 +220,10 @@ class SoftRasterizeFunction(torch.autograd.Function):
             if textures.requires_grad:
                 raise ValueError("4-channel (part-map) textures are constants: no texture gradient is built")
         need_bwd = face_vertices.requires_grad or textures.requires_grad
+        generic = dist_func != "euclidean" or aggr_func_alpha != "prod" or texture_type != "surface"
+        # torch.use_deterministic_algorithms(True): bitwise-reproducible kernels (include/umr_b200.h), read once here so the
+        # backward runs in the mode of its forward
+        det = torch.are_deterministic_algorithms_enabled()
         _attach_events(params, "fwd")
         with torch.cuda.device(dev):
             images = torch.empty(B, NC + 1, image_size, image_size, device=dev, dtype=torch.float32)
@@ -229,12 +233,11 @@ class SoftRasterizeFunction(torch.autograd.Function):
                 colors_hi = images
             aggrs = torch.empty(B, 2, S, S, device=dev, dtype=torch.float32)
             p2f = torch.empty(B, F, 2, device=dev, dtype=torch.float32)
-            ws = torch.empty(lib.umr_raster_workspace_bytes(B, F, int(image_size), params.anti_aliasing), device=dev,
-                             dtype=torch.uint8)
+            ws_bytes = lib.umr_raster_workspace_bytes_deterministic if det else lib.umr_raster_workspace_bytes
+            ws = torch.empty(ws_bytes(B, F, int(image_size), params.anti_aliasing), device=dev, dtype=torch.uint8)
             pairs = None
-            generic = dist_func != "euclidean" or aggr_func_alpha != "prod" or texture_type != "surface"
             pair_key = (S, F, FORWARD_TILE)
-            if need_bwd and not generic and PAIR_CAND_PER_PIXEL > 0:
+            if need_bwd and not generic and not det and PAIR_CAND_PER_PIXEL > 0:
                 capturing = torch.cuda.is_current_stream_capturing()
                 if PAIR_ADAPTIVE and not capturing:
                     _pair_poll()
@@ -242,11 +245,12 @@ class SoftRasterizeFunction(torch.autograd.Function):
                 pairs = torch.empty(pair_buffer_bytes(B, image_size, anti_aliasing, blocks_per_image=need, device=dev), device=dev,
                                     dtype=torch.uint8)
                 params.pair_buffer, params.pair_buffer_bytes = pairs.data_ptr(), pairs.numel()
-            rc = lib.umr_raster_forward(_ptr(fv), _ptr(tex), _ptr(images),
+            fwd = lib.umr_raster_forward_deterministic if det else lib.umr_raster_forward
+            rc = fwd(_ptr(fv), _ptr(tex), _ptr(images),
                                         _ptr(colors_hi) if anti_aliasing else _ptr(None),
                                         _ptr(aggrs), _ptr(p2f), ctypes.byref(params), _ptr(ws),
                                         _stream_ptr(dev))
-        _lib.check(rc, "umr_raster_forward")
+        _lib.check(rc, "umr_raster_forward_deterministic" if det else "umr_raster_forward")
         if pairs is not None:
             _pair_record(pair_key, B, pairs)
         params.ev_kernel_start = params.ev_kernel_stop = None
@@ -255,6 +259,7 @@ class SoftRasterizeFunction(torch.autograd.Function):
         ctx.tex_needs_grad = textures.requires_grad
         ctx.geom_needs_grad = face_vertices.requires_grad
         ctx.has_pairs = pairs is not None
+        ctx.det = det
         if need_bwd:
             if pairs is not None:
                 ctx.save_for_backward(fv, tex, colors_hi, aggrs, pairs)
@@ -277,15 +282,16 @@ class SoftRasterizeFunction(torch.autograd.Function):
         _attach_events(ctx.params, "bwd")
         with torch.cuda.device(dev):
             # detached geometry (UMR's texture branch, train_s2.py:248): texture-only backward, no vertex arithmetic
-            tex_only = ctx.tex_needs_grad and not ctx.geom_needs_grad and ctx.has_pairs
+            tex_only = ctx.tex_needs_grad and not ctx.geom_needs_grad and (ctx.has_pairs or ctx.det)
             grad_faces = None if tex_only else torch.empty_like(fv)
             grad_tex = torch.empty_like(tex) if ctx.tex_needs_grad else None
-            ws = torch.empty(lib.umr_raster_workspace_bytes(B, F, ctx.params.image_size, ctx.params.anti_aliasing),
-                             device=dev, dtype=torch.uint8)
-            rc = lib.umr_raster_backward(_ptr(fv), _ptr(tex), _ptr(colors_hi), _ptr(aggrs), _ptr(g),
+            ws_bytes = lib.umr_raster_workspace_bytes_deterministic if ctx.det else lib.umr_raster_workspace_bytes
+            ws = torch.empty(ws_bytes(B, F, ctx.params.image_size, ctx.params.anti_aliasing), device=dev, dtype=torch.uint8)
+            bwd = lib.umr_raster_backward_deterministic if ctx.det else lib.umr_raster_backward
+            rc = bwd(_ptr(fv), _ptr(tex), _ptr(colors_hi), _ptr(aggrs), _ptr(g),
                                          _ptr(grad_faces), _ptr(grad_tex), ctypes.byref(ctx.params),
                                          _ptr(ws), _stream_ptr(dev))
-        _lib.check(rc, "umr_raster_backward")
+        _lib.check(rc, "umr_raster_backward_deterministic" if ctx.det else "umr_raster_backward")
         ctx.params.ev_kernel_start = ctx.params.ev_kernel_stop = None
         return (None if grad_faces is None else grad_faces.view(ctx.in_shape), grad_tex) + (None,) * 14
 
