@@ -395,6 +395,62 @@ size_t umr_voxelize_workspace_bytes(int32_t B, int32_t vs);
 int umr_voxelize(const void* faces, int32_t dtype, int32_t* voxels, int32_t B, int32_t F, int32_t vs, double scale,
                  void* workspace, void* stream);
 
+/* Deterministic loss kernels (DESIGN.md §2), taken by the autograd Functions of umr_b200/ops.py under
+ * torch.use_deterministic_algorithms(True).  Each takes the arguments of its default symbol above, plus a caller-allocated
+ * device `workspace` of the size its *_workspace_bytes_deterministic query returns (a function of the sizes only; 0 for an
+ * empty size).  Outputs are the default symbol's, bitwise identical for identical inputs (values and memory layout) on
+ * the same device type and library build, whatever the stream, host thread, concurrent work or CUDA-graph replay.  No
+ * host synchronisation; the launch count depends on the arguments only.  No atomics reach an output:
+ *   - reductions (IoU, masked L1, loss head, TexCycle, Laplacian, flatten loss): every CTA of a grid sized from the
+ *     shapes stores its partial (the default kernel's in-CTA tree) into its own float slot, and a finalize kernel sums
+ *     each image's slots in ascending CTA order, in float, then applies the default finalize (+1e-6, 1 - I/U, scales,
+ *     loss-head weights).  The outputs the default call zero-fills or accumulates are fully written instead.
+ *   - umr_chamfer_backward_deterministic: a gather with one writer per gradient element (no workspace).  grad_a[i] is
+ *     its own idx_ab term plus the idx_ba terms of every j with idx_ba[j] == i; likewise grad_b.
+ *   - umr_flatten_backward_deterministic: per-edge vertex terms go to the workspace [B,E,4,3], then a per-vertex gather
+ *     sums them over the transposed incidence table: vert_rowptr [V+1], vert_incidence [4E] = edge * 4 + role
+ *     (role 0..3 = v0..v3 of the edge row) in ascending order per vertex.
+ *   - umr_corr_chamfer_backward_deterministic: per-(render, j) vertex terms go to the workspace [B,NS,3], then a
+ *     per-(render, vertex) gather sums them over the transposed selection table: vert_rowptr [V+1], vert_selection [NS]
+ *     = the j with selection[j] == v in ascending order per vertex.  grad_cams is the default kernel's.  The workspace
+ *     and tables may be NULL when grad_vertices is. */
+size_t umr_iou_workspace_bytes_deterministic(int32_t B, int64_t N);                 /* 8 * B * ceil(N / 16384) */
+int umr_iou_forward_deterministic(const float* predict, int64_t predict_bstride, const float* target, float* inter,
+                                  float* uni, float* loss, int32_t B, int64_t N, void* workspace, void* stream);
+size_t umr_masked_l1_workspace_bytes_deterministic(int32_t B, int64_t HW);          /* 4 * B * ceil(HW / 2048) */
+int umr_masked_l1_forward_deterministic(const float* pred, int64_t pred_bstride, const float* mask_pred,
+                                        int64_t mask_pred_bstride, const float* gt, const float* mask_gt, float* loss,
+                                        int32_t B, int32_t C, int64_t HW, void* workspace, void* stream);
+size_t umr_loss_head_workspace_bytes_deterministic(int32_t B, int64_t HW);          /* 12 * B * ceil(HW / 2048) */
+int umr_loss_head_forward_deterministic(const float* rgba, const float* gt, const float* mask_gt, float* stats,
+                                        float* per_image, float* loss, int32_t B, int64_t HW, float w_iou, float w_tex,
+                                        void* workspace, void* stream);
+size_t umr_texcycle_workspace_bytes_deterministic(int32_t B, int32_t F);            /* 4 * ceil(B * F / 256) */
+int umr_texcycle_forward_deterministic(const float* flow, const float* prob, const float* face_ids, uint8_t* visible,
+                                       float* loss, int32_t B, int32_t F, int32_t T2, int64_t P, void* workspace,
+                                       void* stream);
+size_t umr_laplacian_workspace_bytes_deterministic(int32_t B, int32_t V);           /* 4 * B * ceil(V / 256) */
+int umr_laplacian_forward_deterministic(const float* x, const int32_t* rowptr, const int32_t* col, const float* coef,
+                                        float* y, float* loss, int32_t B, int32_t V, void* workspace, void* stream);
+size_t umr_flatten_forward_workspace_bytes_deterministic(int32_t B, int32_t E);     /* 4 * B * ceil(E / 128) */
+int umr_flatten_forward_deterministic(const float* vertices, const int32_t* edges, float* loss, int32_t B, int32_t V,
+                                      int32_t E, float eps, void* workspace, void* stream);
+size_t umr_flatten_backward_workspace_bytes_deterministic(int32_t B, int32_t E);    /* 48 * B * E */
+int umr_flatten_backward_deterministic(const float* vertices, const int32_t* edges, const int32_t* vert_rowptr,
+                                       const int32_t* vert_incidence, const float* grad_loss, float* grad_vertices,
+                                       int32_t B, int32_t V, int32_t E, float eps, void* workspace, void* stream);
+int umr_chamfer_backward_deterministic(const float* a, const float* b, const int32_t* idx_ab, const int32_t* idx_ba,
+                                       const float* grad_dist_ab, const float* grad_dist_ba, float* grad_a, float* grad_b,
+                                       int32_t B, int32_t N, int32_t M, int32_t D, void* stream);
+size_t umr_corr_chamfer_workspace_bytes_deterministic(int32_t B, int32_t NS);       /* 12 * B * NS */
+int umr_corr_chamfer_backward_deterministic(const float* vertices, int64_t vertices_batch_stride, const float* cams,
+                                            const int32_t* selection, const float* const* targets,
+                                            const int32_t* target_counts, const int32_t* part_ends, const float* weights,
+                                            const float* vert2d, const int32_t* nearest, const float* grad_loss,
+                                            const float* grad_vert2d, float* grad_vertices, float* grad_cams, int32_t B,
+                                            int32_t NS, int32_t V, const int32_t* vert_rowptr,
+                                            const int32_t* vert_selection, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

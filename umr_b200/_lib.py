@@ -120,6 +120,36 @@ EXPORTS = {
     "umr_voxelize_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 2),
     "umr_voxelize": (ctypes.c_int, [c_f32p, ctypes.c_int32, c_f32p] + [ctypes.c_int32] * 3 + [ctypes.c_double, ctypes.c_void_p,
                                                                                            ctypes.c_void_p]),
+    # deterministic loss kernels: the default symbol's arguments + a workspace (+ the transposed tables of flatten / corr)
+    "umr_iou_workspace_bytes_deterministic": (ctypes.c_size_t, [ctypes.c_int32, ctypes.c_int64]),
+    "umr_iou_forward_deterministic": (ctypes.c_int, [c_f32p, ctypes.c_int64] + [c_f32p] * 4 + [ctypes.c_int32, ctypes.c_int64,
+                                                                                                ctypes.c_void_p, ctypes.c_void_p]),
+    "umr_masked_l1_workspace_bytes_deterministic": (ctypes.c_size_t, [ctypes.c_int32, ctypes.c_int64]),
+    "umr_masked_l1_forward_deterministic": (ctypes.c_int, [c_f32p, ctypes.c_int64, c_f32p, ctypes.c_int64, c_f32p, c_f32p, c_f32p,
+                                                           ctypes.c_int32, ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p,
+                                                           ctypes.c_void_p]),
+    "umr_loss_head_workspace_bytes_deterministic": (ctypes.c_size_t, [ctypes.c_int32, ctypes.c_int64]),
+    "umr_loss_head_forward_deterministic": (ctypes.c_int, [c_f32p] * 6 + [ctypes.c_int32, ctypes.c_int64, ctypes.c_float,
+                                                                   ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]),
+    "umr_texcycle_workspace_bytes_deterministic": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_texcycle_forward_deterministic": (ctypes.c_int, [c_f32p] * 5 + [ctypes.c_int32] * 3 + [ctypes.c_int64, ctypes.c_void_p,
+                                                                                              ctypes.c_void_p]),
+    "umr_laplacian_workspace_bytes_deterministic": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_laplacian_forward_deterministic": (ctypes.c_int, [c_f32p] * 6 + [ctypes.c_int32] * 2 + [ctypes.c_void_p, ctypes.c_void_p]),
+    "umr_flatten_forward_workspace_bytes_deterministic": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_flatten_forward_deterministic": (ctypes.c_int, [c_f32p] * 3 + [ctypes.c_int32] * 3 + [ctypes.c_float, ctypes.c_void_p,
+                                                                                             ctypes.c_void_p]),
+    "umr_flatten_backward_workspace_bytes_deterministic": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_flatten_backward_deterministic": (ctypes.c_int, [c_f32p] * 6 + [ctypes.c_int32] * 3 + [ctypes.c_float, ctypes.c_void_p,
+                                                                                              ctypes.c_void_p]),
+    "umr_chamfer_backward_deterministic": (ctypes.c_int, [c_f32p] * 8 + [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
+    "umr_corr_chamfer_workspace_bytes_deterministic": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_corr_chamfer_backward_deterministic": (ctypes.c_int, [c_f32p, ctypes.c_int64, c_f32p, ctypes.c_void_p,
+                                                               ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_int32),
+                                                               ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_float),
+                                                               c_f32p, ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p,
+                                                               ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p,
+                                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
 _lock = threading.Lock()

@@ -90,6 +90,13 @@ __device__ __forceinline__ float warp_sum(float v) {
     v += __shfl_xor_sync(0xffffffffu, v, 1);
     return v;
 }
+// p[0] + p[1] + ... + p[n-1], left to right in float: the fixed order of the deterministic reductions' finalize kernels,
+// which sum per-CTA partials stored in workspace slots instead of adding them with atomics
+__device__ __forceinline__ float sum_ascending(const float* p, int n) {
+    float t = 0.f;
+    for (int k = 0; k < n; ++k) t += p[k];
+    return t;
+}
 __device__ __forceinline__ float warp_max(float v) {
     v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 16));
     v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 8));

@@ -7,6 +7,9 @@
 //   nnutils/loss_utils.py:41-48 `neg_iou_loss`
 //   nnutils/chamfer_python.py:43-64 `distChamfer`
 //   nnutils/loss_utils.py:152-182 `TexCycle.forward`
+//
+// The reductions and the chamfer backward also have deterministic variants (DET template parameter / gather kernels,
+// `*_deterministic` entry points at the end of this file; DESIGN.md §2): no atomics reach their outputs.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -96,6 +99,8 @@ __global__ void __launch_bounds__(256) k_sample_bwd(const float* __restrict__ im
 constexpr int IOU_THREADS = 512;
 constexpr int IOU_PER_CTA = IOU_THREADS * 4 * 8;  // elements per CTA
 
+// DET: `inter` / `uni` are the workspace slots [B][gridDim.x]; the CTA stores its partial instead of adding it
+template <bool DET>
 __global__ void __launch_bounds__(IOU_THREADS) k_iou_partial(const float* __restrict__ p, const float* __restrict__ t,
                                                              float* __restrict__ inter, float* __restrict__ uni,
                                                              int64_t N, int64_t p_bstride) {
@@ -130,8 +135,26 @@ __global__ void __launch_bounds__(IOU_THREADS) k_iou_partial(const float* __rest
         si = lane < IOU_THREADS / 32 ? s_i[lane] : 0.f;
         su = lane < IOU_THREADS / 32 ? s_u[lane] : 0.f;
         si = warp_sum(si); su = warp_sum(su);
-        if (lane == 0) { atomicAdd(inter + b, si); atomicAdd(uni + b, su); }
+        if (DET) {
+            if (lane == 0) {
+                const size_t slot = (size_t)b * gridDim.x + blockIdx.x;
+                inter[slot] = si; uni[slot] = su;
+            }
+        } else {
+            if (lane == 0) { atomicAdd(inter + b, si); atomicAdd(uni + b, su); }
+        }
     }
+}
+// deterministic finalize: image b's slots summed in ascending CTA order, then k_iou_finalize's arithmetic
+__global__ void k_iou_finalize_det(const float* __restrict__ si, const float* __restrict__ su, float* __restrict__ inter,
+                                   float* __restrict__ uni, float* __restrict__ loss, int B, int nslot) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const float I = sum_ascending(si + (size_t)b * nslot, nslot);
+    const float u = sum_ascending(su + (size_t)b * nslot, nslot) + 1e-6f;
+    inter[b] = I;
+    uni[b] = u;
+    loss[b] = 1.f - I / u;
 }
 __global__ void k_iou_finalize(const float* __restrict__ inter, float* __restrict__ uni, float* __restrict__ loss, int B) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -219,6 +242,54 @@ __global__ void __launch_bounds__(256) k_chamfer_bwd(const float* __restrict__ q
     }
 }
 
+// Deterministic backward as a gather, one warp per output point i of `q` (no atomics, no workspace):
+//   gq[i] = own term (gd_q[i], idx_q[i]) + sum over j with idx_k[j] == i of the j terms (gd_k[j])
+// with k_chamfer_bwd's per-term arithmetic.  Lane l owns the j = l (mod 32) in ascending order; the ballot skips the
+// 32-wide chunks with no match; the lanes' sums meet in warp_sum's fixed tree.  gd_q / gd_k may be NULL (no term).
+template <int D>
+__global__ void __launch_bounds__(256) k_chamfer_bwd_gather(const float* __restrict__ q, const float* __restrict__ k,
+                                                            const int32_t* __restrict__ idx_q, const int32_t* __restrict__ idx_k,
+                                                            const float* __restrict__ gd_q, const float* __restrict__ gd_k,
+                                                            float* __restrict__ gq, int NQ, int NK) {
+    const int lane = threadIdx.x & 31;
+    const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int b = blockIdx.y;
+    if (i >= NQ) return;
+    float qv[D], acc[D];
+#pragma unroll
+    for (int d = 0; d < D; ++d) { qv[d] = __ldg(q + ((size_t)b * NQ + i) * D + d); acc[d] = 0.f; }
+    if (gd_k != nullptr) {
+        const int32_t* ik = idx_k + (size_t)b * NK;
+        for (int j0 = 0; j0 < NK; j0 += 32) {
+            const int j = j0 + lane;
+            const bool hit = j < NK && __ldg(ik + j) == i;
+            if (__ballot_sync(0xffffffffu, hit) == 0u) continue;
+            if (hit) {
+                const float g = __ldg(gd_k + (size_t)b * NK + j);
+#pragma unroll
+                for (int d = 0; d < D; ++d) {
+                    const float diff = __ldg(k + ((size_t)b * NK + j) * D + d) - qv[d];
+                    acc[d] += -2.f * g * diff;
+                }
+            }
+        }
+#pragma unroll
+        for (int d = 0; d < D; ++d) acc[d] = warp_sum(acc[d]);
+    }
+    if (lane != 0) return;
+    float own[D];
+#pragma unroll
+    for (int d = 0; d < D; ++d) own[d] = 0.f;
+    if (gd_q != nullptr) {
+        const float g = __ldg(gd_q + (size_t)b * NQ + i);
+        const int j = __ldg(idx_q + (size_t)b * NQ + i);
+#pragma unroll
+        for (int d = 0; d < D; ++d) own[d] = 2.f * g * (qv[d] - __ldg(k + ((size_t)b * NK + j) * D + d));
+    }
+#pragma unroll
+    for (int d = 0; d < D; ++d) gq[((size_t)b * NQ + i) * D + d] = own[d] + acc[d];
+}
+
 // ---------------------------------------------------------------------------------------------
 // texture cycle
 // ---------------------------------------------------------------------------------------------
@@ -250,6 +321,8 @@ __global__ void __launch_bounds__(256) k_visible(const float* __restrict__ ids, 
             mark(__ldg(src + i));
     }
 }
+// DET: `loss` is the workspace slot array [gridDim.x]; every CTA stores its scaled partial
+template <bool DET>
 __global__ void __launch_bounds__(256) k_texcycle_fwd(const float2* __restrict__ flow, const float2* __restrict__ prob,
                                                       const uint8_t* __restrict__ vis, float* __restrict__ loss, int n,
                                                       int T2, float scale) {
@@ -273,8 +346,17 @@ __global__ void __launch_bounds__(256) k_texcycle_fwd(const float2* __restrict__
     if (warp == 0) {
         acc = lane < 8 ? s[lane] : 0.f;
         acc = warp_sum(acc);
-        if (lane == 0 && acc != 0.f) atomicAdd(loss, acc * scale);
+        if (DET) {
+            if (lane == 0) loss[blockIdx.x] = acc * scale;
+        } else {
+            if (lane == 0 && acc != 0.f) atomicAdd(loss, acc * scale);
+        }
     }
+}
+// deterministic finalize of a per-row reduction: out[r] = the row's n slots summed in ascending order
+__global__ void k_sum_slot_rows(const float* __restrict__ slots, float* __restrict__ out, int rows, int n) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < rows) out[r] = sum_ascending(slots + (size_t)r * n, n);
 }
 __global__ void __launch_bounds__(256) k_texcycle_bwd(const float2* __restrict__ flow, const float2* __restrict__ prob,
                                                       const uint8_t* __restrict__ vis, const float* __restrict__ gl,
@@ -305,7 +387,8 @@ __global__ void __launch_bounds__(256) k_texcycle_bwd(const float2* __restrict__
 constexpr int ML1_THREADS = 256;
 constexpr int ML1_PER_CTA = ML1_THREADS * 8;  // pixels per CTA
 
-template <int C>
+// DET: `loss` is the workspace slot array [B][gridDim.x]; every CTA stores its scaled partial
+template <int C, bool DET>
 __global__ void __launch_bounds__(ML1_THREADS) k_masked_l1_fwd(const float* __restrict__ pred, int64_t pred_bs,
                                                               const float* __restrict__ mpred, int64_t mpred_bs,
                                                               const float* __restrict__ gt, const float* __restrict__ mgt,
@@ -331,7 +414,11 @@ __global__ void __launch_bounds__(ML1_THREADS) k_masked_l1_fwd(const float* __re
     if (warp == 0) {
         acc = lane < ML1_THREADS / 32 ? s[lane] : 0.f;
         acc = warp_sum(acc);
-        if (lane == 0) atomicAdd(loss + b, acc * inv_n);
+        if (DET) {
+            if (lane == 0) loss[(size_t)b * gridDim.x + blockIdx.x] = acc * inv_n;
+        } else {
+            if (lane == 0) atomicAdd(loss + b, acc * inv_n);
+        }
     }
 }
 
@@ -372,6 +459,8 @@ constexpr int LH_THREADS = 256;
 constexpr int LH_PER_CTA = LH_THREADS * 8;  // pixels per CTA
 
 // acc [B][3] += (sum alpha*m, sum alpha + m - alpha*m, sum_c |rgb_c*alpha - gt_c*m|)
+// DET: `acc` is the workspace slot array [B][gridDim.x][3]; every CTA stores its three partials
+template <bool DET>
 __global__ void __launch_bounds__(LH_THREADS) k_losshead_partial(const float* __restrict__ rgba, const float* __restrict__ gt,
                                                                 const float* __restrict__ mgt, float* __restrict__ acc,
                                                                 int64_t HW) {
@@ -399,8 +488,24 @@ __global__ void __launch_bounds__(LH_THREADS) k_losshead_partial(const float* __
         su = lane < LH_THREADS / 32 ? s[1][lane] : 0.f;
         sl = lane < LH_THREADS / 32 ? s[2][lane] : 0.f;
         si = warp_sum(si); su = warp_sum(su); sl = warp_sum(sl);
-        if (lane == 0) { atomicAdd(acc + b * 3 + 0, si); atomicAdd(acc + b * 3 + 1, su); atomicAdd(acc + b * 3 + 2, sl); }
+        if (DET) {
+            if (lane == 0) {
+                float* o = acc + ((size_t)b * gridDim.x + blockIdx.x) * 3;
+                o[0] = si; o[1] = su; o[2] = sl;
+            }
+        } else {
+            if (lane == 0) { atomicAdd(acc + b * 3 + 0, si); atomicAdd(acc + b * 3 + 1, su); atomicAdd(acc + b * 3 + 2, sl); }
+        }
     }
+}
+// deterministic pre-pass of k_losshead_finalize: stats[b][k] = image b's slots [nslot][3] summed in ascending CTA order
+__global__ void k_losshead_sum_det(const float* __restrict__ slots, float* __restrict__ stats, int B, int nslot) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;  // (b, k)
+    if (r >= B * 3) return;
+    const float* s = slots + (size_t)(r / 3) * nslot * 3 + r % 3;
+    float t = 0.f;
+    for (int c = 0; c < nslot; ++c) t += s[(size_t)c * 3];
+    stats[r] = t;
 }
 // one warp: stats[b] = (I, U + 1e-6, per-image L1 mean); per_image[b] = (1 - I/U, L1 mean); loss = weighted batch means
 __global__ void k_losshead_finalize(float* __restrict__ acc, float* __restrict__ per_image, float* __restrict__ loss, int B,
@@ -505,7 +610,7 @@ extern "C" int umr_iou_forward(const float* predict, int64_t predict_bstride, co
     e = cudaMemsetAsync(uni, 0, (size_t)B * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     const dim3 grid((unsigned)((N + IOU_PER_CTA - 1) / IOU_PER_CTA), B);
-    count_launch(); k_iou_partial<<<grid, IOU_THREADS, 0, st>>>(predict, target, inter, uni, N, predict_bstride);
+    count_launch(); k_iou_partial<false><<<grid, IOU_THREADS, 0, st>>>(predict, target, inter, uni, N, predict_bstride);
     count_launch(); k_iou_finalize<<<(B + 127) / 128, 128, 0, st>>>(inter, uni, loss, B);
     UMR_RET_LAST();
 }
@@ -581,7 +686,7 @@ extern "C" int umr_texcycle_forward(const float* flow, const float* prob, const 
     }
     const int n = B * F;
     const float scale = 1.f / ((float)n * 2.f);  // MSELoss mean over B*F*2 elements
-    count_launch(); k_texcycle_fwd<<<(n + 255) / 256, 256, 0, st>>>(reinterpret_cast<const float2*>(flow),
+    count_launch(); k_texcycle_fwd<false><<<(n + 255) / 256, 256, 0, st>>>(reinterpret_cast<const float2*>(flow),
                                                     reinterpret_cast<const float2*>(prob), visible, loss, n, T2, scale);
     UMR_RET_LAST();
 }
@@ -610,8 +715,8 @@ extern "C" int umr_masked_l1_forward(const float* pred, int64_t pred_bstride, co
     const dim3 grid((unsigned)((HW + ML1_PER_CTA - 1) / ML1_PER_CTA), B);
     const float inv_n = 1.f / ((float)C * (float)HW);
     count_launch();
-    if (C == 3) k_masked_l1_fwd<3><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, loss, HW, inv_n);
-    else k_masked_l1_fwd<1><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, loss, HW, inv_n);
+    if (C == 3) k_masked_l1_fwd<3, false><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, loss, HW, inv_n);
+    else k_masked_l1_fwd<1, false><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, loss, HW, inv_n);
     UMR_RET_LAST();
 }
 
@@ -641,7 +746,7 @@ extern "C" int umr_loss_head_forward(const float* rgba, const float* gt, const f
     cudaError_t e = cudaMemsetAsync(stats, 0, (size_t)B * 3 * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     count_launch(2);
-    k_losshead_partial<<<dim3((unsigned)((HW + LH_PER_CTA - 1) / LH_PER_CTA), B), LH_THREADS, 0, st>>>(rgba, gt, mask_gt, stats, HW);
+    k_losshead_partial<false><<<dim3((unsigned)((HW + LH_PER_CTA - 1) / LH_PER_CTA), B), LH_THREADS, 0, st>>>(rgba, gt, mask_gt, stats, HW);
     k_losshead_finalize<<<1, 32, 0, st>>>(stats, per_image, loss, B, 1.f / (3.f * (float)HW), w_iou, w_tex);
     return (int)cudaGetLastError();
 }
@@ -656,5 +761,119 @@ extern "C" int umr_loss_head_backward(const float* rgba, const float* gt, const 
     const unsigned gx = (unsigned)std::min<int64_t>((HW + 255) / 256, 1024);
     k_losshead_bwd<<<dim3(gx, B), 256, 0, st>>>(rgba, gt, mask_gt, stats, grad_loss, grad_rgba, HW, B,
                                                 1.f / (3.f * (float)HW), w_iou, w_tex);
+    return (int)cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------
+// deterministic mode (include/umr_b200.h, DESIGN.md §2): each reduction CTA stores its partial into a workspace slot
+// (grids sized from the shapes only, so the slot layout is fixed) and a finalize kernel sums every image's slots in
+// ascending CTA order; the chamfer backward is a gather with one writer per gradient element
+// ---------------------------------------------------------------------------------------------
+static unsigned iou_slots(int64_t N) { return (unsigned)((N + IOU_PER_CTA - 1) / IOU_PER_CTA); }
+static unsigned ml1_slots(int64_t HW) { return (unsigned)((HW + ML1_PER_CTA - 1) / ML1_PER_CTA); }
+static unsigned lh_slots(int64_t HW) { return (unsigned)((HW + LH_PER_CTA - 1) / LH_PER_CTA); }
+
+extern "C" size_t umr_iou_workspace_bytes_deterministic(int32_t B, int64_t N) {
+    if (B <= 0 || N <= 0) return 0;
+    return (size_t)2 * B * iou_slots(N) * sizeof(float);
+}
+extern "C" int umr_iou_forward_deterministic(const float* predict, int64_t predict_bstride, const float* target, float* inter,
+                                             float* uni, float* loss, int32_t B, int64_t N, void* workspace, void* stream_) {
+    if (!predict || !target || !inter || !uni || !loss || !workspace || B <= 0 || N <= 0) return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const unsigned gx = iou_slots(N);
+    float* si = (float*)workspace;
+    float* su = si + (size_t)B * gx;
+    count_launch(); k_iou_partial<true><<<dim3(gx, B), IOU_THREADS, 0, st>>>(predict, target, si, su, N, predict_bstride);
+    count_launch(); k_iou_finalize_det<<<(B + 127) / 128, 128, 0, st>>>(si, su, inter, uni, loss, B, (int)gx);
+    UMR_RET_LAST();
+}
+
+extern "C" int umr_chamfer_backward_deterministic(const float* a, const float* b, const int32_t* idx_ab, const int32_t* idx_ba,
+                                                  const float* grad_dist_ab, const float* grad_dist_ba, float* grad_a,
+                                                  float* grad_b, int32_t B, int32_t N, int32_t M, int32_t D, void* stream_) {
+    if (!a || !b || !grad_a || !grad_b || B <= 0 || N <= 0 || M <= 0) return UMR_ERR_BAD_ARG;
+    if ((grad_dist_ab && !idx_ab) || (grad_dist_ba && !idx_ba)) return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    if (D != 2 && D != 3) return UMR_ERR_UNSUPPORTED;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const dim3 g1((N + 7) / 8, B), g2((M + 7) / 8, B);   // one warp per output point
+    count_launch(2);
+    if (D == 2) {
+        k_chamfer_bwd_gather<2><<<g1, 256, 0, st>>>(a, b, idx_ab, idx_ba, grad_dist_ab, grad_dist_ba, grad_a, N, M);
+        k_chamfer_bwd_gather<2><<<g2, 256, 0, st>>>(b, a, idx_ba, idx_ab, grad_dist_ba, grad_dist_ab, grad_b, M, N);
+    } else {
+        k_chamfer_bwd_gather<3><<<g1, 256, 0, st>>>(a, b, idx_ab, idx_ba, grad_dist_ab, grad_dist_ba, grad_a, N, M);
+        k_chamfer_bwd_gather<3><<<g2, 256, 0, st>>>(b, a, idx_ba, idx_ab, grad_dist_ba, grad_dist_ab, grad_b, M, N);
+    }
+    UMR_RET_LAST();
+}
+
+extern "C" size_t umr_texcycle_workspace_bytes_deterministic(int32_t B, int32_t F) {
+    if (B <= 0 || F <= 0) return 0;
+    return (size_t)(((int64_t)B * F + 255) / 256) * sizeof(float);
+}
+extern "C" int umr_texcycle_forward_deterministic(const float* flow, const float* prob, const float* face_ids, uint8_t* visible,
+                                                  float* loss, int32_t B, int32_t F, int32_t T2, int64_t P, void* workspace,
+                                                  void* stream_) {
+    if (!flow || !prob || !visible || !loss || !workspace || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0))
+        return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (face_ids) {   // the bitmap only ever receives 1s: its bytes do not depend on the order of the stores
+        cudaError_t e = cudaMemsetAsync(visible, 0, (size_t)B * F, st);
+        if (e != cudaSuccess) return (int)e;
+        const int64_t blocks = (P / 4 + 255) / 256 + 1;
+        count_launch(); k_visible<<<dim3((unsigned)(blocks > 1024 ? 1024 : blocks), B), 256, 0, st>>>(face_ids, visible, F, P);
+    }
+    const int n = B * F;
+    const int gx = (n + 255) / 256;
+    const float scale = 1.f / ((float)n * 2.f);
+    float* slots = (float*)workspace;
+    count_launch(); k_texcycle_fwd<true><<<gx, 256, 0, st>>>(reinterpret_cast<const float2*>(flow),
+                                                             reinterpret_cast<const float2*>(prob), visible, slots, n, T2, scale);
+    count_launch(); k_sum_slot_rows<<<1, 32, 0, st>>>(slots, loss, 1, gx);
+    UMR_RET_LAST();
+}
+
+extern "C" size_t umr_masked_l1_workspace_bytes_deterministic(int32_t B, int64_t HW) {
+    if (B <= 0 || HW <= 0) return 0;
+    return (size_t)B * ml1_slots(HW) * sizeof(float);
+}
+extern "C" int umr_masked_l1_forward_deterministic(const float* pred, int64_t pred_bstride, const float* mask_pred,
+                                                   int64_t mask_pred_bstride, const float* gt, const float* mask_gt, float* loss,
+                                                   int32_t B, int32_t C, int64_t HW, void* workspace, void* stream_) {
+    if (!pred || !mask_pred || !gt || !mask_gt || !loss || !workspace || B <= 0 || HW <= 0) return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    if (C != 3 && C != 1) return UMR_ERR_UNSUPPORTED;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const unsigned gx = ml1_slots(HW);
+    const dim3 grid(gx, B);
+    const float inv_n = 1.f / ((float)C * (float)HW);
+    float* slots = (float*)workspace;
+    count_launch(2);
+    if (C == 3) k_masked_l1_fwd<3, true><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, slots, HW, inv_n);
+    else k_masked_l1_fwd<1, true><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, slots, HW, inv_n);
+    k_sum_slot_rows<<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, (int)gx);
+    UMR_RET_LAST();
+}
+
+extern "C" size_t umr_loss_head_workspace_bytes_deterministic(int32_t B, int64_t HW) {
+    if (B <= 0 || HW <= 0) return 0;
+    return (size_t)3 * B * lh_slots(HW) * sizeof(float);
+}
+extern "C" int umr_loss_head_forward_deterministic(const float* rgba, const float* gt, const float* mask_gt, float* stats,
+                                                   float* per_image, float* loss, int32_t B, int64_t HW, float w_iou,
+                                                   float w_tex, void* workspace, void* stream_) {
+    if (!rgba || !gt || !mask_gt || !stats || !per_image || !loss || !workspace || B <= 0 || HW <= 0) return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const unsigned gx = lh_slots(HW);
+    float* slots = (float*)workspace;
+    count_launch(3);
+    k_losshead_partial<true><<<dim3(gx, B), LH_THREADS, 0, st>>>(rgba, gt, mask_gt, slots, HW);
+    k_losshead_sum_det<<<(3 * B + 127) / 128, 128, 0, st>>>(slots, stats, B, (int)gx);
+    k_losshead_finalize<<<1, 32, 0, st>>>(stats, per_image, loss, B, 1.f / (3.f * (float)HW), w_iou, w_tex);
     return (int)cudaGetLastError();
 }

@@ -12,6 +12,8 @@
 //                           forward and hand-derived backward instead of ~40 elementwise torch kernels.
 //   k_edt_*                 utils/image.py:130-141 compute_dt_barrier: exact Euclidean distance transform of the GT mask,
 //                           scipy on the host CPU per image per step in the reference (train_s2.py:196).
+// The Laplacian / flatten sums and the flatten backward have deterministic variants (DET template parameter,
+// k_flatten_gather; `*_deterministic` entry points at the end of this file; DESIGN.md §2).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -101,6 +103,8 @@ __global__ void __launch_bounds__(256) k_load_textures(const float* __restrict__
 // Laplacian regulariser on a CSR neighbour table: y_i = x_i + sum_j coef[i,j] x_j  (coef = -1/deg_i as float32,
 // exactly the off-diagonal entries of the reference's row-normalised matrix), loss_b = sum_i |y_i|^2
 // ---------------------------------------------------------------------------------------------
+// DET: `loss` is the workspace slot array [B][gridDim.x]; every CTA stores its partial
+template <bool DET>
 __global__ void __launch_bounds__(256) k_laplacian_fwd(const float* __restrict__ x, const int32_t* __restrict__ rowptr,
                                                        const int32_t* __restrict__ col, const float* __restrict__ coef,
                                                        float* __restrict__ y, float* __restrict__ loss, int V) {
@@ -127,8 +131,17 @@ __global__ void __launch_bounds__(256) k_laplacian_fwd(const float* __restrict__
     if (warp == 0) {
         acc = lane < 8 ? s[lane] : 0.f;
         acc = warp_sum(acc);
-        if (lane == 0) atomicAdd(loss + b, acc);
+        if (DET) {
+            if (lane == 0) loss[(size_t)b * gridDim.x + blockIdx.x] = acc;
+        } else {
+            if (lane == 0) atomicAdd(loss + b, acc);
+        }
     }
+}
+// deterministic finalize of the Laplacian / flatten sums: loss[b] = image b's n slots summed in ascending CTA order
+__global__ void k_mesh_loss_sum_det(const float* __restrict__ slots, float* __restrict__ loss, int B, int n) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < B) loss[b] = sum_ascending(slots + (size_t)b * n, n);
 }
 // grad_x_j = 2 g_b (y_j + sum_{i : j in N(i)} coef[i,j] y_i); the neighbour relation is symmetric, so the transposed
 // entry of (j, i) is looked up through tcoef[e] = coef of row col[e] towards j (precomputed on the host)
@@ -200,7 +213,9 @@ __device__ __forceinline__ void perp_bwd(const Perp& P, const float* dcb, float 
         db[d] += dab * P.a[d] + 2.f * dbl2 * P.b[d];
     }
 }
-template <bool BWD>
+// DET forward: `loss` is the workspace slot array [B][gridDim.x].  DET backward: `gverts` is the per-edge term array
+// [B][E][4][3] (roles v0..v3), summed per vertex by k_flatten_gather.
+template <bool BWD, bool DET>
 __global__ void __launch_bounds__(128) k_flatten(const float* __restrict__ verts, const int32_t* __restrict__ edges,
                                                  float* __restrict__ loss, const float* __restrict__ gl,
                                                  float* __restrict__ gverts, int V, int E, float eps) {
@@ -233,13 +248,24 @@ __global__ void __launch_bounds__(128) k_flatten(const float* __restrict__ verts
             for (int d = 0; d < 3; ++d) { dcb1[d] = dnum * P2.cb[d]; dcb2[d] = dnum * P1.cb[d]; }
             perp_bwd(P1, dcb1, dden * P2.l, eps, da, db1);
             perp_bwd(P2, dcb2, dden * P1.l, eps, da, db2);
-            float* gb = gverts + (size_t)b * V * 3;
+            if (DET) {
+                float* t = gverts + ((size_t)b * E + e) * 12;
 #pragma unroll
-            for (int d = 0; d < 3; ++d) {
-                atomicAdd(gb + i1 * 3 + d, da[d]);
-                atomicAdd(gb + i2 * 3 + d, db1[d]);
-                atomicAdd(gb + i3 * 3 + d, db2[d]);
-                atomicAdd(gb + i0 * 3 + d, -(da[d] + db1[d] + db2[d]));
+                for (int d = 0; d < 3; ++d) {
+                    t[d] = -(da[d] + db1[d] + db2[d]);
+                    t[3 + d] = da[d];
+                    t[6 + d] = db1[d];
+                    t[9 + d] = db2[d];
+                }
+            } else {
+                float* gb = gverts + (size_t)b * V * 3;
+#pragma unroll
+                for (int d = 0; d < 3; ++d) {
+                    atomicAdd(gb + i1 * 3 + d, da[d]);
+                    atomicAdd(gb + i2 * 3 + d, db1[d]);
+                    atomicAdd(gb + i3 * 3 + d, db2[d]);
+                    atomicAdd(gb + i0 * 3 + d, -(da[d] + db1[d] + db2[d]));
+                }
             }
         }
     }
@@ -252,9 +278,30 @@ __global__ void __launch_bounds__(128) k_flatten(const float* __restrict__ verts
         if (warp == 0) {
             acc = lane < 4 ? s[lane] : 0.f;
             acc = warp_sum(acc);
-            if (lane == 0) atomicAdd(loss + b, acc);
+            if (DET) {
+                if (lane == 0) loss[(size_t)b * gridDim.x + blockIdx.x] = acc;
+            } else {
+                if (lane == 0) atomicAdd(loss + b, acc);
+            }
         }
     }
+}
+// grad_vertices[b][v] = sum of v's per-edge terms over the transposed incidence table: vrowptr [V+1], vinc [4E] lists
+// edge * 4 + role in ascending order, so the sum order is fixed; a vertex on no edge gets 0
+__global__ void __launch_bounds__(256) k_flatten_gather(const float* __restrict__ terms, const int32_t* __restrict__ vrowptr,
+                                                        const int32_t* __restrict__ vinc, float* __restrict__ gverts, int V,
+                                                        int E) {
+    const int b = blockIdx.y;
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    const float* tb = terms + (size_t)b * E * 12;
+    float g0 = 0.f, g1 = 0.f, g2 = 0.f;
+    for (int k = __ldg(vrowptr + v); k < __ldg(vrowptr + v + 1); ++k) {
+        const float* t = tb + (size_t)__ldg(vinc + k) * 3;
+        g0 += t[0]; g1 += t[1]; g2 += t[2];
+    }
+    float* o = gverts + ((size_t)b * V + v) * 3;
+    o[0] = g0; o[1] = g1; o[2] = g2;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -363,7 +410,7 @@ extern "C" int umr_laplacian_forward(const float* x, const int32_t* rowptr, cons
     cudaError_t e = cudaMemsetAsync(loss, 0, (size_t)B * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     count_launch();
-    k_laplacian_fwd<<<dim3((V + 255) / 256, B), 256, 0, st>>>(x, rowptr, col, coef, y, loss, V);
+    k_laplacian_fwd<false><<<dim3((V + 255) / 256, B), 256, 0, st>>>(x, rowptr, col, coef, y, loss, V);
     UMR_RET();
 }
 extern "C" int umr_laplacian_backward(const float* y, const int32_t* rowptr, const int32_t* col, const float* tcoef,
@@ -383,7 +430,7 @@ extern "C" int umr_flatten_forward(const float* vertices, const int32_t* edges, 
     cudaError_t e = cudaMemsetAsync(loss, 0, (size_t)B * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     count_launch();
-    k_flatten<false><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, loss, nullptr, nullptr, V, E, eps);
+    k_flatten<false, false><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, loss, nullptr, nullptr, V, E, eps);
     UMR_RET();
 }
 extern "C" int umr_flatten_backward(const float* vertices, const int32_t* edges, const float* grad_loss, float* grad_vertices,
@@ -394,7 +441,7 @@ extern "C" int umr_flatten_backward(const float* vertices, const int32_t* edges,
     cudaError_t e = cudaMemsetAsync(grad_vertices, 0, (size_t)B * V * 3 * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     count_launch();
-    k_flatten<true><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, nullptr, grad_loss, grad_vertices, V, E, eps);
+    k_flatten<true, false><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, nullptr, grad_loss, grad_vertices, V, E, eps);
     UMR_RET();
 }
 
@@ -412,5 +459,62 @@ extern "C" int umr_dt_barrier(const float* mask, float* dt, void* workspace, int
     count_launch(2);
     k_edt_columns<<<dim3((W + 255) / 256, B), 256, 0, st>>>(mask, g_out, g_in, H, W);
     k_edt_rows<<<dim3(H, B), 256, (size_t)2 * W * sizeof(int32_t), st>>>(g_out, g_in, dt, H, W, k, 1.f / (float)std::max(H, W));
+    UMR_RET();
+}
+
+// ---------------------------------------------------------------------------------------------
+// deterministic mode (include/umr_b200.h, DESIGN.md §2): per-CTA partials stored in workspace slots and summed in
+// ascending CTA order; the flatten backward writes per-edge terms and gathers them per vertex
+// ---------------------------------------------------------------------------------------------
+extern "C" size_t umr_laplacian_workspace_bytes_deterministic(int32_t B, int32_t V) {
+    if (B <= 0 || V <= 0) return 0;
+    return (size_t)B * ((V + 255) / 256) * sizeof(float);
+}
+extern "C" int umr_laplacian_forward_deterministic(const float* x, const int32_t* rowptr, const int32_t* col, const float* coef,
+                                                   float* y, float* loss, int32_t B, int32_t V, void* workspace, void* stream_) {
+    if (!x || !rowptr || !col || !coef || !y || !loss || !workspace || B <= 0 || V <= 0) return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const int gx = (V + 255) / 256;
+    float* slots = (float*)workspace;
+    count_launch(2);
+    k_laplacian_fwd<true><<<dim3(gx, B), 256, 0, st>>>(x, rowptr, col, coef, y, slots, V);
+    k_mesh_loss_sum_det<<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, gx);
+    UMR_RET();
+}
+
+extern "C" size_t umr_flatten_forward_workspace_bytes_deterministic(int32_t B, int32_t E) {
+    if (B <= 0 || E <= 0) return 0;
+    return (size_t)B * ((E + 127) / 128) * sizeof(float);
+}
+extern "C" int umr_flatten_forward_deterministic(const float* vertices, const int32_t* edges, float* loss, int32_t B, int32_t V,
+                                                 int32_t E, float eps, void* workspace, void* stream_) {
+    if (!vertices || !edges || !loss || !workspace || B <= 0 || V <= 0 || E <= 0) return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const int gx = (E + 127) / 128;
+    float* slots = (float*)workspace;
+    count_launch(2);
+    k_flatten<false, true><<<dim3(gx, B), 128, 0, st>>>(vertices, edges, slots, nullptr, nullptr, V, E, eps);
+    k_mesh_loss_sum_det<<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, gx);
+    UMR_RET();
+}
+
+extern "C" size_t umr_flatten_backward_workspace_bytes_deterministic(int32_t B, int32_t E) {
+    if (B <= 0 || E <= 0) return 0;
+    return (size_t)B * E * 12 * sizeof(float);
+}
+extern "C" int umr_flatten_backward_deterministic(const float* vertices, const int32_t* edges, const int32_t* vert_rowptr,
+                                                  const int32_t* vert_incidence, const float* grad_loss, float* grad_vertices,
+                                                  int32_t B, int32_t V, int32_t E, float eps, void* workspace, void* stream_) {
+    if (!vertices || !edges || !vert_rowptr || !vert_incidence || !grad_loss || !grad_vertices || !workspace || B <= 0 ||
+        V <= 0 || E <= 0)
+        return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    cudaStream_t st = (cudaStream_t)stream_;
+    float* terms = (float*)workspace;
+    count_launch(2);
+    k_flatten<true, true><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, nullptr, grad_loss, terms, V, E, eps);
+    k_flatten_gather<<<dim3((V + 255) / 256, B), 256, 0, st>>>(terms, vert_rowptr, vert_incidence, grad_vertices, V, E);
     UMR_RET();
 }

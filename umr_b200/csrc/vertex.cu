@@ -350,6 +350,8 @@ __device__ __forceinline__ void project_point_backward(const Cam& k, float X, fl
 
 // backward: grad_loss [B] (per render), optional grad_vert2d [B,NS,2] -> grad_verts [B,V,3] (zero-filled by the host,
 // atomics: a vertex may sit in several parts) and grad_cams [B,7].  Targets are constants (the reference's are data).
+// DET: `gverts` is the per-(render, j) term array [B,NS,3] (plain stores), summed per vertex by k_corr_gather.
+template <bool DET>
 __global__ void __launch_bounds__(256) k_corr_bwd(const float* __restrict__ verts, int64_t verts_bstride, const float* __restrict__ cams,
                                                   const int32_t* __restrict__ sel, CorrCfg c, const float* __restrict__ vert2d,
                                                   const int32_t* __restrict__ nn, const float* __restrict__ grad_loss,
@@ -376,8 +378,13 @@ __global__ void __launch_bounds__(256) k_corr_bwd(const float* __restrict__ vert
         float o0, o1, o2;
         project_point_backward(k, __ldg(p), __ldg(p + 1), __ldg(p + 2), gx, gy, 0.f, gc, o0, o1, o2);
         if (gverts != nullptr) {
-            float* o = gverts + ((size_t)b * V + vi) * 3;
-            atomicAdd(o, o0); atomicAdd(o + 1, o1); atomicAdd(o + 2, o2);
+            if (DET) {
+                float* o = gverts + ((size_t)b * NS + j) * 3;
+                o[0] = o0; o[1] = o1; o[2] = o2;
+            } else {
+                float* o = gverts + ((size_t)b * V + vi) * 3;
+                atomicAdd(o, o0); atomicAdd(o + 1, o1); atomicAdd(o + 2, o2);
+            }
         }
     }
     if (gcams == nullptr) return;
@@ -392,6 +399,22 @@ __global__ void __launch_bounds__(256) k_corr_bwd(const float* __restrict__ vert
         for (int w = 0; w < 8; ++w) r += s[w][threadIdx.x];
         gcams[(size_t)b * 7 + threadIdx.x] = r;   // one CTA per render: plain store
     }
+}
+// grad_verts[b][v] = sum of v's (render, j) terms over the transposed selection table: vrowptr [V+1], vsel [NS] lists the
+// j with selection[j] == v in ascending order, so the sum order is fixed; an unselected vertex gets 0
+__global__ void __launch_bounds__(256) k_corr_gather(const float* __restrict__ terms, const int32_t* __restrict__ vrowptr,
+                                                     const int32_t* __restrict__ vsel, float* __restrict__ gverts, int NS, int V) {
+    const int b = blockIdx.y;
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    const float* tb = terms + (size_t)b * NS * 3;
+    float g0 = 0.f, g1 = 0.f, g2 = 0.f;
+    for (int k = __ldg(vrowptr + v); k < __ldg(vrowptr + v + 1); ++k) {
+        const float* t = tb + (size_t)__ldg(vsel + k) * 3;
+        g0 += t[0]; g1 += t[1]; g2 += t[2];
+    }
+    float* o = gverts + ((size_t)b * V + v) * 3;
+    o[0] = g0; o[1] = g1; o[2] = g2;
 }
 
 }  // namespace umr
@@ -499,7 +522,39 @@ extern "C" int umr_corr_chamfer_backward(const float* vertices, int64_t vertices
         if (e != cudaSuccess) return (int)e;
     }
     count_launch();
-    k_corr_bwd<<<B, 256, 0, st>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss, grad_vert2d,
+    k_corr_bwd<false><<<B, 256, 0, st>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss, grad_vert2d,
                                   grad_vertices, grad_cams, NS, V);
+    return (int)cudaGetLastError();
+}
+
+// Deterministic backward (include/umr_b200.h): k_corr_bwd<true> stores the per-(render, j) vertex terms in the workspace,
+// k_corr_gather sums them per vertex in ascending j.  grad_cams is the default kernel's plain store.
+extern "C" size_t umr_corr_chamfer_workspace_bytes_deterministic(int32_t B, int32_t NS) {
+    if (B <= 0 || NS <= 0) return 0;
+    return (size_t)B * NS * 3 * sizeof(float);
+}
+extern "C" int umr_corr_chamfer_backward_deterministic(const float* vertices, int64_t vertices_batch_stride, const float* cams,
+                                                       const int32_t* selection, const float* const* targets,
+                                                       const int32_t* target_counts, const int32_t* part_ends,
+                                                       const float* weights, const float* vert2d, const int32_t* nearest,
+                                                       const float* grad_loss, const float* grad_vert2d, float* grad_vertices,
+                                                       float* grad_cams, int32_t B, int32_t NS, int32_t V,
+                                                       const int32_t* vert_rowptr, const int32_t* vert_selection,
+                                                       void* workspace, void* stream_) {
+    if (!vertices || !cams || !selection || !targets || !target_counts || !part_ends || !weights || !vert2d || !nearest ||
+        !grad_loss || B <= 0 || NS <= 0 || V <= 0)
+        return UMR_ERR_BAD_ARG;
+    if (grad_vertices && (!vert_rowptr || !vert_selection || !workspace)) return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    CorrCfg c;
+    const int rc = make_corr_cfg(c, targets, target_counts, part_ends, weights, NS);
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream_;
+    float* terms = grad_vertices ? (float*)workspace : nullptr;
+    count_launch(grad_vertices ? 2 : 1);
+    k_corr_bwd<true><<<B, 256, 0, st>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss, grad_vert2d,
+                                        terms, grad_cams, NS, V);
+    if (grad_vertices)
+        k_corr_gather<<<dim3((V + 255) / 256, B), 256, 0, st>>>(terms, vert_rowptr, vert_selection, grad_vertices, NS, V);
     return (int)cudaGetLastError();
 }

@@ -206,8 +206,10 @@ class CorrLossChamfer(nn.Module):
                 # checked once per (device, vertex count): the kernels gather verts[:, idx] without a bounds test of their own
                 if idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= verts.shape[1]):
                     raise IndexError("part vertex index out of range for a mesh of %d vertices" % verts.shape[1])
-                cache[key] = idx.to(torch.int32)
-            loss, vert2d = ops.corr_chamfer(verts, cams, cache[key], targets, self.nums, self.weights)
+                # with its transposed table (vertex -> ascending j) for the deterministic backward's per-vertex gather
+                cache[key] = (idx.to(torch.int32), _vertex_table(groups, int(verts.shape[1]), verts.device))
+            sel, vert_table = cache[key]
+            loss, vert2d = ops.corr_chamfer(verts, cams, sel, targets, self.nums, self.weights, vert_table)
             if avg:
                 return torch.mean(loss), vert2d
             return loss
@@ -222,6 +224,12 @@ class CorrLossChamfer(nn.Module):
         if avg:
             return torch.mean(loss), vert2d
         return loss
+
+
+def _vertex_table(groups, num_vertices, device):
+    """The concatenated part selection transposed on the host (ops.vertex_incidence), uploaded to `device`."""
+    rowptr, pos = ops.vertex_incidence(torch.cat(groups).numpy(), num_vertices)
+    return torch.from_numpy(rowptr).to(device), torch.from_numpy(pos).to(device)
 
 
 # ---------------------------------------------------------------------------------------------

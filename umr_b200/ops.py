@@ -1,9 +1,14 @@
 """torch.autograd bindings of the geometric-loss kernels (C ABI: include/umr_b200.h).
 
 CUDA only: there is no CPU fallback (the CPU oracles live in oracle/ and are test infrastructure).
+
+Under torch.use_deterministic_algorithms(True) the Functions whose default kernels sum with float atomics call the
+`*_deterministic` symbols instead (bitwise reproducible, DESIGN.md §2).  The flag is read once in `forward` and kept in
+`ctx`, so a backward runs in the mode of its forward.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -14,6 +19,30 @@ def _need_cuda(*ts):
     for t in ts:
         if not t.is_cuda:
             raise TypeError("umr_b200 ops support only cuda Tensors")
+
+
+def _workspace(nbytes, device):
+    """Device scratch of a deterministic call (an allocation, no fill: CUDA-graph safe)."""
+    return torch.empty(nbytes, device=device, dtype=torch.uint8)
+
+
+def vertex_incidence(index, num_vertices):
+    """Transposed index table of the deterministic gathers: `index` (any shape, values in [0, num_vertices)) ->
+    (rowptr [V+1], positions) int32 numpy arrays, where positions[rowptr[v]:rowptr[v+1]] are the flat positions k with
+    index.flat[k] == v in ascending order.  The flatten loss passes its [E,4] edge table (position = edge * 4 + role), the
+    part-chamfer loss its vertex selection [NS] (position = j)."""
+    flat = np.asarray(index, dtype=np.int64).reshape(-1)
+    if flat.size and (flat.min() < 0 or flat.max() >= num_vertices):
+        raise IndexError("vertex index out of range for a mesh of %d vertices" % num_vertices)
+    positions = np.argsort(flat, kind="stable").astype(np.int32)
+    rowptr = np.zeros(num_vertices + 1, np.int64)
+    np.cumsum(np.bincount(flat, minlength=num_vertices), out=rowptr[1:])
+    return rowptr.astype(np.int32), positions
+
+
+def _incidence_on(index, num_vertices, device):
+    rowptr, pos = vertex_incidence(index.detach().cpu().numpy(), num_vertices)
+    return torch.from_numpy(rowptr).to(device), torch.from_numpy(pos).to(device)
 
 
 def _batch_view(t, inner):
@@ -86,13 +115,19 @@ class NegIouFunction(torch.autograd.Function):
         t = target.detach().contiguous().float().view(B, -1)
         N = t.shape[1]
         p, pbs = _batch_view(predict.detach(), N)  # e.g. the alpha plane of the RGBA render, read in place
+        det = torch.are_deterministic_algorithms_enabled()
         with torch.cuda.device(p.device):
             inter = torch.empty(B, device=p.device, dtype=torch.float32)
             uni = torch.empty_like(inter)
             loss = torch.empty_like(inter)
-            rc = lib.umr_iou_forward(_ptr(p), pbs, _ptr(t), _ptr(inter), _ptr(uni), _ptr(loss), B, N,
-                                     _stream_ptr(p.device))
-        _lib.check(rc, "umr_iou_forward")
+            if det:
+                ws = _workspace(lib.umr_iou_workspace_bytes_deterministic(B, N), p.device)
+                rc = lib.umr_iou_forward_deterministic(_ptr(p), pbs, _ptr(t), _ptr(inter), _ptr(uni), _ptr(loss), B, N,
+                                                       _ptr(ws), _stream_ptr(p.device))
+            else:
+                rc = lib.umr_iou_forward(_ptr(p), pbs, _ptr(t), _ptr(inter), _ptr(uni), _ptr(loss), B, N,
+                                         _stream_ptr(p.device))
+        _lib.check(rc, "umr_iou_forward_deterministic" if det else "umr_iou_forward")
         ctx.save_for_backward(t, inter, uni)
         ctx.shape = tuple(predict.shape)
         return loss
@@ -135,11 +170,17 @@ class MaskedL1Function(torch.autograd.Function):
         mp, mbs = _batch_view(mask_pred.detach(), HW)
         g = img_gt.detach().contiguous().float()
         mg = mask_gt.detach().contiguous().float()
+        det = torch.are_deterministic_algorithms_enabled()
         with torch.cuda.device(p.device):
             loss = torch.empty(B, device=p.device, dtype=torch.float32)
-            rc = lib.umr_masked_l1_forward(_ptr(p), pbs, _ptr(mp), mbs, _ptr(g), _ptr(mg), _ptr(loss), B, C, HW,
-                                           _stream_ptr(p.device))
-        _lib.check(rc, "umr_masked_l1_forward")
+            if det:
+                ws = _workspace(lib.umr_masked_l1_workspace_bytes_deterministic(B, HW), p.device)
+                rc = lib.umr_masked_l1_forward_deterministic(_ptr(p), pbs, _ptr(mp), mbs, _ptr(g), _ptr(mg), _ptr(loss), B, C,
+                                                             HW, _ptr(ws), _stream_ptr(p.device))
+            else:
+                rc = lib.umr_masked_l1_forward(_ptr(p), pbs, _ptr(mp), mbs, _ptr(g), _ptr(mg), _ptr(loss), B, C, HW,
+                                               _stream_ptr(p.device))
+        _lib.check(rc, "umr_masked_l1_forward_deterministic" if det else "umr_masked_l1_forward")
         ctx.save_for_backward(p, mp, g, mg)
         ctx.meta = (pbs, mbs, img_pred.requires_grad, mask_pred.requires_grad, tuple(img_pred.shape),
                     tuple(mask_pred.shape))
@@ -184,13 +225,20 @@ class LossHeadFunction(torch.autograd.Function):
         x = images.detach().contiguous().float()
         g = img_gt.detach().contiguous().float()
         m = mask_gt.detach().contiguous().float()
+        det = torch.are_deterministic_algorithms_enabled()
         with torch.cuda.device(x.device):
             stats = torch.empty(B, 3, device=x.device, dtype=torch.float32)
             per_image = torch.empty(B, 2, device=x.device, dtype=torch.float32)
             loss = torch.empty((), device=x.device, dtype=torch.float32)
-            rc = lib.umr_loss_head_forward(_ptr(x), _ptr(g), _ptr(m), _ptr(stats), _ptr(per_image), _ptr(loss), B, H * W,
-                                           float(w_iou), float(w_tex), _stream_ptr(x.device))
-        _lib.check(rc, "umr_loss_head_forward")
+            if det:
+                ws = _workspace(lib.umr_loss_head_workspace_bytes_deterministic(B, H * W), x.device)
+                rc = lib.umr_loss_head_forward_deterministic(_ptr(x), _ptr(g), _ptr(m), _ptr(stats), _ptr(per_image),
+                                                             _ptr(loss), B, H * W, float(w_iou), float(w_tex), _ptr(ws),
+                                                             _stream_ptr(x.device))
+            else:
+                rc = lib.umr_loss_head_forward(_ptr(x), _ptr(g), _ptr(m), _ptr(stats), _ptr(per_image), _ptr(loss), B,
+                                               H * W, float(w_iou), float(w_tex), _stream_ptr(x.device))
+        _lib.check(rc, "umr_loss_head_forward_deterministic" if det else "umr_loss_head_forward")
         ctx.save_for_backward(x, g, m, stats)
         ctx.w = (float(w_iou), float(w_tex))
         ctx.mark_non_differentiable(per_image)
@@ -238,6 +286,7 @@ class ChamferFunction(torch.autograd.Function):
         _lib.check(rc, "umr_chamfer_forward")
         ctx.save_for_backward(x, y, i_ab, i_ba)
         ctx.mark_non_differentiable(i_ab, i_ba)
+        ctx.det = torch.are_deterministic_algorithms_enabled()   # the forward has no atomics; the backward's mode
         return d_ab, d_ba, i_ab, i_ba
 
     @staticmethod
@@ -251,9 +300,10 @@ class ChamferFunction(torch.autograd.Function):
         with torch.cuda.device(x.device):
             gx = torch.empty_like(x)
             gy = torch.empty_like(y)
-            rc = lib.umr_chamfer_backward(_ptr(x), _ptr(y), _ptr(i_ab), _ptr(i_ba), _ptr(g1), _ptr(g2),
-                                          _ptr(gx), _ptr(gy), B, N, M, D, _stream_ptr(x.device))
-        _lib.check(rc, "umr_chamfer_backward")
+            bwd = lib.umr_chamfer_backward_deterministic if ctx.det else lib.umr_chamfer_backward
+            rc = bwd(_ptr(x), _ptr(y), _ptr(i_ab), _ptr(i_ba), _ptr(g1), _ptr(g2), _ptr(gx), _ptr(gy), B, N, M, D,
+                     _stream_ptr(x.device))
+        _lib.check(rc, "umr_chamfer_backward_deterministic" if ctx.det else "umr_chamfer_backward")
         return gx, gy
 
 
@@ -282,12 +332,18 @@ class TexCycleFunction(torch.autograd.Function):
         else:
             ids = face_ids.detach().contiguous().float()
             P = ids.shape[1]
+        det = torch.are_deterministic_algorithms_enabled()
         with torch.cuda.device(fl.device):
             vis = visible.contiguous() if visible is not None else torch.empty(B, F, device=fl.device, dtype=torch.uint8)
             loss = torch.empty(1, device=fl.device, dtype=torch.float32)
-            rc = lib.umr_texcycle_forward(_ptr(fl), _ptr(pr), _ptr(ids), _ptr(vis), _ptr(loss), B, F, T2, P,
-                                          _stream_ptr(fl.device))
-        _lib.check(rc, "umr_texcycle_forward")
+            if det:
+                ws = _workspace(lib.umr_texcycle_workspace_bytes_deterministic(B, F), fl.device)
+                rc = lib.umr_texcycle_forward_deterministic(_ptr(fl), _ptr(pr), _ptr(ids), _ptr(vis), _ptr(loss), B, F, T2,
+                                                            P, _ptr(ws), _stream_ptr(fl.device))
+            else:
+                rc = lib.umr_texcycle_forward(_ptr(fl), _ptr(pr), _ptr(ids), _ptr(vis), _ptr(loss), B, F, T2, P,
+                                              _stream_ptr(fl.device))
+        _lib.check(rc, "umr_texcycle_forward_deterministic" if det else "umr_texcycle_forward")
         ctx.save_for_backward(fl, pr, vis)
         return loss.view(())
 
@@ -321,12 +377,18 @@ class LaplacianFunction(torch.autograd.Function):
         lib = _lib.load()
         xx = x.detach().contiguous().float()
         B, V = xx.shape[:2]
+        det = torch.are_deterministic_algorithms_enabled()
         with torch.cuda.device(xx.device):
             y = torch.empty_like(xx)
             loss = torch.empty(B, device=xx.device, dtype=torch.float32)
-            rc = lib.umr_laplacian_forward(_ptr(xx), _ptr(rowptr), _ptr(col), _ptr(coef), _ptr(y), _ptr(loss), B, V,
-                                           _stream_ptr(xx.device))
-        _lib.check(rc, "umr_laplacian_forward")
+            if det:
+                ws = _workspace(lib.umr_laplacian_workspace_bytes_deterministic(B, V), xx.device)
+                rc = lib.umr_laplacian_forward_deterministic(_ptr(xx), _ptr(rowptr), _ptr(col), _ptr(coef), _ptr(y),
+                                                             _ptr(loss), B, V, _ptr(ws), _stream_ptr(xx.device))
+            else:
+                rc = lib.umr_laplacian_forward(_ptr(xx), _ptr(rowptr), _ptr(col), _ptr(coef), _ptr(y), _ptr(loss), B, V,
+                                               _stream_ptr(xx.device))
+        _lib.check(rc, "umr_laplacian_forward_deterministic" if det else "umr_laplacian_forward")
         ctx.save_for_backward(y, rowptr, col, tcoef)
         return loss
 
@@ -345,35 +407,62 @@ class LaplacianFunction(torch.autograd.Function):
 
 
 class FlattenFunction(torch.autograd.Function):
-    """vertices [B,V,3] + edge table [E,4] int32 -> per-sample sum_e (cos + 1)^2 [B] (SoftRas/losses.py:71-114)."""
+    """vertices [B,V,3] + edge table [E,4] int32 -> per-sample sum_e (cos + 1)^2 [B] (SoftRas/losses.py:71-114).
+    `vert_rowptr` / `vert_incidence`: the edge table's transposed incidence (`vertex_incidence(edges, V)` on the device),
+    used by the deterministic backward; FlattenLoss builds it once.  Without it a deterministic call builds it here (a
+    device-to-host copy of the edge table)."""
 
     @staticmethod
-    def forward(ctx, vertices, edges, eps):
+    def forward(ctx, vertices, edges, eps, vert_rowptr=None, vert_incidence=None):
         _need_cuda(vertices)
         lib = _lib.load()
         v = vertices.detach().contiguous().float()
         B, V = v.shape[:2]
         E = edges.shape[0]
+        det = torch.are_deterministic_algorithms_enabled()
         with torch.cuda.device(v.device):
             loss = torch.empty(B, device=v.device, dtype=torch.float32)
-            rc = lib.umr_flatten_forward(_ptr(v), _ptr(edges), _ptr(loss), B, V, E, float(eps), _stream_ptr(v.device))
-        _lib.check(rc, "umr_flatten_forward")
-        ctx.save_for_backward(v, edges)
+            if det:
+                ws = _workspace(lib.umr_flatten_forward_workspace_bytes_deterministic(B, E), v.device)
+                rc = lib.umr_flatten_forward_deterministic(_ptr(v), _ptr(edges), _ptr(loss), B, V, E, float(eps), _ptr(ws),
+                                                           _stream_ptr(v.device))
+            else:
+                rc = lib.umr_flatten_forward(_ptr(v), _ptr(edges), _ptr(loss), B, V, E, float(eps), _stream_ptr(v.device))
+        _lib.check(rc, "umr_flatten_forward_deterministic" if det else "umr_flatten_forward")
+        if det:
+            if vert_rowptr is None or vert_incidence is None:
+                vert_rowptr, vert_incidence = _incidence_on(edges, V, v.device)
+            elif vert_rowptr.numel() < V + 1:   # vertices beyond the table's are on no edge
+                vert_rowptr = torch.cat((vert_rowptr, vert_rowptr[-1:].expand(V + 1 - vert_rowptr.numel())))
+            elif vert_rowptr.numel() > V + 1:
+                raise ValueError("flatten loss: the edge table indexes %d vertices, the mesh has %d"
+                                 % (vert_rowptr.numel() - 1, V))
+            ctx.save_for_backward(v, edges, vert_rowptr, vert_incidence)
+        else:
+            ctx.save_for_backward(v, edges)
         ctx.eps = float(eps)
+        ctx.det = det
         return loss
 
     @staticmethod
     def backward(ctx, g):
         lib = _lib.load()
-        v, edges = ctx.saved_tensors
+        v, edges = ctx.saved_tensors[:2]
         B, V = v.shape[:2]
+        E = edges.shape[0]
         gl = g.contiguous().float()
         with torch.cuda.device(v.device):
             gv = torch.empty_like(v)
-            rc = lib.umr_flatten_backward(_ptr(v), _ptr(edges), _ptr(gl), _ptr(gv), B, V, edges.shape[0], ctx.eps,
-                                          _stream_ptr(v.device))
-        _lib.check(rc, "umr_flatten_backward")
-        return gv, None, None
+            if ctx.det:
+                rowptr, inc = ctx.saved_tensors[2:]
+                ws = _workspace(lib.umr_flatten_backward_workspace_bytes_deterministic(B, E), v.device)
+                rc = lib.umr_flatten_backward_deterministic(_ptr(v), _ptr(edges), _ptr(rowptr), _ptr(inc), _ptr(gl), _ptr(gv),
+                                                            B, V, E, ctx.eps, _ptr(ws), _stream_ptr(v.device))
+            else:
+                rc = lib.umr_flatten_backward(_ptr(v), _ptr(edges), _ptr(gl), _ptr(gv), B, V, E, ctx.eps,
+                                              _stream_ptr(v.device))
+        _lib.check(rc, "umr_flatten_backward_deterministic" if ctx.det else "umr_flatten_backward")
+        return gv, None, None, None, None
 
 
 def dt_barrier(masks, k=50.0):
@@ -433,7 +522,10 @@ def load_textures(image, faces_uv, textures, is_update):
 class CorrChamferFunction(torch.autograd.Function):
     """verts [B,V,3] (or [1,V,3] / an expanded view: one mesh for all renders), cams [B,7], selection [NS] int32 (the four
     parts' vertex indices concatenated), targets = 4 tensors [B,m_g,2], part_ends (4 cumulative counts), weights (4 floats)
-    -> (loss [B], vert2d [B,NS,2]).  One kernel per direction instead of ~250 torch launches."""
+    -> (loss [B], vert2d [B,NS,2]).  One kernel per direction instead of ~250 torch launches.  `vert_rowptr` /
+    `vert_selection`: the selection's transposed table (`vertex_incidence(selection, V)` on the device) for the
+    deterministic backward; CorrLossChamfer caches it.  Without it a deterministic call builds it here (a device-to-host
+    copy of the selection)."""
 
     @staticmethod
     def _cfg(targets, part_ends, weights):
@@ -444,7 +536,7 @@ class CorrChamferFunction(torch.autograd.Function):
         return tp, tc, pe, wt
 
     @staticmethod
-    def forward(ctx, verts, cams, selection, t0, t1, t2, t3, part_ends, weights):
+    def forward(ctx, verts, cams, selection, t0, t1, t2, t3, part_ends, weights, vert_rowptr=None, vert_selection=None):
         _need_cuda(verts, cams, selection, t0, t1, t2, t3)
         lib = _lib.load()
         B = cams.shape[0]
@@ -468,7 +560,11 @@ class CorrChamferFunction(torch.autograd.Function):
             rc = lib.umr_corr_chamfer_forward(_ptr(vv), 0 if shared else V * 3, _ptr(cc), _ptr(sel), tp, tc, pe, wt, _ptr(vert2d),
                                               _ptr(nn), _ptr(loss), B, NS, _stream_ptr(vv.device))
         _lib.check(rc, "umr_corr_chamfer_forward")
+        ctx.det = torch.are_deterministic_algorithms_enabled()   # the forward has no atomics; the backward's mode
+        if ctx.det and (vert_rowptr is None or vert_selection is None):
+            vert_rowptr, vert_selection = _incidence_on(sel, V, vv.device)
         ctx.save_for_backward(vv, cc, sel, vert2d, nn, *targets)
+        ctx.vert_table = (vert_rowptr, vert_selection) if ctx.det else None   # constants of the loss module
         ctx.cfg = (tuple(int(e) for e in part_ends), tuple(float(w) for w in weights), shared, tuple(verts.shape))
         return loss, vert2d
 
@@ -485,17 +581,24 @@ class CorrChamferFunction(torch.autograd.Function):
             gverts = torch.empty(B, V, 3, device=vv.device, dtype=torch.float32) if ctx.needs_input_grad[0] else None
             gcams = torch.empty(B, 7, device=vv.device, dtype=torch.float32) if ctx.needs_input_grad[1] else None
             tp, tc, pe, wt = CorrChamferFunction._cfg(targets, part_ends, weights)
-            rc = lib.umr_corr_chamfer_backward(_ptr(vv), 0 if shared else V * 3, _ptr(cc), _ptr(sel), tp, tc, pe, wt, _ptr(vert2d),
-                                               _ptr(nn), _ptr(gl), _ptr(gv2), _ptr(gverts), _ptr(gcams), B, NS, V,
-                                               _stream_ptr(vv.device))
-        _lib.check(rc, "umr_corr_chamfer_backward")
+            if ctx.det:
+                rowptr, vsel = ctx.vert_table
+                ws = _workspace(lib.umr_corr_chamfer_workspace_bytes_deterministic(B, NS), vv.device)
+                rc = lib.umr_corr_chamfer_backward_deterministic(
+                    _ptr(vv), 0 if shared else V * 3, _ptr(cc), _ptr(sel), tp, tc, pe, wt, _ptr(vert2d), _ptr(nn), _ptr(gl),
+                    _ptr(gv2), _ptr(gverts), _ptr(gcams), B, NS, V, _ptr(rowptr), _ptr(vsel), _ptr(ws), _stream_ptr(vv.device))
+            else:
+                rc = lib.umr_corr_chamfer_backward(_ptr(vv), 0 if shared else V * 3, _ptr(cc), _ptr(sel), tp, tc, pe, wt,
+                                                   _ptr(vert2d), _ptr(nn), _ptr(gl), _ptr(gv2), _ptr(gverts), _ptr(gcams), B,
+                                                   NS, V, _stream_ptr(vv.device))
+        _lib.check(rc, "umr_corr_chamfer_backward_deterministic" if ctx.det else "umr_corr_chamfer_backward")
         if gverts is not None and shared and vshape[0] == 1:
             gverts = gverts.sum(0, keepdim=True)   # a [1,V,3] input broadcast here; an expanded [B,V,3] view gets the per-render
-        return (gverts, gcams) + (None,) * 7      # gradients and autograd's expand-backward sums them
+        return (gverts, gcams) + (None,) * 9      # gradients and autograd's expand-backward sums them
 
 
-def corr_chamfer(verts, cams, selection, targets, part_ends, weights):
-    return CorrChamferFunction.apply(verts, cams, selection, *targets, part_ends, weights)
+def corr_chamfer(verts, cams, selection, targets, part_ends, weights, vert_table=(None, None)):
+    return CorrChamferFunction.apply(verts, cams, selection, *targets, part_ends, weights, *vert_table)
 
 
 _VOXEL_DTYPES = {torch.float32: 0, torch.float64: 1}  # UMR_DTYPE_FLOAT32 / UMR_DTYPE_FLOAT64

@@ -69,6 +69,12 @@ class FlattenLoss(nn.Module):
         for name, v in (("v0s", v0), ("v1s", v1), ("v2s", v2), ("v3s", v3)):
             self.register_buffer(name, torch.tensor(v, dtype=torch.long))
         self.register_buffer("edge_table", torch.tensor(list(zip(v0, v1, v2, v3)), dtype=torch.int32).reshape(-1, 4))
+        # the edge table transposed (vertex -> ascending edge * 4 + role), for the deterministic backward's per-vertex
+        # gather under torch.use_deterministic_algorithms(True); not part of the state dict
+        from ..ops import vertex_incidence
+        rowptr, inc = vertex_incidence(self.edge_table.numpy(), int(f.max()) + 1 if f.size else 0)
+        self.register_buffer("vert_rowptr", torch.from_numpy(rowptr), persistent=False)
+        self.register_buffer("vert_incidence", torch.from_numpy(inc), persistent=False)
 
     @staticmethod
     def _perp(a, b, eps):
@@ -87,7 +93,7 @@ class FlattenLoss(nn.Module):
         batch_size = vertices.size(0)
         if vertices.is_cuda and vertices.dim() == 3:
             from .. import ops
-            loss = ops.FlattenFunction.apply(vertices, self.edge_table, eps)
+            loss = ops.FlattenFunction.apply(vertices, self.edge_table, eps, self.vert_rowptr, self.vert_incidence)
             return loss.sum() / batch_size if self.average else loss
         p0, p1 = vertices[:, self.v0s, :], vertices[:, self.v1s, :]
         p2, p3 = vertices[:, self.v2s, :], vertices[:, self.v3s, :]
