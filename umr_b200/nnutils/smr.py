@@ -141,6 +141,10 @@ class SoftRenderer(torch.nn.Module):
             if textures is not None and textures.shape[0] > 1:
                 textures = textures.repeat_interleave(cams.shape[0] // textures.shape[0], dim=0)
         faces = faces.int()
+        if faces.dim() == 2:
+            faces = faces[None]
+        if faces.shape[0] == 1 and cams.shape[0] > 1:  # one face list for every render, as the fused path accepts it
+            faces = faces.expand(cams.shape[0], -1, -1)
         verts = self.proj_fn(vertices, cams, offset_z=self.offset_z)
         if textures is not None:
             return Render(self.renderer)(verts, faces, textures)
