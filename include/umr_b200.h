@@ -451,6 +451,47 @@ int umr_corr_chamfer_backward_deterministic(const float* vertices, int64_t verti
                                             int32_t NS, int32_t V, const int32_t* vert_rowptr,
                                             const int32_t* vert_selection, void* workspace, void* stream);
 
+/* Deterministic backwards of the vertex pipeline, the NMR texture gradient and the sampler's image gradient (DESIGN.md §2),
+ * taken by vertex.ProjectFacesFunction, neural_renderer's _NmrFunction and ops.BilinearSampleFunction under
+ * torch.use_deterministic_algorithms(True).  Same guarantees as the loss kernels above: the default symbol's outputs,
+ * bitwise identical for identical inputs on the same device type and library build, no atomics reaching an output, no
+ * host synchronisation, a launch count that depends on the arguments only.  The transposed tables are "row -> ascending
+ * positions" tables (rowptr [R+1], positions), built on the device by umr_b200.ops.device_incidence.
+ *   - umr_project_faces_backward_deterministic: the arguments of umr_project_faces_backward, plus the faces' incidence
+ *     table and a workspace.  Positions are face * 3 + corner of the flattened faces: rows v over V vertices when the faces
+ *     are shared (faces_batch_stride == 0), rows vb * V + v over the Bv meshes otherwise, with positions vb * F * 3 +
+ *     face * 3 + corner.  An out-of-range face index must have no row (the builder drops it).  The per-(render, face,
+ *     corner) gradients, light term included, are stored to the workspace (zeros for a face with an out-of-range index);
+ *     grad_proj[b][v] is their sum in ascending table order; grad_vertices sums the per-render vertex terms in ascending
+ *     hypothesis (plain store when num_hypotheses <= 1); grad_cams keeps the default in-CTA tree, each CTA stores its
+ *     partial into a slot and the slots are summed in ascending CTA order.
+ *     Workspace: 4 * B * (9 * F + 3 * V + 7 * ceil(V / 256)) bytes.
+ *   - umr_nmr_backward_textures_deterministic: the arguments and workspace of umr_nmr_backward_textures.  One warp per
+ *     (texture group, face) gathers the face's texel gradients over the pixel boxes of its copies (DESIGN.md §3); a thin
+ *     or non-finite face is walked over the whole raster.
+ *   - umr_bilinear_sample_cells: one int32 cell key per sample (cells [B,N]): (y0+1) * (W+1) + (x0+1) + b * (H+1) * (W+1)
+ *     of the sample's top-left corner (x0, y0) as umr_bilinear_sample_backward computes it, or the drop key
+ *     B * (H+1) * (W+1) when none of its four corners is inside the image.  UMR_ERR_TOO_LARGE when B * (H+1) * (W+1)
+ *     exceeds INT32_MAX.
+ *   - umr_bilinear_sample_backward_deterministic: the arguments of umr_bilinear_sample_backward, plus the table of those
+ *     keys over R = B * (H+1) * (W+1) rows (cell_rowptr [R+1], cell_samples: flat sample indices b * N + n), NULL when
+ *     grad_image is.  grad_flow is the default kernel's; grad_image is fully written by a per-pixel gather (no zero-fill):
+ *     roles 00 of cell (y,x), 10 of (y,x-1), 01 of (y-1,x), 11 of (y-1,x-1), samples in ascending order within each. */
+size_t umr_project_faces_workspace_bytes_deterministic(int32_t B, int32_t V, int32_t F);
+int umr_project_faces_backward_deterministic(const float* vertices, const float* cams, const int32_t* faces,
+                                             const float* grad_face_vertices, const float* grad_light, float* grad_proj,
+                                             float* grad_vertices, float* grad_cams, const UmrProjectParams* params,
+                                             const int32_t* vert_rowptr, const int32_t* vert_incidence, void* workspace,
+                                             void* stream);
+int umr_nmr_backward_textures_deterministic(const float* vertices, const int32_t* faces, const int32_t* face_index,
+                                            const float* grad_rgb, float* grad_textures, const UmrNmrParams* params,
+                                            void* workspace, void* stream);
+int umr_bilinear_sample_cells(const float* flow, int32_t* cells, int32_t B, int32_t H, int32_t W, int32_t N, void* stream);
+int umr_bilinear_sample_backward_deterministic(const float* image, const float* flow, const float* grad_out,
+                                               float* grad_flow, float* grad_image, int32_t B, int32_t C, int32_t H,
+                                               int32_t W, int32_t N, const int32_t* cell_rowptr,
+                                               const int32_t* cell_samples, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,8 +1,11 @@
-"""Cost of the loss kernels' deterministic mode (torch.use_deterministic_algorithms(True)): the train_s2-shaped loss step of
+"""Cost of the deterministic mode (torch.use_deterministic_algorithms(True)): the train_s2-shaped loss step of
 tools/train_step_bench.py with the flag off and on, and every loss op that has a deterministic entry point, default vs
 deterministic, at the C2 / C3 batch shapes of BASELINE.md.  CUDA events after warm-up, one process; medians.
+--texture-renderer picks MultiTextureLoss's renderer (the soft rasteriser or the NMR z-buffer); --no-ops skips the
+per-op table.
 
-    CUBLAS_WORKSPACE_CONFIG=:4096:8 python tools/deterministic_step_bench.py [--iters 20] [--steps 10] [--out FILE.json]
+    python tools/deterministic_step_bench.py [--iters 20] [--steps 10] [--texture-renderer smr|nmr] [--no-ops]
+                                             [--out FILE.json]
 """
 import argparse
 import json
@@ -10,7 +13,7 @@ import os
 import subprocess
 import sys
 
-os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")  # the generic SoftRenderer chain's matmul under the flag
+os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")  # SoftRenderer's generic torch chain, where it falls back to it
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
@@ -84,7 +87,7 @@ def op_cases(B, S):
     }
 
 
-def make_step(B=16, H=8, IS=256, subdiv=3, T=6):
+def make_step(B=16, H=8, IS=256, subdiv=3, T=6, texture_renderer="smr"):
     """tools/train_step_bench.py's step: -> (step() returning the total loss after its backward)."""
     rng = np.random.default_rng(0)
     v, f = synth.icosphere(subdiv)
@@ -101,7 +104,7 @@ def make_step(B=16, H=8, IS=256, subdiv=3, T=6):
     head, belly, neck, back = [torch.from_numpy(p).to(DEV) for p in synth.part_points(rng, B)]
     rep = lambda t: t.unsqueeze(1).repeat(1, H, 1, 1).view(-1, t.size(1), t.size(2))
     mask_fn = loss_utils.MultiMaskLoss(IS, "softmax", H).to(DEV)
-    tex_fn = loss_utils.MultiTextureLoss(B, H, IS, "softmax", "l1", "smr").to(DEV)
+    tex_fn = loss_utils.MultiTextureLoss(B, H, IS, "softmax", "l1", texture_renderer).to(DEV)
     part_fn = loss_utils.part_matching_loss(None, None, 0, im_size=IS, batch_size=B, tex_size=T, stex_one_hot=one_hot).to(DEV)
     corr_fn = loss_utils.CorrLossChamfer(None, IS, part_vertices=part_vertices)
     fcpu = torch.from_numpy(f.astype(np.int64))
@@ -141,6 +144,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--texture-renderer", choices=("smr", "nmr"), default="smr")
+    ap.add_argument("--no-ops", action="store_true")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -148,7 +153,7 @@ def main():
     res = {"device": torch.cuda.get_device_name(0), "power_limit": power_limit(), "ops": {}}
     print("device: %s, power limit %s" % (res["device"], res["power_limit"]))
 
-    step = make_step()
+    step = make_step(texture_renderer=args.texture_renderer)
     row = {}
     for mode in ("default", "deterministic"):
         torch.use_deterministic_algorithms(mode == "deterministic")
@@ -171,12 +176,13 @@ def main():
         row[mode] = {"step_ms": float(np.median(ms)), "bitwise_equal": bool(equal)}
     torch.use_deterministic_algorithms(False)
     row["ratio"] = row["deterministic"]["step_ms"] / row["default"]["step_ms"]
+    row["texture_renderer"] = args.texture_renderer
     res["step"] = row
     print("train_s2-shaped step (16 x 8 hypotheses, 256^2, 1280 faces, T=6):", json.dumps(row))
     del step
     torch.cuda.empty_cache()
 
-    for shape, (B, S) in SIZES.items():
+    for shape, (B, S) in ({} if args.no_ops else SIZES).items():
         cases = op_cases(B, S)
         for name, fn in cases.items():
             r = {}

@@ -150,6 +150,14 @@ EXPORTS = {
                                                                c_f32p, ctypes.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p,
                                                                ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p,
                                                                ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
+    # deterministic vertex / NMR texture / sampler image backwards (+ the device-built transposed tables)
+    "umr_project_faces_workspace_bytes_deterministic": (ctypes.c_size_t, [ctypes.c_int32] * 3),
+    "umr_project_faces_backward_deterministic": (ctypes.c_int, [c_f32p] * 8 + [ctypes.POINTER(UmrProjectParams)] +
+                                                 [ctypes.c_void_p] * 4),
+    "umr_nmr_backward_textures_deterministic": (ctypes.c_int, [c_f32p] * 5 + [ctypes.POINTER(UmrNmrParams), ctypes.c_void_p,
+                                                                              ctypes.c_void_p]),
+    "umr_bilinear_sample_cells": (ctypes.c_int, [c_f32p, ctypes.c_void_p] + [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
+    "umr_bilinear_sample_backward_deterministic": (ctypes.c_int, [c_f32p] * 5 + [ctypes.c_int32] * 5 + [ctypes.c_void_p] * 3),
 }
 
 _lock = threading.Lock()

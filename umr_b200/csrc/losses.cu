@@ -93,6 +93,65 @@ __global__ void __launch_bounds__(256) k_sample_bwd(const float* __restrict__ im
     gflow[(size_t)b * N + n] = make_float2(gix * ((float)(W - 1) / 2.f), giy * ((float)(H - 1) / 2.f));
 }
 
+// Deterministic image gradient of the sampler.  Samples are keyed by the cell (y0, x0) of their top-left corner,
+// shifted by one so that every cell with an in-bounds corner is in [0, H] x [0, W]: key = b * (H+1)(W+1) +
+// (y0+1)(W+1) + (x0+1), from k_sample_bwd's own expressions (so a non-finite coordinate reaches the same pixels);
+// a sample with no in-bounds corner gets the drop key B * (H+1)(W+1).
+__global__ void __launch_bounds__(256) k_sample_cells(const float2* __restrict__ flow, int32_t* __restrict__ cells, int B,
+                                                      int H, int W, int N) {
+    const int n = blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.y;
+    if (n >= N) return;
+    const float2 xy = __ldg(flow + (size_t)b * N + n);
+    const float ix = ((xy.x + 1.f) / 2.f) * (float)(W - 1);
+    const float iy = ((xy.y + 1.f) / 2.f) * (float)(H - 1);
+    const float fx = floorf(ix), fy = floorf(iy);
+    const int x0 = (int)fx, y0 = (int)fy, x1 = x0 + 1, y1 = y0 + 1;
+    const bool any = inb(x0, y0, W, H) || inb(x1, y0, W, H) || inb(x0, y1, W, H) || inb(x1, y1, W, H);
+    const int cell = (H + 1) * (W + 1);
+    cells[(size_t)b * N + n] = any ? b * cell + (y0 + 1) * (W + 1) + (x0 + 1) : B * cell;
+}
+
+// grad_image[b][c][y][x], one thread per (image, pixel): the terms of the four roles the pixel plays, in the order
+// 00 of cell (y,x), 10 of cell (y,x-1), 01 of cell (y-1,x), 11 of cell (y-1,x-1); within a role the samples of the
+// cell table (rowptr [B(H+1)(W+1)+1], samples: flat sample indices b * N + n) in ascending order.  Each term is
+// k_sample_bwd's product, rounded as there.  A pixel no sample touches gets 0.
+template <int C>
+__global__ void __launch_bounds__(256) k_sample_bwd_image_gather(const float2* __restrict__ flow, const float* __restrict__ gout,
+                                                                 const int32_t* __restrict__ rowptr,
+                                                                 const int32_t* __restrict__ samples,
+                                                                 float* __restrict__ gimage, int H, int W) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.y;
+    if (p >= H * W) return;
+    const int y = p / W, x = p - y * W;
+    const size_t c0 = (size_t)b * (H + 1) * (W + 1);
+    const size_t cell[4] = {c0 + (size_t)(y + 1) * (W + 1) + (x + 1), c0 + (size_t)(y + 1) * (W + 1) + x,
+                            c0 + (size_t)y * (W + 1) + (x + 1), c0 + (size_t)y * (W + 1) + x};
+    float acc[C];
+#pragma unroll
+    for (int c = 0; c < C; ++c) acc[c] = 0.f;
+#pragma unroll
+    for (int role = 0; role < 4; ++role) {
+        const int k1 = __ldg(rowptr + cell[role] + 1);
+        for (int k = __ldg(rowptr + cell[role]); k < k1; ++k) {
+            const int s = __ldg(samples + k);
+            const float2 xy = __ldg(flow + s);
+            const float ix = ((xy.x + 1.f) / 2.f) * (float)(W - 1);
+            const float iy = ((xy.y + 1.f) / 2.f) * (float)(H - 1);
+            const float fx = floorf(ix), fy = floorf(iy);
+            const int x0 = (int)fx, y0 = (int)fy, x1 = x0 + 1, y1 = y0 + 1;
+            const float wx1 = (float)x1 - ix, wx0 = ix - (float)x0, wy1 = (float)y1 - iy, wy0 = iy - (float)y0;
+            const float wa = (role & 1) ? wx0 : wx1, wb = (role & 2) ? wy0 : wy1;
+            const float* go = gout + (size_t)s * C;
+#pragma unroll
+            for (int c = 0; c < C; ++c) acc[c] = __fadd_rn(acc[c], __fmul_rn(__fmul_rn(__ldg(go + c), wa), wb));
+        }
+    }
+#pragma unroll
+    for (int c = 0; c < C; ++c) gimage[((size_t)b * C + c) * H * W + p] = acc[c];
+}
+
 // ---------------------------------------------------------------------------------------------
 // IoU
 // ---------------------------------------------------------------------------------------------
@@ -876,4 +935,45 @@ extern "C" int umr_loss_head_forward_deterministic(const float* rgba, const floa
     k_losshead_sum_det<<<(3 * B + 127) / 128, 128, 0, st>>>(slots, stats, B, (int)gx);
     k_losshead_finalize<<<1, 32, 0, st>>>(stats, per_image, loss, B, 1.f / (3.f * (float)HW), w_iou, w_tex);
     return (int)cudaGetLastError();
+}
+
+// Sampler (include/umr_b200.h): grad_flow from k_sample_bwd itself (one writer per element, no image gradient there), the
+// image gradient from a per-pixel gather over the cell table.
+extern "C" int umr_bilinear_sample_cells(const float* flow, int32_t* cells, int32_t B, int32_t H, int32_t W, int32_t N,
+                                         void* stream_) {
+    if (!flow || !cells || B <= 0 || H <= 0 || W <= 0 || N <= 0) return UMR_ERR_BAD_ARG;
+    if (B > 65535 || (int64_t)B * ((int64_t)H + 1) * ((int64_t)W + 1) > INT_MAX) return UMR_ERR_TOO_LARGE;
+    count_launch(); k_sample_cells<<<dim3((N + 255) / 256, B), 256, 0, (cudaStream_t)stream_>>>(
+        reinterpret_cast<const float2*>(flow), cells, B, H, W, N);
+    UMR_RET_LAST();
+}
+extern "C" int umr_bilinear_sample_backward_deterministic(const float* image, const float* flow, const float* grad_out,
+                                                          float* grad_flow, float* grad_image, int32_t B, int32_t C, int32_t H,
+                                                          int32_t W, int32_t N, const int32_t* cell_rowptr,
+                                                          const int32_t* cell_samples, void* stream_) {
+    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0)
+        return UMR_ERR_BAD_ARG;
+    if (grad_image && (!cell_rowptr || !cell_samples)) return UMR_ERR_BAD_ARG;
+    if (B > 65535 || (int64_t)B * ((int64_t)H + 1) * ((int64_t)W + 1) > INT_MAX) return UMR_ERR_TOO_LARGE;
+    if (C < 1 || C > 4) return UMR_ERR_UNSUPPORTED;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const dim3 grid((N + 255) / 256, B), gpix((H * W + 255) / 256, B);
+    const float2* fl = reinterpret_cast<const float2*>(flow);
+    float2* gf = reinterpret_cast<float2*>(grad_flow);
+    count_launch(grad_image ? 2 : 1);
+    switch (C) {
+        case 1: k_sample_bwd<1><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, nullptr, H, W, N); break;
+        case 2: k_sample_bwd<2><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, nullptr, H, W, N); break;
+        case 3: k_sample_bwd<3><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, nullptr, H, W, N); break;
+        default: k_sample_bwd<4><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, nullptr, H, W, N); break;
+    }
+    if (grad_image) {
+        switch (C) {
+            case 1: k_sample_bwd_image_gather<1><<<gpix, 256, 0, st>>>(fl, grad_out, cell_rowptr, cell_samples, grad_image, H, W); break;
+            case 2: k_sample_bwd_image_gather<2><<<gpix, 256, 0, st>>>(fl, grad_out, cell_rowptr, cell_samples, grad_image, H, W); break;
+            case 3: k_sample_bwd_image_gather<3><<<gpix, 256, 0, st>>>(fl, grad_out, cell_rowptr, cell_samples, grad_image, H, W); break;
+            default: k_sample_bwd_image_gather<4><<<gpix, 256, 0, st>>>(fl, grad_out, cell_rowptr, cell_samples, grad_image, H, W); break;
+        }
+    }
+    UMR_RET_LAST();
 }

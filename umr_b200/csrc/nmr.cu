@@ -385,6 +385,84 @@ __global__ void __launch_bounds__(256) k_nmr_bwd_tex(const float* __restrict__ r
 }
 
 // ---------------------------------------------------------------------------------------------
+// deterministic texture gradient: a face-parallel gather.  One warp per (texture group, face f) is the only writer of
+// face f's texels.  It walks the group's G images in ascending order; in each, copy f and then (fill_back) copy F + f;
+// for each copy the pixel box of k_nmr_prep (the one k_nmr_zbuf tests, so it holds every pixel the copy can win) in
+// ascending rows, lanes over 32-pixel row segments.  A raster pixel the copy won contributes k_nmr_bwd_tex's terms.
+// Per corner, the lanes that hit one texel are summed in ascending lane order and the lowest of them adds the sum in.
+// ---------------------------------------------------------------------------------------------
+constexpr int DET_WARPS = 8;
+
+__global__ void __launch_bounds__(DET_WARPS * 32) k_nmr_bwd_tex_det(const float* __restrict__ rec, const int4* __restrict__ box,
+                                                                    const int32_t* __restrict__ face_index,
+                                                                    const float* __restrict__ grad_rgb,
+                                                                    float* __restrict__ grad_tex, Consts K) {
+    __shared__ float s_v[DET_WARPS][3][32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long gw = (long long)blockIdx.x * DET_WARPS + warp;
+    if (gw >= (long long)(K.B / K.tex_div) * K.F) return;  // whole warps
+    const int grp = (int)(gw / K.F), f = (int)(gw - (long long)grp * K.F);
+    const int T3 = K.T * K.T * K.T, IS = K.IS, S = K.S;
+    const size_t plane = (size_t)IS * IS;
+    float* gt = grad_tex + ((size_t)grp * K.F + f) * T3 * 3;
+    for (int i = 0; i < K.tex_div; ++i) {
+        const int b = grp * K.tex_div + i;
+        for (int fc = f; fc < K.Fc; fc += K.F) {
+            const int4 bb = __ldg(box + (size_t)b * K.Fc + fc);
+            const bool back = fc >= K.F;
+            const float* rc = rec + ((size_t)b * K.Fc + fc) * REC;
+            const float l0 = __ldg(rc + R_L), l1 = __ldg(rc + R_L + 1), l2 = __ldg(rc + R_L + 2);
+            for (int yi = bb.z; yi <= bb.w; ++yi) {
+                const int r = K.aa ? (S - 1 - yi) >> 1 : S - 1 - yi;
+                for (int xs = bb.x; xs <= bb.y; xs += 32) {
+                    const int xi = xs + lane;
+                    float g[3] = {0.f, 0.f, 0.f};
+                    bool hit = false;
+                    if (xi <= bb.y && __ldg(face_index + ((size_t)b * S + yi) * S + xi) == fc) {
+                        const size_t o = (size_t)r * IS + (K.aa ? xi >> 1 : xi);
+#pragma unroll
+                        for (int ch = 0; ch < 3; ++ch) g[ch] = __ldg(grad_rgb + ((size_t)b * 3 + ch) * plane + o);
+                        if (K.aa) { g[0] = g[0] / 4.f; g[1] = g[1] / 4.f; g[2] = g[2] / 4.f; }
+                        hit = !(g[0] == 0.f && g[1] == 0.f && g[2] == 0.f);
+                    }
+                    if (!__any_sync(0xffffffffu, hit)) continue;
+                    int idx[8];
+                    float wt[8];
+#pragma unroll
+                    for (int pn = 0; pn < 8; ++pn) { idx[pn] = -1; wt[pn] = 0.f; }
+                    if (hit) {
+                        float w[3], zp;
+                        bary(rc, xi, yi, w, zp);
+                        int pn = 0;
+                        corners(w, zp, rc, K.T, back, [&](int id, float wgt) { idx[pn] = id; wt[pn] = wgt; ++pn; });
+                    }
+#pragma unroll
+                    for (int pn = 0; pn < 8; ++pn) {
+                        const unsigned same = __match_any_sync(0xffffffffu, idx[pn]);
+                        s_v[warp][0][lane] = (l0 * wt[pn]) * g[0];
+                        s_v[warp][1][lane] = (l1 * wt[pn]) * g[1];
+                        s_v[warp][2][lane] = (l2 * wt[pn]) * g[2];
+                        __syncwarp();
+                        if (hit && lane == __ffs(same) - 1) {
+                            float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+                            for (unsigned m = same; m; m &= m - 1) {
+                                const int l = __ffs(m) - 1;
+                                a0 = a0 + s_v[warp][0][l];
+                                a1 = a1 + s_v[warp][1][l];
+                                a2 = a2 + s_v[warp][2][l];
+                            }
+                            float* t = gt + (size_t)idx[pn] * 3;
+                            t[0] = t[0] + a0; t[1] = t[1] + a1; t[2] = t[2] + a2;
+                        }
+                        __syncwarp();
+                    }
+                }
+            }
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
 static int check(const UmrNmrParams* p, bool need_tex) {
@@ -489,6 +567,31 @@ extern "C" int umr_nmr_backward_textures(const float* vertices, const int32_t* f
     launch_prep(vertices, faces, rec, box, K, stream);
     const size_t nthr = (size_t)K.B * K.IS * K.IS;
     k_nmr_bwd_tex<<<(unsigned)((nthr + 255) / 256), 256, 0, stream>>>(rec, face_index, grad_rgb, grad_textures, K);
+    umr::count_launch();
+    return (int)cudaGetLastError();
+}
+
+// Deterministic texture gradient (include/umr_b200.h): the default call's arguments and workspace; k_nmr_bwd_tex_det in
+// place of k_nmr_bwd_tex.
+extern "C" int umr_nmr_backward_textures_deterministic(const float* vertices, const int32_t* faces, const int32_t* face_index,
+                                                       const float* grad_rgb, float* grad_textures, const UmrNmrParams* p,
+                                                       void* workspace, void* stream_) {
+    int rc = check(p, true);
+    if (rc) return rc;
+    if (!vertices || !faces || !face_index || !grad_rgb || !grad_textures || !workspace) return UMR_ERR_BAD_ARG;
+    if (((uintptr_t)workspace & 255) != 0 || ((uintptr_t)grad_textures & 3) != 0) return UMR_ERR_BAD_ARG;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const Consts K = make_consts(p);
+    const size_t gbytes = (size_t)(K.B / K.tex_div) * K.F * K.T * K.T * K.T * 3 * sizeof(float);
+    cudaError_t e = cudaMemsetAsync(grad_textures, 0, gbytes, stream);
+    if (e != cudaSuccess) return (int)e;
+    char* ws = (char*)workspace;
+    float* rec = (float*)ws;
+    int4* box = (int4*)(ws + rec_bytes(K.B, K.Fc));
+    launch_prep(vertices, faces, rec, box, K, stream);
+    const long long nwarp = (long long)(K.B / K.tex_div) * K.F;
+    k_nmr_bwd_tex_det<<<(unsigned)((nwarp + DET_WARPS - 1) / DET_WARPS), DET_WARPS * 32, 0, stream>>>(rec, box, face_index,
+                                                                                                      grad_rgb, grad_textures, K);
     umr::count_launch();
     return (int)cudaGetLastError();
 }

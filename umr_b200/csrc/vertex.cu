@@ -123,6 +123,9 @@ __global__ void __launch_bounds__(256) k_project_faces(const float* __restrict__
 }
 
 // backward A: per face -> add d(light)/d(corners) to the corner gradients, scatter to gproj[B,V,3]
+// DET: `gproj` is the per-(render, face, corner) term array [B,F,3,3] (plain stores, zeros for a face with an index
+// outside [0, V)), summed per vertex by k_vertex_gather.
+template <bool DET>
 __global__ void __launch_bounds__(256) k_scatter_face_grads(const float* __restrict__ verts, const float* __restrict__ cams,
                                                             const int32_t* __restrict__ faces, const float* __restrict__ gfv,
                                                             const float* __restrict__ glight, float* __restrict__ gproj,
@@ -136,7 +139,14 @@ __global__ void __launch_bounds__(256) k_scatter_face_grads(const float* __restr
 #pragma unroll
     for (int c = 0; c < 3; ++c) vid[c] = __ldg(fi + c);
     // face with an index outside [0, V) (forward wrote NaN for it): never write out of bounds
-    if ((unsigned)vid[0] >= (unsigned)V || (unsigned)vid[1] >= (unsigned)V || (unsigned)vid[2] >= (unsigned)V) return;
+    if ((unsigned)vid[0] >= (unsigned)V || (unsigned)vid[1] >= (unsigned)V || (unsigned)vid[2] >= (unsigned)V) {
+        if (DET) {
+            float* q = gproj + ((size_t)b * F + f) * 9;
+#pragma unroll
+            for (int i = 0; i < 9; ++i) q[i] = 0.f;
+        }
+        return;
+    }
     float g[9];
     const float* gi = gfv + ((size_t)b * F + f) * 9;
     // d/d(pre) of out: x,y scaled by view_scale, z unchanged
@@ -183,16 +193,25 @@ __global__ void __launch_bounds__(256) k_scatter_face_grads(const float* __restr
             }
         }
     }
+    if (DET) {
+        float* q = gproj + ((size_t)b * F + f) * 9;
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        float* q = gproj + ((size_t)b * V + vid[c]) * 3;
-        atomicAdd(q + 0, g[3 * c + 0]);
-        atomicAdd(q + 1, g[3 * c + 1]);
-        atomicAdd(q + 2, g[3 * c + 2]);
+        for (int i = 0; i < 9; ++i) q[i] = g[i];
+    } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            float* q = gproj + ((size_t)b * V + vid[c]) * 3;
+            atomicAdd(q + 0, g[3 * c + 0]);
+            atomicAdd(q + 1, g[3 * c + 1]);
+            atomicAdd(q + 2, g[3 * c + 2]);
+        }
     }
 }
 
 // backward B: per vertex -> grad_vertices (direct store) and grad_cams (block reduce + 7 atomics)
+// DET: `gverts` is indexed by render (the per-render term array [B,V,3] when H > 1, summed by k_hypothesis_sum), and
+// `gcams` is the slot array [B][gridDim.x][7]: each CTA stores its partial, k_cam_finalize sums the slots.
+template <bool DET>
 __global__ void __launch_bounds__(256) k_project_backward(const float* __restrict__ verts, const float* __restrict__ cams,
                                                           const float* __restrict__ gproj, float* __restrict__ gverts,
                                                           float* __restrict__ gcams, int V, int H, ProjCfg pc) {
@@ -225,11 +244,11 @@ __global__ void __launch_bounds__(256) k_project_backward(const float* __restric
         const float c0 = q0 * q0 - vv;
         const float cx = vy * Gz - vz * Gy, cy = vz * Gx - vx * Gz, cz = vx * Gy - vy * Gx;  // v x G
         if (gverts != nullptr) {
-            float* o = gverts + ((size_t)vb * V + v) * 3;
+            float* o = gverts + ((size_t)(DET ? b : vb) * V + v) * 3;
             const float o0 = c0 * Gx + 2.f * vG * vx - 2.f * q0 * cx;
             const float o1 = c0 * Gy + 2.f * vG * vy - 2.f * q0 * cy;
             const float o2 = c0 * Gz + 2.f * vG * vz - 2.f * q0 * cz;
-            if (H == 1) { o[0] = o0; o[1] = o1; o[2] = o2; }
+            if (DET || H == 1) { o[0] = o0; o[1] = o1; o[2] = o2; }
             else { atomicAdd(o, o0); atomicAdd(o + 1, o1); atomicAdd(o + 2, o2); }  // sum over the hypotheses (zero-filled by the host)
         }
         // dL/dq0 = G . (2 q0 X + 2 (v x X))
@@ -253,8 +272,59 @@ __global__ void __launch_bounds__(256) k_project_backward(const float* __restric
     if (threadIdx.x < 7) {
         float r = 0.f;
         for (int w = 0; w < (int)(blockDim.x >> 5); ++w) r += s[w][threadIdx.x];
-        atomicAdd(gcams + (size_t)b * 7 + threadIdx.x, r);
+        if (DET) gcams[((size_t)b * gridDim.x + blockIdx.x) * 7 + threadIdx.x] = r;
+        else atomicAdd(gcams + (size_t)b * 7 + threadIdx.x, r);
     }
+}
+
+// Deterministic backward, per-vertex sums of k_scatter_face_grads<true>'s corner terms: gproj[b][v] = the terms of v's
+// incidence entries in render b, added in ascending table order.  The table lists positions face * 3 + corner of the
+// flattened faces: rows v over V vertices when the faces are shared, rows vb * V + v over the Bv meshes otherwise (their
+// positions then lie in mesh vb's [vb * F * 3, (vb + 1) * F * 3)).
+__global__ void __launch_bounds__(256) k_vertex_gather(const float* __restrict__ terms, const int32_t* __restrict__ rowptr,
+                                                       const int32_t* __restrict__ incidence, float* __restrict__ gproj,
+                                                       int V, int F, int H, int batched) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.y;
+    if (v >= V) return;
+    const int vb = b / H;
+    const size_t row = batched ? (size_t)vb * V + v : (size_t)v;
+    const int64_t base = batched ? (int64_t)vb * F * 3 : 0;
+    const float* tb = terms + (size_t)b * F * 9;
+    float g0 = 0.f, g1 = 0.f, g2 = 0.f;
+    const int k1 = __ldg(rowptr + row + 1);
+    for (int k = __ldg(rowptr + row); k < k1; ++k) {
+        const float* t = tb + (size_t)(__ldg(incidence + k) - base) * 3;
+        g0 += t[0]; g1 += t[1]; g2 += t[2];
+    }
+    float* o = gproj + ((size_t)b * V + v) * 3;
+    o[0] = g0; o[1] = g1; o[2] = g2;
+}
+
+// gverts[vb][v] = the per-render terms [B,V,3] of the H hypotheses of mesh vb, added in ascending h
+__global__ void __launch_bounds__(256) k_hypothesis_sum(const float* __restrict__ terms, float* __restrict__ gverts, int V,
+                                                        int H) {
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    const int vb = blockIdx.y;
+    if (v >= V) return;
+    float g0 = 0.f, g1 = 0.f, g2 = 0.f;
+    for (int h = 0; h < H; ++h) {
+        const float* t = terms + ((size_t)(vb * H + h) * V + v) * 3;
+        g0 += t[0]; g1 += t[1]; g2 += t[2];
+    }
+    float* o = gverts + ((size_t)vb * V + v) * 3;
+    o[0] = g0; o[1] = g1; o[2] = g2;
+}
+
+// gcams[b][i] = render b's CTA slots [nslot][7] added in ascending CTA order
+__global__ void k_cam_finalize(const float* __restrict__ slots, float* __restrict__ gcams, int B, int nslot) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= B * 7) return;
+    const int b = t / 7, i = t - b * 7;
+    const float* s = slots + (size_t)b * nslot * 7 + i;
+    float r = 0.f;
+    for (int w = 0; w < nslot; ++w) r += s[(size_t)w * 7];
+    gcams[t] = r;
 }
 
 
@@ -471,11 +541,50 @@ extern "C" int umr_project_faces_backward(const float* vertices, const float* ca
         if (e != cudaSuccess) return (int)e;
     }
     count_launch(2);
-    k_scatter_face_grads<<<dim3((F + 255) / 256, B), 256, 0, st>>>(vertices, cams, faces, grad_face_vertices, grad_light,
-                                                                   grad_proj, V, F, H, p->faces_batch_stride, make_pc(p),
-                                                                   make_lc(p));
-    k_project_backward<<<dim3((V + 255) / 256, B), 256, 0, st>>>(vertices, cams, grad_proj, grad_vertices, grad_cams, V, H,
-                                                                 make_pc(p));
+    k_scatter_face_grads<false><<<dim3((F + 255) / 256, B), 256, 0, st>>>(vertices, cams, faces, grad_face_vertices,
+                                                                          grad_light, grad_proj, V, F, H,
+                                                                          p->faces_batch_stride, make_pc(p), make_lc(p));
+    k_project_backward<false><<<dim3((V + 255) / 256, B), 256, 0, st>>>(vertices, cams, grad_proj, grad_vertices, grad_cams,
+                                                                        V, H, make_pc(p));
+    return (int)cudaGetLastError();
+}
+
+// Deterministic backward (include/umr_b200.h): corner terms to the workspace, a per-vertex gather over the caller's
+// incidence table, the default projection backward with per-render vertex terms and per-CTA camera slots, then the
+// ascending sums over the hypotheses and the slots.  Workspace: terms [B,F,9] | vertex terms [B,V,3] | slots
+// [B][ceil(V/256)][7], all float.
+extern "C" size_t umr_project_faces_workspace_bytes_deterministic(int32_t B, int32_t V, int32_t F) {
+    if (B <= 0 || V <= 0 || F <= 0) return 0;
+    return (size_t)B * (9 * (size_t)F + 3 * (size_t)V + 7 * (size_t)((V + 255) / 256)) * sizeof(float);
+}
+extern "C" int umr_project_faces_backward_deterministic(const float* vertices, const float* cams, const int32_t* faces,
+                                                        const float* grad_face_vertices, const float* grad_light,
+                                                        float* grad_proj, float* grad_vertices, float* grad_cams,
+                                                        const UmrProjectParams* p, const int32_t* vert_rowptr,
+                                                        const int32_t* vert_incidence, void* workspace, void* stream_) {
+    if (!vertices || !cams || !faces || !grad_face_vertices || !grad_proj || !p) return UMR_ERR_BAD_ARG;
+    if (!vert_rowptr || !vert_incidence || !workspace) return UMR_ERR_BAD_ARG;
+    if (p->batch_size <= 0 || p->num_vertices <= 0 || p->num_faces <= 0) return UMR_ERR_BAD_ARG;
+    if (p->batch_size > 65535) return UMR_ERR_TOO_LARGE;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const int B = p->batch_size, V = p->num_vertices, F = p->num_faces;
+    const int H = p->num_hypotheses > 1 ? p->num_hypotheses : 1;
+    if (B % H != 0) return UMR_ERR_BAD_ARG;
+    const unsigned nslot = (unsigned)((V + 255) / 256);
+    float* terms = (float*)workspace;
+    float* vterms = terms + (size_t)B * F * 9;
+    float* slots = vterms + (size_t)B * V * 3;
+    float* gv = (grad_vertices && H > 1) ? vterms : grad_vertices;
+    count_launch(3 + (grad_vertices && H > 1 ? 1 : 0) + (grad_cams ? 1 : 0));
+    k_scatter_face_grads<true><<<dim3((F + 255) / 256, B), 256, 0, st>>>(vertices, cams, faces, grad_face_vertices, grad_light,
+                                                                         terms, V, F, H, p->faces_batch_stride, make_pc(p),
+                                                                         make_lc(p));
+    k_vertex_gather<<<dim3(nslot, B), 256, 0, st>>>(terms, vert_rowptr, vert_incidence, grad_proj, V, F, H,
+                                                    p->faces_batch_stride != 0 ? 1 : 0);
+    k_project_backward<true><<<dim3(nslot, B), 256, 0, st>>>(vertices, cams, grad_proj, gv, grad_cams ? slots : nullptr, V, H,
+                                                             make_pc(p));
+    if (grad_vertices && H > 1) k_hypothesis_sum<<<dim3(nslot, B / H), 256, 0, st>>>(vterms, grad_vertices, V, H);
+    if (grad_cams) k_cam_finalize<<<(B * 7 + 255) / 256, 256, 0, st>>>(slots, grad_cams, B, (int)nslot);
     return (int)cudaGetLastError();
 }
 

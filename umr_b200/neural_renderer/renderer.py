@@ -15,7 +15,9 @@ _NO_VERTEX_GRAD = (
 
 
 class _NmrFunction(torch.autograd.Function):
-    """(textures | None, vertices, faces) -> (rgb | None, alpha | None, depth | None); gradient for textures only."""
+    """(textures | None, vertices, faces) -> (rgb | None, alpha | None, depth | None); gradient for textures only.
+    Under torch.use_deterministic_algorithms(True), read once in `forward`, the texture gradient is the bitwise
+    reproducible face-parallel gather (umr_nmr_backward_textures_deterministic)."""
 
     @staticmethod
     def forward(ctx, textures, vertices, faces, params, want_rgb, want_alpha, want_depth):
@@ -35,6 +37,7 @@ class _NmrFunction(torch.autograd.Function):
                                      _ptr(alpha), _ptr(depth), ctypes.byref(params), _ptr(ws), _stream_ptr(dev))
         _lib.check(rc, "umr_nmr_forward")
         ctx.params = params
+        ctx.det = torch.are_deterministic_algorithms_enabled()   # the forward has no atomics; the backward's mode
         ctx.tex_shape = None if textures is None else textures.shape
         ctx.save_for_backward(vertices, faces, fidx)
         for t in (alpha, depth):
@@ -55,9 +58,10 @@ class _NmrFunction(torch.autograd.Function):
             ws = torch.empty(lib.umr_nmr_workspace_bytes(p.batch_size, p.num_faces, p.fill_back), device=dev,
                              dtype=torch.uint8)
             grad_tex = torch.empty(ctx.tex_shape, device=dev, dtype=torch.float32)
-            rc = lib.umr_nmr_backward_textures(_ptr(vertices), _ptr(faces), _ptr(fidx), _ptr(g), _ptr(grad_tex),
-                                               ctypes.byref(p), _ptr(ws), _stream_ptr(dev))
-        _lib.check(rc, "umr_nmr_backward_textures")
+            bwd = lib.umr_nmr_backward_textures_deterministic if ctx.det else lib.umr_nmr_backward_textures
+            rc = bwd(_ptr(vertices), _ptr(faces), _ptr(fidx), _ptr(g), _ptr(grad_tex), ctypes.byref(p), _ptr(ws),
+                     _stream_ptr(dev))
+        _lib.check(rc, "umr_nmr_backward_textures_deterministic" if ctx.det else "umr_nmr_backward_textures")
         return (grad_tex,) + (None,) * 6
 
 

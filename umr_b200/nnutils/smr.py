@@ -53,10 +53,9 @@ class SoftRenderer(torch.nn.Module):
     fuse_vertex_pipeline = True  # class-level switch (tests compare both paths)
 
     def _fusable(self, vertices):
-        """True when forward() takes the fused vertex kernel.  Not under torch.use_deterministic_algorithms(True): its
-        backward scatters with float atomics, while the generic torch chain computes the same forward and differentiates
-        deterministically (its look_at matmul needs CUBLAS_WORKSPACE_CONFIG, README)."""
-        return self._projectable(vertices) and not torch.are_deterministic_algorithms_enabled()
+        """True when forward() takes the fused vertex kernel.  Under torch.use_deterministic_algorithms(True) too: its
+        backward then takes the deterministic gather (vertex.ProjectFacesFunction)."""
+        return self._projectable(vertices)
 
     def _projectable(self, vertices):
         """The fused vertex kernel covers exactly the configuration this wrapper sets up (smr.py:56-66):

@@ -40,6 +40,22 @@ def vertex_incidence(index, num_vertices):
     return rowptr.astype(np.int32), positions
 
 
+def device_incidence(keys, rows):
+    """The same transposed table, built on the keys' device: keys (any shape, integer) -> (rowptr [rows+1],
+    positions [keys.numel()]) int32 tensors, where positions[rowptr[r]:rowptr[r+1]] are the flat positions k with
+    keys.flat[k] == r in ascending order.  Keys outside [0, rows) are dropped: they sort past the last row, so they sit
+    after rowptr[rows].  Torch ops only (a stable sort and a searchsorted), which are deterministic, need no host
+    synchronisation and can be captured in a CUDA graph.  Used by the deterministic backwards of the vertex pipeline
+    (vertex -> face corners) and of the sampler's image gradient (pixel cell -> samples)."""
+    flat = keys.reshape(-1).long()
+    if flat.numel() > 2 ** 31 - 1 or rows > 2 ** 31 - 2:
+        raise ValueError("device_incidence: %d positions over %d rows do not fit int32" % (flat.numel(), rows))
+    flat = flat.masked_fill((flat < 0) | (flat >= rows), rows)
+    sorted_keys, positions = torch.sort(flat, stable=True)
+    rowptr = torch.searchsorted(sorted_keys, torch.arange(rows + 1, device=flat.device, dtype=torch.int64))
+    return rowptr.to(torch.int32), positions.to(torch.int32)
+
+
 def _incidence_on(index, num_vertices, device):
     rowptr, pos = vertex_incidence(index.detach().cpu().numpy(), num_vertices)
     return torch.from_numpy(rowptr).to(device), torch.from_numpy(pos).to(device)
@@ -76,6 +92,7 @@ class BilinearSampleFunction(torch.autograd.Function):
         _lib.check(rc, "umr_bilinear_sample_forward")
         ctx.save_for_backward(img, fl)
         ctx.img_grad = images.requires_grad
+        ctx.det = torch.are_deterministic_algorithms_enabled()   # the forward has no atomics; the backward's mode
         return out
 
     @staticmethod
@@ -88,9 +105,20 @@ class BilinearSampleFunction(torch.autograd.Function):
         with torch.cuda.device(img.device):
             gflow = torch.empty_like(fl)
             gimg = torch.empty_like(img) if ctx.img_grad else None
-            rc = lib.umr_bilinear_sample_backward(_ptr(img), _ptr(fl), _ptr(g), _ptr(gflow), _ptr(gimg),
-                                                  B, C, H, W, N, _stream_ptr(img.device))
-        _lib.check(rc, "umr_bilinear_sample_backward")
+            if ctx.det:
+                rowptr = samples = None
+                if gimg is not None:   # samples keyed by their top-left cell, then the cell -> samples table
+                    cells = torch.empty(B, N, device=img.device, dtype=torch.int32)
+                    _lib.check(lib.umr_bilinear_sample_cells(_ptr(fl), _ptr(cells), B, H, W, N, _stream_ptr(img.device)),
+                               "umr_bilinear_sample_cells")
+                    rowptr, samples = device_incidence(cells, B * (H + 1) * (W + 1))
+                rc = lib.umr_bilinear_sample_backward_deterministic(_ptr(img), _ptr(fl), _ptr(g), _ptr(gflow), _ptr(gimg),
+                                                                    B, C, H, W, N, _ptr(rowptr), _ptr(samples),
+                                                                    _stream_ptr(img.device))
+            else:
+                rc = lib.umr_bilinear_sample_backward(_ptr(img), _ptr(fl), _ptr(g), _ptr(gflow), _ptr(gimg),
+                                                      B, C, H, W, N, _stream_ptr(img.device))
+        _lib.check(rc, "umr_bilinear_sample_backward_deterministic" if ctx.det else "umr_bilinear_sample_backward")
         return gimg, gflow
 
 

@@ -2,12 +2,16 @@
 
 project_faces(vertices, cams, faces, ...) = orthographic_proj_withz -> y flip -> look_at(eye on z)
 -> orthogonal -> face gather [-> per-face surface light], one kernel forward and two backward,
-replacing ~70 tiny torch launches per render of the reference host path (SURVEY.md §8f-1)."""
+replacing ~70 tiny torch launches per render of the reference host path (SURVEY.md §8f-1).
+
+Under torch.use_deterministic_algorithms(True) (read once in `forward`, kept in `ctx`) the backward takes
+umr_project_faces_backward_deterministic: a gather over the faces' vertex -> corner table instead of float atomics."""
 import ctypes
 
 import torch
 
 from . import _lib
+from .ops import device_incidence
 from .raster import _ptr, _stream_ptr
 
 
@@ -29,6 +33,19 @@ def make_project_params(B, V, F, faces_bstride, offset_z, eye_z, viewing_scale, 
             p.light_color_directional[k] = float(cd[k])
             p.light_direction[k] = float(d[k])
     return p
+
+
+def _corner_incidence(faces, V, batched):
+    """vertex -> (face * 3 + corner) table of the deterministic backward (include/umr_b200.h): rows v over V vertices for
+    one shared face list, rows vb * V + v over the meshes of batched faces [Bv,F,3].  A face index outside [0, V) has no
+    row: the kernel stores zeros for such a face, and in a batched list it must not land in another mesh's rows."""
+    if not batched:
+        return device_incidence(faces, V)
+    Bv = faces.shape[0]
+    idx = faces.long()
+    keys = (idx + torch.arange(Bv, device=faces.device, dtype=torch.int64).view(Bv, 1, 1) * V).masked_fill(
+        (idx < 0) | (idx >= V), -1)
+    return device_incidence(keys, Bv * V)
 
 
 class ProjectFacesFunction(torch.autograd.Function):
@@ -63,6 +80,7 @@ class ProjectFacesFunction(torch.autograd.Function):
         ctx.save_for_backward(v, c, f)
         ctx.needs = (vertices.requires_grad, cams.requires_grad)
         ctx.has_light = light is not None
+        ctx.det = torch.are_deterministic_algorithms_enabled()   # the forward has no atomics; the backward's mode
         if lt is None:
             lt = fv.new_empty(0)
             ctx.mark_non_differentiable(lt)
@@ -83,9 +101,17 @@ class ProjectFacesFunction(torch.autograd.Function):
             gproj = torch.empty(B, V, 3, device=dev, dtype=torch.float32)
             gv = torch.empty_like(v) if ctx.needs[0] else None
             gc = torch.empty_like(c) if ctx.needs[1] else None
-            rc = lib.umr_project_faces_backward(_ptr(v), _ptr(c), _ptr(f), _ptr(g), _ptr(gl), _ptr(gproj), _ptr(gv),
-                                                _ptr(gc), ctypes.byref(ctx.params), _stream_ptr(dev))
-        _lib.check(rc, "umr_project_faces_backward")
+            if ctx.det:
+                rowptr, inc = _corner_incidence(f, V, ctx.params.faces_batch_stride != 0)
+                ws = torch.empty(lib.umr_project_faces_workspace_bytes_deterministic(B, V, ctx.params.num_faces), device=dev,
+                                 dtype=torch.uint8)
+                rc = lib.umr_project_faces_backward_deterministic(_ptr(v), _ptr(c), _ptr(f), _ptr(g), _ptr(gl), _ptr(gproj),
+                                                                  _ptr(gv), _ptr(gc), ctypes.byref(ctx.params), _ptr(rowptr),
+                                                                  _ptr(inc), _ptr(ws), _stream_ptr(dev))
+            else:
+                rc = lib.umr_project_faces_backward(_ptr(v), _ptr(c), _ptr(f), _ptr(g), _ptr(gl), _ptr(gproj), _ptr(gv),
+                                                    _ptr(gc), ctypes.byref(ctx.params), _stream_ptr(dev))
+        _lib.check(rc, "umr_project_faces_backward_deterministic" if ctx.det else "umr_project_faces_backward")
         return gv, gc, None, None, None, None, None, None
 
 
