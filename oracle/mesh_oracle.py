@@ -79,13 +79,16 @@ def load_textures_np(image, faces_uv, is_update, textures):
     wx0 = (f32(1) - wx1).astype(f32)
     wy1 = (pos_y - iy.astype(f32)).astype(f32)
     wy0 = (f32(1) - wy1).astype(f32)
+    # the four corners clamped into the image (the reference reads outside it at uv = 1 and uv < 0; DESIGN.md §2)
+    x0, x1 = np.clip(ix, 0, W - 1), np.clip(ix + 1, 0, W - 1)
+    y0, y1 = np.clip(iy, 0, H - 1), np.clip(iy1, 0, H - 1)
     flat = out.reshape(-1, 3)
     upd = np.asarray(is_update)[fn] != 0
     c = np.zeros((F_ * RR, 3), f32)
-    c = (c + image[iy, ix] * (wx0 * wy0)[:, None]).astype(f32)
-    c = (c + image[iy1, ix] * (wx0 * wy1)[:, None]).astype(f32)
-    c = (c + image[iy, ix + 1] * (wx1 * wy0)[:, None]).astype(f32)
-    c = (c + image[iy1, ix + 1] * (wx1 * wy1)[:, None]).astype(f32)
+    c = (c + image[y0, x0] * (wx0 * wy0)[:, None]).astype(f32)
+    c = (c + image[y1, x0] * (wx0 * wy1)[:, None]).astype(f32)
+    c = (c + image[y0, x1] * (wx1 * wy0)[:, None]).astype(f32)
+    c = (c + image[y1, x1] * (wx1 * wy1)[:, None]).astype(f32)
     flat[upd] = c[upd]
     return flat.reshape(F_, RR, 3)
 

@@ -41,7 +41,11 @@ def test_load_textures_bit_exact(F, R, H, W):
     rng = np.random.default_rng(R)
     image = rng.uniform(0, 1, size=(H, W, 3)).astype(np.float32)
     uv = rng.uniform(0.02, 0.95, size=(F, 3, 2)).astype(np.float32)
+    # the edges of the uv range (whole faces on u or v = 0 or 1, negative uv): the kernel clamps its corners there
+    uv[:4] = np.float32([[[0, 1], [0.5, 1], [1, 1]], [[1, 0], [1, 0.3], [1, 1]], [[0, 0], [0, 0], [0, 0]],
+                         [[-0.4, -1.2], [-0.1, 0.5], [0.2, -0.3]]])
     upd = (rng.uniform(size=F) > 0.3).astype(np.int32)
+    upd[:4] = 1
     base = rng.uniform(0, 1, size=(F, R * R, 3)).astype(np.float32)
     got = ops.load_textures(torch.from_numpy(image).to(DEV), torch.from_numpy(uv).to(DEV), torch.from_numpy(base.copy()).to(DEV),
                             torch.from_numpy(upd).to(DEV)).cpu().numpy()

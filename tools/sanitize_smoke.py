@@ -91,6 +91,11 @@ def main():
     assert torch.isfinite(dtb).all()
     atlas, _ = sr.functional.create_texture_image(tex[0].detach(), 8)
     assert np.isfinite(atlas).all()
+    # texture reload at the edges of the uv range (whole faces on u or v = 1, negative uv): corners clamped to the image
+    uv_edge = torch.tensor([[[1.0, 1.0]] * 3, [[1.0, 0.0], [1.0, 0.5], [1.0, 1.0]], [[-0.5, -1.0]] * 3], device=dev)
+    tex_edge = ops.load_textures(torch.rand(5, 4, 3, device=dev), uv_edge, torch.zeros(3, 9, 3, device=dev),
+                                 torch.ones(3, dtype=torch.int32, device=dev))
+    assert torch.isfinite(tex_edge).all()
     total.backward()
     torch.cuda.synchronize()
     assert torch.isfinite(verts.grad).all() and torch.isfinite(cams.grad).all() and torch.isfinite(flow.grad).all()

@@ -87,14 +87,19 @@ __global__ void __launch_bounds__(256) k_load_textures(const float* __restrict__
     const float wx1 = pos_x - (int)pos_x, wx0 = 1 - wx1;
     const float wy1 = pos_y - (int)pos_y, wy0 = 1 - wy1;
     const int ix = (int)pos_x, iy = (int)pos_y, iy1 = (int)(pos_y + 1);
+    // The reference reads these four corners unclamped: uv = 1 on a whole face puts ix + 1 = W or iy1 = H (with weight
+    // 0), negative uv puts them below 0, and (int)(pos_y + 1) can skip to H when pos_y lies just below H - 1.  Clamped
+    // into the image here (DESIGN.md §2); a texel whose corners are all inside computes the reference's bits.
+    const int x0 = min(max(ix, 0), image_width - 1), x1 = max(min(ix, image_width - 2) + 1, 0);
+    const int y0 = min(max(iy, 0), image_height - 1), y1 = min(max(iy1, 0), image_height - 1);
     float* texture = textures + i * 3;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         float c = 0.f;
-        c += image[((size_t)iy * image_width + ix) * 3 + k] * (wx0 * wy0);
-        c += image[((size_t)iy1 * image_width + ix) * 3 + k] * (wx0 * wy1);
-        c += image[((size_t)iy * image_width + ix + 1) * 3 + k] * (wx1 * wy0);
-        c += image[((size_t)iy1 * image_width + ix + 1) * 3 + k] * (wx1 * wy1);
+        c += image[((size_t)y0 * image_width + x0) * 3 + k] * (wx0 * wy0);
+        c += image[((size_t)y1 * image_width + x0) * 3 + k] * (wx0 * wy1);
+        c += image[((size_t)y0 * image_width + x1) * 3 + k] * (wx1 * wy0);
+        c += image[((size_t)y1 * image_width + x1) * 3 + k] * (wx1 * wy1);
         texture[k] = c;
     }
 }
@@ -308,7 +313,9 @@ __global__ void __launch_bounds__(256) k_flatten_gather(const float* __restrict_
 // exact Euclidean distance transform + barrier sigmoid (utils/image.py:130-141)
 //   pass 1 (per column): g(y, x) = distance along the column to the nearest FEATURE pixel (inf if none)
 //   pass 2 (per row):    d^2(y, x) = min_x' (x - x')^2 + g(y, x')^2      -- exact integers
-// run for feature = (mask != 0) [dist_out: distance of outside pixels to the object] and feature = (mask == 0) [dist_in]
+// run for feature = (mask == 1) [dist_out = edt(1 - mask): distance to the object] and feature = (mask == 0) [dist_in =
+// edt(mask)].  On a binary mask the two are complements; a value strictly between (the bilinear edge of a resized mask)
+// is a feature of neither, as in scipy.
 // ---------------------------------------------------------------------------------------------
 constexpr int EDT_INF = 1 << 28;
 __global__ void __launch_bounds__(256) k_edt_columns(const float* __restrict__ mask, int32_t* __restrict__ g_out,
@@ -321,17 +328,19 @@ __global__ void __launch_bounds__(256) k_edt_columns(const float* __restrict__ m
     int32_t* gi = g_in + (size_t)b * H * W;
     int d_obj = EDT_INF, d_bg = EDT_INF;  // distance to the last object / background pixel above
     for (int y = 0; y < H; ++y) {
-        const bool obj = m[(size_t)y * W + x] != 0.f;
+        const float v = m[(size_t)y * W + x];
+        const bool obj = v == 1.f, bg = v == 0.f;
         d_obj = obj ? 0 : (d_obj >= EDT_INF ? EDT_INF : d_obj + 1);
-        d_bg = !obj ? 0 : (d_bg >= EDT_INF ? EDT_INF : d_bg + 1);
+        d_bg = bg ? 0 : (d_bg >= EDT_INF ? EDT_INF : d_bg + 1);
         go[(size_t)y * W + x] = d_obj;
         gi[(size_t)y * W + x] = d_bg;
     }
     d_obj = EDT_INF; d_bg = EDT_INF;
     for (int y = H - 1; y >= 0; --y) {
-        const bool obj = m[(size_t)y * W + x] != 0.f;
+        const float v = m[(size_t)y * W + x];
+        const bool obj = v == 1.f, bg = v == 0.f;
         d_obj = obj ? 0 : (d_obj >= EDT_INF ? EDT_INF : d_obj + 1);
-        d_bg = !obj ? 0 : (d_bg >= EDT_INF ? EDT_INF : d_bg + 1);
+        d_bg = bg ? 0 : (d_bg >= EDT_INF ? EDT_INF : d_bg + 1);
         go[(size_t)y * W + x] = min(go[(size_t)y * W + x], d_obj);
         gi[(size_t)y * W + x] = min(gi[(size_t)y * W + x], d_bg);
     }

@@ -494,8 +494,10 @@ class FlattenFunction(torch.autograd.Function):
 
 
 def dt_barrier(masks, k=50.0):
-    """utils/image.py:130-141 `compute_dt_barrier` for a batch on the GPU: masks [B,H,W] or [H,W] (non-zero = object)
-    -> same shape float32, exact Euclidean distances (the reference runs scipy on the host per image per step)."""
+    """utils/image.py:130-141 `compute_dt_barrier` for a batch on the GPU: masks [B,H,W] or [H,W] -> same shape float32,
+    exact Euclidean distances (the reference runs scipy on the host per image per step).  As in scipy, the outside
+    distance is measured to the pixels equal to 1 and the inside distance to the pixels equal to 0; a value in between
+    (the edge of a bilinearly resized mask) is neither."""
     _need_cuda(masks)
     lib = _lib.load()
     m = masks.detach().float()
