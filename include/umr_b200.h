@@ -175,6 +175,26 @@ int umr_raster_backward_deterministic(const float* face_vertices, const float* t
                                       float* grad_textures, const UmrRasterParams* params, void* workspace,
                                       void* stream);
 
+/* Double precision (DESIGN.md §9).  The arguments, outputs, validation and error codes of umr_raster_forward /
+ * umr_raster_backward with every buffer in double: an operation-for-operation twin of the reference kernels' `scalar_t =
+ * double` instantiation (every operation one IEEE binary64 rounding; the scalars of UmrRasterParams stay float, as in the
+ * reference binding, and are widened on use; background_color is the float value widened).  Every mode combination with 3
+ * colour channels (color_channels 0 or 3; 4 returns UMR_ERR_BAD_ARG), shared textures, any F up to UMR_RASTER_MAX_FACES,
+ * grad_faces == NULL or grad_textures == NULL in the backward; pair_buffer and tile_mode are ignored.  A raster side S
+ * above 65535 * 16 returns UMR_ERR_TOO_LARGE.  Every output is bitwise identical for identical inputs on the same device
+ * type and library build, whatever the stream, host thread, concurrent work or CUDA-graph replay: p2f sums are exact fixed
+ * point with 128 fractional bits (integer REDs), and the backward is a face-parallel gather in which every gradient element
+ * has exactly one writer, so there is no separate deterministic variant.  A face covering most of the raster is walked by
+ * one warp in the backward.  No host synchronisation; constant launch count.  The workspace must hold
+ * umr_raster_workspace_bytes_f64() bytes (256-byte aligned): 440 bytes per (image, face), each part rounded up to 256. */
+size_t umr_raster_workspace_bytes_f64(int32_t batch_size, int32_t num_faces, int32_t image_size, int32_t anti_aliasing);
+int umr_raster_forward_f64(const double* face_vertices, const double* textures, double* images, double* soft_colors,
+                           double* aggrs_info, double* p2f_info, const UmrRasterParams* params, void* workspace,
+                           void* stream);
+int umr_raster_backward_f64(const double* face_vertices, const double* textures, const double* soft_colors,
+                            const double* aggrs_info, const double* grad_images, double* grad_faces,
+                            double* grad_textures, const UmrRasterParams* params, void* workspace, void* stream);
+
 /* Fused vertex pipeline (SURVEY.md §8f-1): 7-dof orthographic camera projection with z
  * (nnutils/geom_utils.py:74-91,119-165), y flip (nnutils/smr.py:36), look_at with the eye on the z axis
  * + orthogonal scale (SoftRas/functional/look_at.py:48-60, orthogonal.py:13-16), the face gather

@@ -60,11 +60,12 @@ class SoftRenderer(torch.nn.Module):
     def _projectable(self, vertices):
         """The fused vertex kernel covers exactly the configuration this wrapper sets up (smr.py:56-66):
         look_at camera with the eye on the z axis, orthographic, surface lighting with at most the one
-        default directional light.  Anything else takes the generic torch path below."""
+        default directional light, in float32.  Anything else takes the generic torch path below; float64 vertices then
+        reach the float64 rasteriser."""
         r = self.renderer
         tr = r.transform.transformer
         eye = getattr(tr, "_eye", None)
-        if not (self.fuse_vertex_pipeline and vertices.is_cuda and r.transform.camera_mode == "look_at"
+        if not (self.fuse_vertex_pipeline and vertices.is_cuda and vertices.dtype != torch.float64 and r.transform.camera_mode == "look_at"
                 and not tr.perspective and isinstance(eye, (list, tuple)) and len(eye) == 3):
             return False
         if float(eye[0]) != 0.0 or float(eye[1]) != 0.0 or not float(eye[2]) < 0.0:

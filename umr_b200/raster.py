@@ -177,9 +177,79 @@ def make_params(B, F, T2, image_size, anti_aliasing, background_color, near, far
     return p
 
 
+# --- float64 path (umr_raster_forward_f64 / umr_raster_backward_f64, DESIGN.md §9): float64 face vertices select it, as the
+# reference's kernels dispatch on `faces.type()`.  Everything is float64 (textures and incoming gradients are converted),
+# there is no pair buffer, and the kernels are bitwise reproducible, so torch.use_deterministic_algorithms changes nothing.
+def _forward_f64(ctx, face_vertices, textures, image_size, background_color, near, far, fill_back, eps, sigma_val,
+                 dist_func, dist_eps, gamma_val, aggr_func_rgb, aggr_func_alpha, texture_type, anti_aliasing):
+    lib = _lib.load()
+    dev = face_vertices.device
+    B, F = face_vertices.shape[:2]
+    fv = face_vertices.detach().reshape(B, F, 9).contiguous()
+    Bt = textures.shape[0]
+    if Bt != B and (Bt <= 0 or B % Bt != 0):
+        raise ValueError("textures batch %d does not divide face_vertices batch %d" % (Bt, B))
+    group = B // Bt
+    tex = textures.detach().contiguous().double()
+    if int(tex.shape[-1]) != 3:
+        raise ValueError("float64 rasterisation takes 3 colour channels, got %d (part-map textures are float32 only)"
+                         % int(tex.shape[-1]))
+    S = int(image_size) * (2 if anti_aliasing else 1)
+    params = make_params(B, F, tex.shape[2], image_size, anti_aliasing, background_color, near, far, fill_back, eps,
+                         sigma_val, dist_func, dist_eps, gamma_val, aggr_func_rgb, aggr_func_alpha, texture_type)
+    params.shared_textures = group if group > 1 else 0
+    params.color_channels = 3
+    need_bwd = face_vertices.requires_grad or textures.requires_grad
+    _attach_events(params, "fwd")
+    with torch.cuda.device(dev):
+        images = torch.empty(B, 4, image_size, image_size, device=dev, dtype=torch.float64)
+        colors_hi = images
+        if anti_aliasing:
+            colors_hi = torch.empty(B, 4, S, S, device=dev, dtype=torch.float64) if need_bwd else None
+        aggrs = torch.empty(B, 2, S, S, device=dev, dtype=torch.float64)
+        p2f = torch.empty(B, F, 2, device=dev, dtype=torch.float64)
+        ws = torch.empty(lib.umr_raster_workspace_bytes_f64(B, F, int(image_size), params.anti_aliasing), device=dev,
+                         dtype=torch.uint8)
+        rc = lib.umr_raster_forward_f64(_ptr(fv), _ptr(tex), _ptr(images), _ptr(colors_hi) if anti_aliasing else _ptr(None),
+                                        _ptr(aggrs), _ptr(p2f), ctypes.byref(params), _ptr(ws), _stream_ptr(dev))
+    _lib.check(rc, "umr_raster_forward_f64")
+    params.ev_kernel_start = params.ev_kernel_stop = None
+    ctx.params = params
+    ctx.in_shape = tuple(face_vertices.shape)
+    ctx.tex_needs_grad = textures.requires_grad
+    ctx.geom_needs_grad = face_vertices.requires_grad
+    ctx.tex_dtype = textures.dtype
+    if need_bwd:
+        ctx.save_for_backward(fv, tex, colors_hi, aggrs)
+    ctx.mark_non_differentiable(p2f, aggrs)
+    return images, p2f, aggrs
+
+
+def _backward_f64(ctx, grad_images):
+    lib = _lib.load()
+    fv, tex, colors_hi, aggrs = ctx.saved_tensors
+    dev = fv.device
+    B, F = fv.shape[:2]
+    g = grad_images.contiguous().double()
+    _attach_events(ctx.params, "bwd")
+    with torch.cuda.device(dev):
+        grad_faces = torch.empty_like(fv) if ctx.geom_needs_grad else None
+        grad_tex = torch.empty_like(tex) if ctx.tex_needs_grad else None
+        ws = torch.empty(lib.umr_raster_workspace_bytes_f64(B, F, ctx.params.image_size, ctx.params.anti_aliasing),
+                         device=dev, dtype=torch.uint8)
+        rc = lib.umr_raster_backward_f64(_ptr(fv), _ptr(tex), _ptr(colors_hi), _ptr(aggrs), _ptr(g), _ptr(grad_faces),
+                                         _ptr(grad_tex), ctypes.byref(ctx.params), _ptr(ws), _stream_ptr(dev))
+    _lib.check(rc, "umr_raster_backward_f64")
+    ctx.params.ev_kernel_start = ctx.params.ev_kernel_stop = None
+    if grad_tex is not None:
+        grad_tex = grad_tex.to(ctx.tex_dtype)  # textures of another dtype were converted on the way in
+    return (None if grad_faces is None else grad_faces.view(ctx.in_shape), grad_tex) + (None,) * 14
+
+
 class SoftRasterizeFunction(torch.autograd.Function):
     """forward(face_vertices[B,F,3,3|9], textures[B,F,T2,3], ...) ->
-    (images[B,4,is,is], p2f_info[B,F,2], aggrs_info[B,2,S,S]),  S = is * (2 if anti_aliasing else 1)."""
+    (images[B,4,is,is], p2f_info[B,F,2], aggrs_info[B,2,S,S]),  S = is * (2 if anti_aliasing else 1).
+    float64 face_vertices render in double precision and return float64; every other dtype renders in float32."""
 
     @staticmethod
     def forward(ctx, face_vertices, textures, image_size=256, background_color=(0, 0, 0), near=1,
@@ -188,6 +258,11 @@ class SoftRasterizeFunction(torch.autograd.Function):
                 texture_type="surface", anti_aliasing=False):
         if not face_vertices.is_cuda or not textures.is_cuda:
             raise TypeError("Rasterize module supports only cuda Tensors")  # soft_rasterize.py:117-118
+        ctx.f64 = face_vertices.dtype == torch.float64
+        if ctx.f64:
+            return _forward_f64(ctx, face_vertices, textures, image_size, background_color, near, far, fill_back, eps,
+                                sigma_val, dist_func, dist_eps, gamma_val, aggr_func_rgb, aggr_func_alpha, texture_type,
+                                anti_aliasing)
         lib = _lib.load()
         dev = face_vertices.device
         B, F = face_vertices.shape[:2]
@@ -270,6 +345,8 @@ class SoftRasterizeFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_images, grad_p2f=None, grad_aggrs=None):
+        if ctx.f64:
+            return _backward_f64(ctx, grad_images)
         lib = _lib.load()
         if ctx.has_pairs:
             fv, tex, colors_hi, aggrs, pairs = ctx.saved_tensors

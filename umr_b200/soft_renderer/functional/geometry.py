@@ -20,8 +20,10 @@ def face_vertices(vertices, faces):
     return vertices.reshape(B * V, vertices.shape[2])[idx]
 
 
-def _as_batch(x, B, device):
-    t = torch.as_tensor(x, dtype=torch.float32, device=device)
+def _as_batch(x, B, vertices):
+    """A camera constant (eye, at, up, direction) as [B,3]: float64 beside float64 vertices, float32 otherwise."""
+    dtype = torch.float64 if vertices.dtype == torch.float64 else torch.float32
+    t = torch.as_tensor(x, dtype=dtype, device=vertices.device)
     if t.dim() == 1:
         t = t[None, :].expand(B, -1)
     return t
@@ -31,8 +33,8 @@ def look_at(vertices, eye, at=(0, 0, 0), up=(0, 1, 0)):
     """Camera frame with origin `eye` looking at `at` (look_at.py:48-60; normalise eps 1e-5)."""
     if vertices.dim() != 3:
         raise ValueError("vertices Tensor should have 3 dimensions")
-    B, dev = vertices.shape[0], vertices.device
-    eye, at, up = _as_batch(eye, B, dev), _as_batch(at, B, dev), _as_batch(up, B, dev)
+    B = vertices.shape[0]
+    eye, at, up = _as_batch(eye, B, vertices), _as_batch(at, B, vertices), _as_batch(up, B, vertices)
     z_axis = F.normalize(at - eye, eps=1e-5)
     x_axis = F.normalize(torch.cross(up, z_axis, dim=-1), eps=1e-5)
     y_axis = F.normalize(torch.cross(z_axis, x_axis, dim=-1), eps=1e-5)
@@ -68,8 +70,8 @@ def look(vertices, eye, direction=(0, 1, 0), up=(0, 1, 0)):
     """Camera at `eye` looking along `direction` (functional/look.py)."""
     if vertices.dim() != 3:
         raise ValueError("vertices Tensor should have 3 dimensions")
-    B, dev = vertices.shape[0], vertices.device
-    eye, direction, up = _as_batch(eye, B, dev), _as_batch(direction, B, dev), _as_batch(up, B, dev)
+    B = vertices.shape[0]
+    eye, direction, up = _as_batch(eye, B, vertices), _as_batch(direction, B, vertices), _as_batch(up, B, vertices)
     rot = _camera_frame(direction, up)
     return torch.matmul(vertices - eye[:, None, :], rot.transpose(1, 2))
 

@@ -52,7 +52,8 @@ class Lighting(nn.Module):
     def forward(self, mesh):
         per_face = self.light_mode == "surface"
         count = mesh.num_faces if per_face else mesh.num_vertices
-        light = self.ambient(torch.zeros(mesh.batch_size, count, 3, dtype=torch.float32, device=mesh.device))
+        dtype = torch.float64 if mesh.vertices.dtype == torch.float64 else torch.float32
+        light = self.ambient(torch.zeros(mesh.batch_size, count, 3, dtype=dtype, device=mesh.device))
         if self._needs_normals():  # zero-intensity lights add exactly 0: skip the normal computation
             normals = mesh.surface_normals if per_face else mesh.vertex_normals
             for directional in self.directionals:

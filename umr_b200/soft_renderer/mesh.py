@@ -47,7 +47,9 @@ class Mesh(object):
             shape, res = (self.batch_size, self.num_faces, texture_res ** 2, 3), texture_res
         else:
             shape, res = (self.batch_size, self.num_vertices, 3), 1
-        return torch.ones(shape, dtype=torch.float32, device=self.device), res
+        # float64 vertices render in double precision: their default texture follows them
+        dtype = torch.float64 if self._vertices.dtype == torch.float64 else torch.float32
+        return torch.ones(shape, dtype=dtype, device=self.device), res
 
     # --- sizes ------------------------------------------------------------------------------
     @property
