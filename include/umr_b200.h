@@ -512,6 +512,81 @@ int umr_bilinear_sample_backward_deterministic(const float* image, const float* 
                                                int32_t W, int32_t N, const int32_t* cell_rowptr,
                                                const int32_t* cell_samples, void* stream);
 
+/* Float64 loss kernels (DESIGN.md §10), taken by the autograd Functions of umr_b200/ops.py when any floating-point input
+ * of an op is float64.  Each symbol takes the arguments of its float32 counterpart above with double buffers and double
+ * scalars (w_iou, w_tex, eps, the part weights), plus, for the reductions, a caller-allocated device `workspace` of the
+ * size its *_workspace_bytes_f64 query returns (a function of the sizes only; 0 for invalid sizes).  They are double twins
+ * of the deterministic kernels: reductions store per-CTA partials into workspace slots summed in ascending order, every
+ * gradient element has one writer, and no atomics reach an output, so every output is bitwise identical for identical
+ * inputs on the same device type and library build, whatever torch's deterministic flag says.  Arguments are validated
+ * as in float32 (UMR_ERR_BAD_ARG, UMR_ERR_TOO_LARGE for B > 65535), nothing synchronises with the host, and the launch
+ * count depends on the arguments only (CUDA-graph capturable).
+ *   - sampler: the coordinate map is computed in double.  umr_bilinear_sample_cells_f64 writes the cell keys of
+ *     umr_bilinear_sample_cells from that map; umr_bilinear_sample_backward_f64 takes their table as
+ *     umr_bilinear_sample_backward_deterministic does (NULL when grad_image is) and writes grad_image fully.
+ *   - umr_chamfer_backward_f64 is the gather of umr_chamfer_backward_deterministic (no workspace).
+ *   - umr_texcycle_forward_f64 keeps a float32 face-id plane (ids below UMR_RASTER_MAX_FACES are exact in float).
+ *   - umr_flatten_backward_f64 / umr_corr_chamfer_backward_f64 take the transposed tables of their deterministic
+ *     counterparts; the corr workspace is needed only with grad_vertices. */
+int umr_bilinear_sample_forward_f64(const double* image, const double* flow, double* out, int32_t B, int32_t C, int32_t H,
+                                    int32_t W, int32_t N, void* stream);
+int umr_bilinear_sample_cells_f64(const double* flow, int32_t* cells, int32_t B, int32_t H, int32_t W, int32_t N,
+                                  void* stream);
+int umr_bilinear_sample_backward_f64(const double* image, const double* flow, const double* grad_out, double* grad_flow,
+                                     double* grad_image, int32_t B, int32_t C, int32_t H, int32_t W, int32_t N,
+                                     const int32_t* cell_rowptr, const int32_t* cell_samples, void* stream);
+size_t umr_iou_workspace_bytes_f64(int32_t B, int64_t N);                           /* 16 * B * ceil(N / 2048) */
+int umr_iou_forward_f64(const double* predict, int64_t predict_bstride, const double* target, double* inter, double* uni,
+                        double* loss, int32_t B, int64_t N, void* workspace, void* stream);
+int umr_iou_backward_f64(const double* target, const double* inter, const double* uni, const double* grad_loss,
+                         double* grad_predict, int32_t B, int64_t N, void* stream);
+size_t umr_masked_l1_workspace_bytes_f64(int32_t B, int64_t HW);                    /* 8 * B * ceil(HW / 2048) */
+int umr_masked_l1_forward_f64(const double* pred, int64_t pred_bstride, const double* mask_pred, int64_t mask_pred_bstride,
+                              const double* gt, const double* mask_gt, double* loss, int32_t B, int32_t C, int64_t HW,
+                              void* workspace, void* stream);
+int umr_masked_l1_backward_f64(const double* pred, int64_t pred_bstride, const double* mask_pred, int64_t mask_pred_bstride,
+                               const double* gt, const double* mask_gt, const double* grad_loss, double* grad_pred,
+                               double* grad_mask_pred, int32_t B, int32_t C, int64_t HW, void* stream);
+size_t umr_loss_head_workspace_bytes_f64(int32_t B, int64_t HW);                    /* 24 * B * ceil(HW / 2048) */
+int umr_loss_head_forward_f64(const double* rgba, const double* gt, const double* mask_gt, double* stats, double* per_image,
+                              double* loss, int32_t B, int64_t HW, double w_iou, double w_tex, void* workspace, void* stream);
+int umr_loss_head_backward_f64(const double* rgba, const double* gt, const double* mask_gt, const double* stats,
+                               const double* grad_loss, double* grad_rgba, int32_t B, int64_t HW, double w_iou, double w_tex,
+                               void* stream);
+int umr_chamfer_forward_f64(const double* a, const double* b, double* dist_ab, double* dist_ba, int32_t* idx_ab,
+                            int32_t* idx_ba, int32_t B, int32_t N, int32_t M, int32_t D, void* stream);
+int umr_chamfer_backward_f64(const double* a, const double* b, const int32_t* idx_ab, const int32_t* idx_ba,
+                             const double* grad_dist_ab, const double* grad_dist_ba, double* grad_a, double* grad_b, int32_t B,
+                             int32_t N, int32_t M, int32_t D, void* stream);
+size_t umr_texcycle_workspace_bytes_f64(int32_t B, int32_t F);                      /* 8 * ceil(B * F / 256) */
+int umr_texcycle_forward_f64(const double* flow, const double* prob, const float* face_ids, uint8_t* visible, double* loss,
+                             int32_t B, int32_t F, int32_t T2, int64_t P, void* workspace, void* stream);
+int umr_texcycle_backward_f64(const double* flow, const double* prob, const uint8_t* visible, const double* grad_loss,
+                              double* grad_flow, int32_t B, int32_t F, int32_t T2, void* stream);
+size_t umr_laplacian_workspace_bytes_f64(int32_t B, int32_t V);                     /* 8 * B * ceil(V / 256) */
+int umr_laplacian_forward_f64(const double* x, const int32_t* rowptr, const int32_t* col, const double* coef, double* y,
+                              double* loss, int32_t B, int32_t V, void* workspace, void* stream);
+int umr_laplacian_backward_f64(const double* y, const int32_t* rowptr, const int32_t* col, const double* tcoef,
+                               const double* grad_loss, double* grad_x, int32_t B, int32_t V, void* stream);
+size_t umr_flatten_forward_workspace_bytes_f64(int32_t B, int32_t E);               /* 8 * B * ceil(E / 128) */
+int umr_flatten_forward_f64(const double* vertices, const int32_t* edges, double* loss, int32_t B, int32_t V, int32_t E,
+                            double eps, void* workspace, void* stream);
+size_t umr_flatten_backward_workspace_bytes_f64(int32_t B, int32_t E);              /* 96 * B * E */
+int umr_flatten_backward_f64(const double* vertices, const int32_t* edges, const int32_t* vert_rowptr,
+                             const int32_t* vert_incidence, const double* grad_loss, double* grad_vertices, int32_t B,
+                             int32_t V, int32_t E, double eps, void* workspace, void* stream);
+int umr_corr_chamfer_forward_f64(const double* vertices, int64_t vertices_batch_stride, const double* cams,
+                                 const int32_t* selection, const double* const* targets, const int32_t* target_counts,
+                                 const int32_t* part_ends, const double* weights, double* vert2d, int32_t* nearest,
+                                 double* loss, int32_t B, int32_t NS, void* stream);
+size_t umr_corr_chamfer_workspace_bytes_f64(int32_t B, int32_t NS);                 /* 24 * B * NS */
+int umr_corr_chamfer_backward_f64(const double* vertices, int64_t vertices_batch_stride, const double* cams,
+                                  const int32_t* selection, const double* const* targets, const int32_t* target_counts,
+                                  const int32_t* part_ends, const double* weights, const double* vert2d,
+                                  const int32_t* nearest, const double* grad_loss, const double* grad_vert2d,
+                                  double* grad_vertices, double* grad_cams, int32_t B, int32_t NS, int32_t V,
+                                  const int32_t* vert_rowptr, const int32_t* vert_selection, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -164,6 +164,49 @@ EXPORTS = {
                                                                               ctypes.c_void_p]),
     "umr_bilinear_sample_cells": (ctypes.c_int, [c_f32p, ctypes.c_void_p] + [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
     "umr_bilinear_sample_backward_deterministic": (ctypes.c_int, [c_f32p] * 5 + [ctypes.c_int32] * 5 + [ctypes.c_void_p] * 3),
+    # float64 loss kernels: the float32 symbol's arguments with double buffers / scalars (+ a workspace for reductions)
+    "umr_bilinear_sample_forward_f64": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 5 + [ctypes.c_void_p]),
+    "umr_bilinear_sample_cells_f64": (ctypes.c_int, [ctypes.c_void_p] * 2 + [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
+    "umr_bilinear_sample_backward_f64": (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.c_int32] * 5 + [ctypes.c_void_p] * 3),
+    "umr_iou_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32, ctypes.c_int64]),
+    "umr_iou_forward_f64": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64] + [ctypes.c_void_p] * 4 +
+                            [ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    "umr_iou_backward_f64": (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p]),
+    "umr_masked_l1_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32, ctypes.c_int64]),
+    "umr_masked_l1_forward_f64": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64] +
+                                  [ctypes.c_void_p] * 3 + [ctypes.c_int32, ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p,
+                                                           ctypes.c_void_p]),
+    "umr_masked_l1_backward_f64": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64] +
+                                   [ctypes.c_void_p] * 5 + [ctypes.c_int32, ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p]),
+    "umr_loss_head_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32, ctypes.c_int64]),
+    "umr_loss_head_forward_f64": (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.c_int32, ctypes.c_int64, ctypes.c_double,
+                                                                         ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p]),
+    "umr_loss_head_backward_f64": (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.c_int32, ctypes.c_int64, ctypes.c_double,
+                                                                          ctypes.c_double, ctypes.c_void_p]),
+    "umr_chamfer_forward_f64": (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
+    "umr_chamfer_backward_f64": (ctypes.c_int, [ctypes.c_void_p] * 8 + [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
+    "umr_texcycle_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_texcycle_forward_f64": (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.c_int32] * 3 + [ctypes.c_int64, ctypes.c_void_p,
+                                                                                               ctypes.c_void_p]),
+    "umr_texcycle_backward_f64": (ctypes.c_int, [ctypes.c_void_p] * 5 + [ctypes.c_int32] * 3 + [ctypes.c_void_p]),
+    "umr_laplacian_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_laplacian_forward_f64": (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.c_int32] * 2 + [ctypes.c_void_p] * 2),
+    "umr_laplacian_backward_f64": (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.c_int32] * 2 + [ctypes.c_void_p]),
+    "umr_flatten_forward_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_flatten_forward_f64": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 3 + [ctypes.c_double, ctypes.c_void_p,
+                                                                                              ctypes.c_void_p]),
+    "umr_flatten_backward_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_flatten_backward_f64": (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.c_int32] * 3 + [ctypes.c_double, ctypes.c_void_p,
+                                                                                               ctypes.c_void_p]),
+    "umr_corr_chamfer_forward_f64": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
+                                                    ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_int32),
+                                                    ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_double)] +
+                                     [ctypes.c_void_p] * 3 + [ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p]),
+    "umr_corr_chamfer_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "umr_corr_chamfer_backward_f64": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p,
+                                                     ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_int32),
+                                                     ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_double)] +
+                                      [ctypes.c_void_p] * 6 + [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 4),
 }
 
 _lock = threading.Lock()

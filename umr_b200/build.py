@@ -21,8 +21,8 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-I", os.path
           "-I", CSRC]
 # raster.cu must not contract a*b+c into FMA: its per-(pixel,face) arithmetic is an exact IEEE twin
 # of the reference (DESIGN.md §4).  The loss kernels have no such constraint.
-PER_FILE = {"raster.cu": ["-fmad=false"], "raster_f64.cu": ["-fmad=false"], "vertex.cu": ["-fmad=false"], "mesh_ops.cu": ["-fmad=false"],
-            "nmr.cu": ["-fmad=false"], "voxel.cu": ["-fmad=false"]}
+PER_FILE = {"raster.cu": ["-fmad=false"], "raster_f64.cu": ["-fmad=false"], "losses_f64.cu": ["-fmad=false"],
+            "vertex.cu": ["-fmad=false"], "mesh_ops.cu": ["-fmad=false"], "nmr.cu": ["-fmad=false"], "voxel.cu": ["-fmad=false"]}
 
 
 def sources():
