@@ -159,6 +159,44 @@ def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
 
 
+class KernelMode(object):
+    """The kernel family one autograd call uses, chosen once in `forward` and kept in `ctx` so that the backward runs in
+    the mode of its forward: float32 (`umr_<op>`, may sum with float atomics), deterministic float32 (`*_deterministic`,
+    under torch.use_deterministic_algorithms(True)) or float64 (`*_f64`, always bitwise reproducible, so the flag does
+    not change it).  A `*_f64` symbol takes the arguments of the `*_deterministic` one where that exists (a workspace,
+    transposed tables), else those of the default one; `gather` says whether a call takes that longer list."""
+
+    __slots__ = ("f64", "det", "dtype")
+
+    def __init__(self, f64):
+        self.f64 = bool(f64)
+        self.det = not self.f64 and torch.are_deterministic_algorithms_enabled()
+        self.dtype = torch.float64 if self.f64 else torch.float32
+
+    @property
+    def gather(self):
+        return self.f64 or self.det
+
+    def symbol(self, name, has_deterministic):
+        """(bound symbol, its name) of `name` in this mode.  `has_deterministic`: whether `name_deterministic` exists;
+        without it the deterministic mode calls `name` itself."""
+        if self.f64:
+            name += "_f64"
+        elif self.det and has_deterministic:
+            name += "_deterministic"
+        return getattr(_lib.load(), name), name
+
+    def call(self, name, has_deterministic, *args):
+        fn, name = self.symbol(name, has_deterministic)
+        _lib.check(fn(*args), name)
+
+    def workspace(self, query, device, *args):
+        """The device scratch of a gather-mode call (an allocation, no fill: CUDA-graph safe), else None."""
+        if not self.gather:
+            return None
+        return torch.empty(self.symbol(query, True)[0](*args), device=device, dtype=torch.uint8)
+
+
 def make_params(B, F, T2, image_size, anti_aliasing, background_color, near, far, fill_back, eps,
                 sigma_val, dist_func, dist_eps, gamma_val, aggr_func_rgb, aggr_func_alpha, texture_type):
     p = _lib.UmrRasterParams()
@@ -177,79 +215,12 @@ def make_params(B, F, T2, image_size, anti_aliasing, background_color, near, far
     return p
 
 
-# --- float64 path (umr_raster_forward_f64 / umr_raster_backward_f64, DESIGN.md §9): float64 face vertices select it, as the
-# reference's kernels dispatch on `faces.type()`.  Everything is float64 (textures and incoming gradients are converted),
-# there is no pair buffer, and the kernels are bitwise reproducible, so torch.use_deterministic_algorithms changes nothing.
-def _forward_f64(ctx, face_vertices, textures, image_size, background_color, near, far, fill_back, eps, sigma_val,
-                 dist_func, dist_eps, gamma_val, aggr_func_rgb, aggr_func_alpha, texture_type, anti_aliasing):
-    lib = _lib.load()
-    dev = face_vertices.device
-    B, F = face_vertices.shape[:2]
-    fv = face_vertices.detach().reshape(B, F, 9).contiguous()
-    Bt = textures.shape[0]
-    if Bt != B and (Bt <= 0 or B % Bt != 0):
-        raise ValueError("textures batch %d does not divide face_vertices batch %d" % (Bt, B))
-    group = B // Bt
-    tex = textures.detach().contiguous().double()
-    if int(tex.shape[-1]) != 3:
-        raise ValueError("float64 rasterisation takes 3 colour channels, got %d (part-map textures are float32 only)"
-                         % int(tex.shape[-1]))
-    S = int(image_size) * (2 if anti_aliasing else 1)
-    params = make_params(B, F, tex.shape[2], image_size, anti_aliasing, background_color, near, far, fill_back, eps,
-                         sigma_val, dist_func, dist_eps, gamma_val, aggr_func_rgb, aggr_func_alpha, texture_type)
-    params.shared_textures = group if group > 1 else 0
-    params.color_channels = 3
-    need_bwd = face_vertices.requires_grad or textures.requires_grad
-    _attach_events(params, "fwd")
-    with torch.cuda.device(dev):
-        images = torch.empty(B, 4, image_size, image_size, device=dev, dtype=torch.float64)
-        colors_hi = images
-        if anti_aliasing:
-            colors_hi = torch.empty(B, 4, S, S, device=dev, dtype=torch.float64) if need_bwd else None
-        aggrs = torch.empty(B, 2, S, S, device=dev, dtype=torch.float64)
-        p2f = torch.empty(B, F, 2, device=dev, dtype=torch.float64)
-        ws = torch.empty(lib.umr_raster_workspace_bytes_f64(B, F, int(image_size), params.anti_aliasing), device=dev,
-                         dtype=torch.uint8)
-        rc = lib.umr_raster_forward_f64(_ptr(fv), _ptr(tex), _ptr(images), _ptr(colors_hi) if anti_aliasing else _ptr(None),
-                                        _ptr(aggrs), _ptr(p2f), ctypes.byref(params), _ptr(ws), _stream_ptr(dev))
-    _lib.check(rc, "umr_raster_forward_f64")
-    params.ev_kernel_start = params.ev_kernel_stop = None
-    ctx.params = params
-    ctx.in_shape = tuple(face_vertices.shape)
-    ctx.tex_needs_grad = textures.requires_grad
-    ctx.geom_needs_grad = face_vertices.requires_grad
-    ctx.tex_dtype = textures.dtype
-    if need_bwd:
-        ctx.save_for_backward(fv, tex, colors_hi, aggrs)
-    ctx.mark_non_differentiable(p2f, aggrs)
-    return images, p2f, aggrs
-
-
-def _backward_f64(ctx, grad_images):
-    lib = _lib.load()
-    fv, tex, colors_hi, aggrs = ctx.saved_tensors
-    dev = fv.device
-    B, F = fv.shape[:2]
-    g = grad_images.contiguous().double()
-    _attach_events(ctx.params, "bwd")
-    with torch.cuda.device(dev):
-        grad_faces = torch.empty_like(fv) if ctx.geom_needs_grad else None
-        grad_tex = torch.empty_like(tex) if ctx.tex_needs_grad else None
-        ws = torch.empty(lib.umr_raster_workspace_bytes_f64(B, F, ctx.params.image_size, ctx.params.anti_aliasing),
-                         device=dev, dtype=torch.uint8)
-        rc = lib.umr_raster_backward_f64(_ptr(fv), _ptr(tex), _ptr(colors_hi), _ptr(aggrs), _ptr(g), _ptr(grad_faces),
-                                         _ptr(grad_tex), ctypes.byref(ctx.params), _ptr(ws), _stream_ptr(dev))
-    _lib.check(rc, "umr_raster_backward_f64")
-    ctx.params.ev_kernel_start = ctx.params.ev_kernel_stop = None
-    if grad_tex is not None:
-        grad_tex = grad_tex.to(ctx.tex_dtype)  # textures of another dtype were converted on the way in
-    return (None if grad_faces is None else grad_faces.view(ctx.in_shape), grad_tex) + (None,) * 14
-
-
 class SoftRasterizeFunction(torch.autograd.Function):
     """forward(face_vertices[B,F,3,3|9], textures[B,F,T2,3], ...) ->
     (images[B,4,is,is], p2f_info[B,F,2], aggrs_info[B,2,S,S]),  S = is * (2 if anti_aliasing else 1).
-    float64 face_vertices render in double precision and return float64; every other dtype renders in float32."""
+    float64 face_vertices render in double precision and return float64, as the reference's kernels dispatch on
+    `faces.type()` (DESIGN.md §9): textures are converted, and only 3 colour channels are taken.  Every other dtype
+    renders in float32."""
 
     @staticmethod
     def forward(ctx, face_vertices, textures, image_size=256, background_color=(0, 0, 0), near=1,
@@ -258,17 +229,11 @@ class SoftRasterizeFunction(torch.autograd.Function):
                 texture_type="surface", anti_aliasing=False):
         if not face_vertices.is_cuda or not textures.is_cuda:
             raise TypeError("Rasterize module supports only cuda Tensors")  # soft_rasterize.py:117-118
-        ctx.f64 = face_vertices.dtype == torch.float64
-        if ctx.f64:
-            return _forward_f64(ctx, face_vertices, textures, image_size, background_color, near, far, fill_back, eps,
-                                sigma_val, dist_func, dist_eps, gamma_val, aggr_func_rgb, aggr_func_alpha, texture_type,
-                                anti_aliasing)
-        lib = _lib.load()
+        # torch.use_deterministic_algorithms(True): bitwise-reproducible kernels (include/umr_b200.h)
+        mode = KernelMode(face_vertices.dtype == torch.float64)
         dev = face_vertices.device
         B, F = face_vertices.shape[:2]
-        fv = face_vertices.detach().reshape(B, F, 9).contiguous().float()
-        # a [1,F,T2,3] texture with B > 1 is a batch-SHARED parameter: the kernels read the one copy for every image and
-        # accumulate its gradient directly (the reference materialises repeat(B,...) copies, loss_utils.py:305)
+        fv = face_vertices.detach().reshape(B, F, 9).contiguous().to(mode.dtype)
         # fewer textures than renders: every B / Bt consecutive renders share one texture -- Bt == 1: a batch-shared
         # parameter; Bt == B / 8: the 8 camera hypotheses of each sample (the reference materialises repeat(...) copies,
         # loss_utils.py:305).  The kernels index textures[b // group] and accumulate the group's gradient directly.
@@ -276,11 +241,14 @@ class SoftRasterizeFunction(torch.autograd.Function):
         if Bt != B and (Bt <= 0 or B % Bt != 0):
             raise ValueError("textures batch %d does not divide face_vertices batch %d" % (Bt, B))
         group = B // Bt
-        tex = textures.detach().contiguous().float()
+        tex = textures.detach().contiguous().to(mode.dtype)
         T2 = tex.shape[2]
+        if mode.f64 and int(tex.shape[-1]) != 3:
+            raise ValueError("float64 rasterisation takes 3 colour channels, got %d (part-map textures are float32 only)"
+                             % int(tex.shape[-1]))
         # colour channels: 3, or 4 for the one-render part maps of part_matching_loss (SURVEY.md §8f-2); images then
         # carry NC + 1 planes (colours + alpha)
-        NC = int(tex.shape[-1]) if texture_type == "surface" else 3
+        NC = int(tex.shape[-1]) if texture_type == "surface" and not mode.f64 else 3
         if NC not in (3, 4):
             raise ValueError("textures must have 3 (or, surface textures only, 4) colour channels, got %d" % NC)
         S = int(image_size) * (2 if anti_aliasing else 1)
@@ -296,23 +264,20 @@ class SoftRasterizeFunction(torch.autograd.Function):
                 raise ValueError("4-channel (part-map) textures are constants: no texture gradient is built")
         need_bwd = face_vertices.requires_grad or textures.requires_grad
         generic = dist_func != "euclidean" or aggr_func_alpha != "prod" or texture_type != "surface"
-        # torch.use_deterministic_algorithms(True): bitwise-reproducible kernels (include/umr_b200.h), read once here so the
-        # backward runs in the mode of its forward
-        det = torch.are_deterministic_algorithms_enabled()
         _attach_events(params, "fwd")
         with torch.cuda.device(dev):
-            images = torch.empty(B, NC + 1, image_size, image_size, device=dev, dtype=torch.float32)
+            images = torch.empty(B, NC + 1, image_size, image_size, device=dev, dtype=mode.dtype)
             if anti_aliasing:
-                colors_hi = torch.empty(B, NC + 1, S, S, device=dev, dtype=torch.float32) if need_bwd else None
+                colors_hi = torch.empty(B, NC + 1, S, S, device=dev, dtype=mode.dtype) if need_bwd else None
             else:
                 colors_hi = images
-            aggrs = torch.empty(B, 2, S, S, device=dev, dtype=torch.float32)
-            p2f = torch.empty(B, F, 2, device=dev, dtype=torch.float32)
-            ws_bytes = lib.umr_raster_workspace_bytes_deterministic if det else lib.umr_raster_workspace_bytes
+            aggrs = torch.empty(B, 2, S, S, device=dev, dtype=mode.dtype)
+            p2f = torch.empty(B, F, 2, device=dev, dtype=mode.dtype)
+            ws_bytes, _ = mode.symbol("umr_raster_workspace_bytes", True)
             ws = torch.empty(ws_bytes(B, F, int(image_size), params.anti_aliasing), device=dev, dtype=torch.uint8)
             pairs = None
             pair_key = (S, F, FORWARD_TILE)
-            if need_bwd and not generic and not det and PAIR_CAND_PER_PIXEL > 0:
+            if need_bwd and not generic and not mode.gather and PAIR_CAND_PER_PIXEL > 0:
                 capturing = torch.cuda.is_current_stream_capturing()
                 if PAIR_ADAPTIVE and not capturing:
                     _pair_poll()
@@ -320,12 +285,9 @@ class SoftRasterizeFunction(torch.autograd.Function):
                 pairs = torch.empty(pair_buffer_bytes(B, image_size, anti_aliasing, blocks_per_image=need, device=dev), device=dev,
                                     dtype=torch.uint8)
                 params.pair_buffer, params.pair_buffer_bytes = pairs.data_ptr(), pairs.numel()
-            fwd = lib.umr_raster_forward_deterministic if det else lib.umr_raster_forward
-            rc = fwd(_ptr(fv), _ptr(tex), _ptr(images),
-                                        _ptr(colors_hi) if anti_aliasing else _ptr(None),
-                                        _ptr(aggrs), _ptr(p2f), ctypes.byref(params), _ptr(ws),
-                                        _stream_ptr(dev))
-        _lib.check(rc, "umr_raster_forward_deterministic" if det else "umr_raster_forward")
+            mode.call("umr_raster_forward", True, _ptr(fv), _ptr(tex), _ptr(images),
+                      _ptr(colors_hi) if anti_aliasing else _ptr(None), _ptr(aggrs), _ptr(p2f), ctypes.byref(params),
+                      _ptr(ws), _stream_ptr(dev))
         if pairs is not None:
             _pair_record(pair_key, B, pairs)
         params.ev_kernel_start = params.ev_kernel_stop = None
@@ -334,7 +296,7 @@ class SoftRasterizeFunction(torch.autograd.Function):
         ctx.tex_needs_grad = textures.requires_grad
         ctx.geom_needs_grad = face_vertices.requires_grad
         ctx.has_pairs = pairs is not None
-        ctx.det = det
+        ctx.mode = mode
         if need_bwd:
             if pairs is not None:
                 ctx.save_for_backward(fv, tex, colors_hi, aggrs, pairs)
@@ -345,9 +307,7 @@ class SoftRasterizeFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_images, grad_p2f=None, grad_aggrs=None):
-        if ctx.f64:
-            return _backward_f64(ctx, grad_images)
-        lib = _lib.load()
+        mode = ctx.mode
         if ctx.has_pairs:
             fv, tex, colors_hi, aggrs, pairs = ctx.saved_tensors
             assert ctx.params.pair_buffer == pairs.data_ptr()
@@ -355,20 +315,17 @@ class SoftRasterizeFunction(torch.autograd.Function):
             fv, tex, colors_hi, aggrs = ctx.saved_tensors
         dev = fv.device
         B, F = fv.shape[:2]
-        g = grad_images.contiguous().float()
+        g = grad_images.contiguous().to(mode.dtype)
         _attach_events(ctx.params, "bwd")
         with torch.cuda.device(dev):
             # detached geometry (UMR's texture branch, train_s2.py:248): texture-only backward, no vertex arithmetic
-            tex_only = ctx.tex_needs_grad and not ctx.geom_needs_grad and (ctx.has_pairs or ctx.det)
+            tex_only = ctx.tex_needs_grad and not ctx.geom_needs_grad and (ctx.has_pairs or mode.gather)
             grad_faces = None if tex_only else torch.empty_like(fv)
             grad_tex = torch.empty_like(tex) if ctx.tex_needs_grad else None
-            ws_bytes = lib.umr_raster_workspace_bytes_deterministic if ctx.det else lib.umr_raster_workspace_bytes
+            ws_bytes, _ = mode.symbol("umr_raster_workspace_bytes", True)
             ws = torch.empty(ws_bytes(B, F, ctx.params.image_size, ctx.params.anti_aliasing), device=dev, dtype=torch.uint8)
-            bwd = lib.umr_raster_backward_deterministic if ctx.det else lib.umr_raster_backward
-            rc = bwd(_ptr(fv), _ptr(tex), _ptr(colors_hi), _ptr(aggrs), _ptr(g),
-                                         _ptr(grad_faces), _ptr(grad_tex), ctypes.byref(ctx.params),
-                                         _ptr(ws), _stream_ptr(dev))
-        _lib.check(rc, "umr_raster_backward_deterministic" if ctx.det else "umr_raster_backward")
+            mode.call("umr_raster_backward", True, _ptr(fv), _ptr(tex), _ptr(colors_hi), _ptr(aggrs), _ptr(g),
+                      _ptr(grad_faces), _ptr(grad_tex), ctypes.byref(ctx.params), _ptr(ws), _stream_ptr(dev))
         ctx.params.ev_kernel_start = ctx.params.ev_kernel_stop = None
         return (None if grad_faces is None else grad_faces.view(ctx.in_shape), grad_tex) + (None,) * 14
 
