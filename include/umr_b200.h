@@ -382,7 +382,8 @@ typedef struct UmrNmrParams {
 } UmrNmrParams;
 
 size_t umr_sizeof_nmr_params(void);
-/* Bytes of 256-byte aligned device scratch umr_nmr_forward / umr_nmr_backward_textures need. */
+/* Bytes of 256-byte aligned device scratch umr_nmr_forward / umr_nmr_backward_textures need; 0 for a batch size or
+ * face count they refuse. */
 size_t umr_nmr_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t fill_back);
 /* vertices [B,V,3] f32 (what nmr_pytorch.Render hands over: orthographic_proj_withz(..., offset_z=5) with y negated),
  * faces [B,F,3] int32 (an index outside [0,V) makes that face invisible), textures [B/G,F,T,T,T,3] f32 or NULL.

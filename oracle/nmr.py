@@ -109,17 +109,21 @@ def _region(xy, S, exhaustive):
 
 
 def zbuffer(vertices, faces, image_size, anti_aliasing=True, fill_back=True, eye_z=-2.732, near=0.1, far=100.0,
-            exhaustive=False):
-    """Contract steps 1 and 3.  Returns (face_index [B,S,S] int32, raster depth [B,S,S] f32), raster row order."""
+            exhaustive=False, window=None):
+    """Contract steps 1 and 3.  Returns (face_index [B,S,S] int32, raster depth [B,S,S] f32), raster row order.
+    `window` = (c0, c1, r0, r1), inclusive raster columns and rows: only that rectangle is computed and returned
+    ([B, r1-r0+1, c1-c0+1]), for rasters too large to walk whole."""
     S = image_size * (2 if anti_aliasing else 1)
+    wc0, wc1, wr0, wr1 = (0, S - 1, 0, S - 1) if window is None else window
+    assert 0 <= wc0 <= wc1 < S and 0 <= wr0 <= wr1 < S, window
     fv = face_copies(vertices, faces, fill_back)
     xy, z, inv = _records(fv, S, eye_z)
     B, Fc = fv.shape[:2]
     cp = pixel_coords(S)
     idx = np.arange(S, dtype=f32)
     near, far = f32(near), f32(far)
-    fidx = np.full((B, S, S), -1, np.int32)
-    depth = np.full((B, S, S), far, f32)
+    fidx = np.full((B, wr1 - wr0 + 1, wc1 - wc0 + 1), -1, np.int32)
+    depth = np.full((B, wr1 - wr0 + 1, wc1 - wc0 + 1), far, f32)
     with np.errstate(all="ignore"):
         for b in range(B):
             for f in range(Fc):
@@ -127,6 +131,7 @@ def zbuffer(vertices, faces, image_size, anti_aliasing=True, fill_back=True, eye
                 if (y2 - y0) * (x1 - x0) < (y1 - y0) * (x2 - x0):  # back-facing
                     continue
                 c0, c1, r0, r1 = _region(xy[b, f], S, exhaustive)
+                c0, c1, r0, r1 = max(c0, wc0), min(c1, wc1), max(r0, wr0), min(r1, wr1)
                 if c0 > c1 or r0 > r1:
                     continue
                 xp, yp = cp[None, c0:c1 + 1], cp[r0:r1 + 1, None]
@@ -135,10 +140,10 @@ def zbuffer(vertices, faces, image_size, anti_aliasing=True, fill_back=True, eye
                 if out.all():
                     continue
                 _, zp = bary(inv[b, f], z[b, f], idx[None, c0:c1 + 1], idx[r0:r1 + 1, None])
-                cur = depth[b, r0:r1 + 1, c0:c1 + 1]
+                cur = depth[b, r0 - wr0:r1 - wr0 + 1, c0 - wc0:c1 - wc0 + 1]
                 win = ~out & (zp > near) & (zp < far) & (zp < cur)
                 cur[win] = zp[win]
-                fidx[b, r0:r1 + 1, c0:c1 + 1][win] = f
+                fidx[b, r0 - wr0:r1 - wr0 + 1, c0 - wc0:c1 - wc0 + 1][win] = f
     return fidx, depth
 
 
@@ -244,9 +249,11 @@ def render_rgb_linear(textures, vertices, faces, image_size, zbuf, anti_aliasing
 
 
 def grad_textures(grad_rgb, vertices, faces, texture_shape, zbuf, anti_aliasing=True, fill_back=True, eye_z=-2.732,
-                  shared_textures=1, **light):
+                  shared_textures=1, magnitude=False, counts=False, **light):
     """Contract step 6 in float64: light * w_pn * grad_rgb at the 8 texels of every covered raster pixel, back copies
-    on the transposed texel, through the adjoint of the flip and the pool.  Returns texture_shape [B/G,F,T,T,T,3]."""
+    on the transposed texel, through the adjoint of the flip and the pool.  Returns texture_shape [B/G,F,T,T,T,3].
+    `magnitude` also returns the sum of the terms' absolute values per element, `counts` the number of terms that
+    land on each texel ([B/G,F,T,T,T]): what a float32 summation in any order needs for its error bound."""
     fidx = zbuf[0]
     S = fidx.shape[1]
     T = texture_shape[2]
@@ -254,6 +261,17 @@ def grad_textures(grad_rgb, vertices, faces, texture_shape, zbuf, anti_aliasing=
     b, yi, xi, f, fc, texel, weight = _samples(fidx, vertices, faces, T, fill_back, eye_z, S)
     g = _raster_grad(grad_rgb, S, anti_aliasing)[b, :, yi, xi]  # [N,3]
     out = np.zeros((texture_shape[0], texture_shape[1], T ** 3, 3))
+    mag = np.zeros_like(out)
+    cnt = np.zeros(out.shape[:3], np.int64)
     for pn in range(8):
-        np.add.at(out, (b // shared_textures, f, texel[:, pn]), lit[b, fc] * weight[:, pn, None].astype(np.float64) * g)
-    return out.reshape(texture_shape)
+        at = (b // shared_textures, f, texel[:, pn])
+        term = lit[b, fc] * weight[:, pn, None].astype(np.float64) * g
+        np.add.at(out, at, term)
+        np.add.at(mag, at, np.abs(term))
+        np.add.at(cnt, at, 1)
+    res = (out.reshape(texture_shape),)
+    if magnitude:
+        res += (mag.reshape(texture_shape),)
+    if counts:
+        res += (cnt.reshape(tuple(texture_shape[:-1])),)
+    return res if len(res) > 1 else res[0]

@@ -235,7 +235,8 @@ __global__ void __launch_bounds__(CTA) k_nmr_zbuf(const float* __restrict__ rec,
                 float wb[3], zp;
                 bary(rc, xi, yi, wb, zp);
                 if (!(zp > K.near_ && zp < K.far_)) continue;  // zp <= near, zp >= far or NaN
-                uint32_t zb = __float_as_uint(zp);
+                // -0 packs as +0: NMR's '<' does not order them (near < 0 admits both); the epilogue restores the sign
+                uint32_t zb = __float_as_uint(zp == 0.f ? 0.f : zp);
                 zb = (zb & 0x80000000u) ? ~zb : (zb | 0x80000000u);  // total order of floats as unsigned integers
                 atomicMin(&s_z[(yi - by0) * BIN + (xi - bx0)], ((unsigned long long)zb << 32) | (uint32_t)ff);
             }
@@ -256,6 +257,10 @@ __global__ void __launch_bounds__(CTA) k_nmr_zbuf(const float* __restrict__ rec,
             uint32_t zb = (uint32_t)(key >> 32);
             zb = (zb & 0x80000000u) ? (zb & 0x7fffffffu) : ~zb;
             z = __uint_as_float(zb);
+            if (z == 0.f) {  // the winner's own zero, sign included
+                float wb[3];
+                bary(rec_img + (size_t)fi * REC, bx0 + col, by0 + row, wb, z);
+            }
         }
         const size_t o = ((size_t)b * S + by0 + row) * S + bx0 + col;
         face_index[o] = fi;
@@ -472,7 +477,9 @@ static int check(const UmrNmrParams* p, bool need_tex) {
     if (p->shared_textures > 1 && p->batch_size % p->shared_textures != 0) return UMR_ERR_BAD_ARG;
     const long long S = (long long)p->image_size * (p->anti_aliasing ? 2 : 1);
     const long long Fc = (long long)p->num_faces * (p->fill_back ? 2 : 1);
-    if (S > 16384 || Fc > (1ll << 30) || p->batch_size > 65535 || (long long)p->texture_res * p->texture_res * p->texture_res > (1 << 20))
+    if (S > 16384 || Fc > (1ll << 30) || p->batch_size > 65535) return UMR_ERR_TOO_LARGE;
+    // T^3 <= 2^20 (T <= 101); T is ignored without textures
+    if (need_tex && (p->texture_res > 1024 || (long long)p->texture_res * p->texture_res * p->texture_res > (1 << 20)))
         return UMR_ERR_TOO_LARGE;
     return UMR_OK;
 }
@@ -514,9 +521,11 @@ static void launch_prep(const float* vertices, const int32_t* faces, float* rec,
 using namespace umr::nmr;
 
 extern "C" size_t umr_nmr_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t fill_back) {
-    if (batch_size <= 0 || num_faces <= 0) return 0;
-    const int Fc = num_faces * (fill_back ? 2 : 1);
-    return rec_bytes(batch_size, Fc) + box_bytes(batch_size, Fc);
+    // 0 for the shapes check() refuses, like B <= 0
+    if (batch_size <= 0 || num_faces <= 0 || batch_size > 65535) return 0;
+    const long long Fc = (long long)num_faces * (fill_back ? 2 : 1);
+    if (Fc > (1ll << 30)) return 0;
+    return rec_bytes(batch_size, (int)Fc) + box_bytes(batch_size, (int)Fc);
 }
 
 extern "C" size_t umr_sizeof_nmr_params(void) { return sizeof(UmrNmrParams); }
