@@ -82,7 +82,9 @@ __device__ __forceinline__ void red_add_shared(float* addr, float v) {
     asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(smem_u32(addr)), "f"(v) : "memory");
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
+// warp_sum and sum_ascending serve float and double alike
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {
     v += __shfl_xor_sync(0xffffffffu, v, 16);
     v += __shfl_xor_sync(0xffffffffu, v, 8);
     v += __shfl_xor_sync(0xffffffffu, v, 4);
@@ -90,13 +92,55 @@ __device__ __forceinline__ float warp_sum(float v) {
     v += __shfl_xor_sync(0xffffffffu, v, 1);
     return v;
 }
-// p[0] + p[1] + ... + p[n-1], left to right in float: the fixed order of the deterministic reductions' finalize kernels,
-// which sum per-CTA partials stored in workspace slots instead of adding them with atomics
-__device__ __forceinline__ float sum_ascending(const float* p, int n) {
-    float t = 0.f;
+// p[0] + p[1] + ... + p[n-1], left to right: the fixed order of the deterministic reductions' finalize kernels, which sum
+// per-CTA partials stored in workspace slots instead of adding them with atomics
+template <typename T>
+__device__ __forceinline__ T sum_ascending(const T* p, int n) {
+    T t = 0;
     for (int k = 0; k < n; ++k) t += p[k];
     return t;
 }
+// deterministic finalize of a per-row reduction: out[r] = the row's n slots summed in ascending order
+template <typename T>
+__global__ void k_sum_slot_rows(const T* __restrict__ slots, T* __restrict__ out, int rows, int n) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < rows) out[r] = sum_ascending(slots + (size_t)r * n, n);
+}
+// grad[b][v] = v's 3-vectors of terms[b] ([width][3] per batch item) summed over a transposed table (vrowptr [V+1], vinc
+// listing term indices in ascending order, so the sum order is fixed); a vertex with no entry gets 0.  Serves the flatten
+// backward (width 4E: edge * 4 + role) and CorrLossChamfer's (width NS: the selection index j).
+template <typename T>
+__global__ void __launch_bounds__(256) k_gather3(const T* __restrict__ terms, const int32_t* __restrict__ vrowptr,
+                                                 const int32_t* __restrict__ vinc, T* __restrict__ gverts, int V,
+                                                 int64_t width) {
+    const int b = blockIdx.y;
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    const T* tb = terms + (size_t)b * width * 3;
+    T g0 = 0, g1 = 0, g2 = 0;
+    for (int k = __ldg(vrowptr + v); k < __ldg(vrowptr + v + 1); ++k) {
+        const T* t = tb + (size_t)__ldg(vinc + k) * 3;
+        g0 += t[0]; g1 += t[1]; g2 += t[2];
+    }
+    T* o = gverts + ((size_t)b * V + v) * 3;
+    o[0] = g0; o[1] = g1; o[2] = g2;
+}
+
+// Operations rounded once and never contracted to FMA, whatever the compile flags, for float and double
+__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ float sub_rn(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+
+// float2 / double2 by scalar type
+template <typename T> struct Vec2;
+template <> struct Vec2<float> { using type = float2; };
+template <> struct Vec2<double> { using type = double2; };
+template <typename T> using vec2_t = typename Vec2<T>::type;
+__device__ __forceinline__ float2 make_vec2(float x, float y) { return make_float2(x, y); }
+__device__ __forceinline__ double2 make_vec2(double x, double y) { return make_double2(x, y); }
 __device__ __forceinline__ float warp_max(float v) {
     v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 16));
     v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 8));

@@ -12,12 +12,15 @@
 //                           forward and hand-derived backward instead of ~40 elementwise torch kernels.
 //   k_edt_*                 utils/image.py:130-141 compute_dt_barrier: exact Euclidean distance transform of the GT mask,
 //                           scipy on the host CPU per image per step in the reference (train_s2.py:196).
-// The Laplacian / flatten sums and the flatten backward have deterministic variants (DET template parameter,
-// k_flatten_gather; `*_deterministic` entry points at the end of this file; DESIGN.md §2).
+// The Laplacian / flatten sums and the flatten backward have deterministic variants (DET template parameter, k_gather3;
+// `*_deterministic` entry points at the end of this file; DESIGN.md §2).  The Laplacian and flatten kernels are templated
+// on the scalar type: the float64 entry points at the end of this file (DESIGN.md §10) run their double instantiations,
+// which share the deterministic structure and launchers.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "umr_b200.h"
@@ -109,32 +112,32 @@ __global__ void __launch_bounds__(256) k_load_textures(const float* __restrict__
 // exactly the off-diagonal entries of the reference's row-normalised matrix), loss_b = sum_i |y_i|^2
 // ---------------------------------------------------------------------------------------------
 // DET: `loss` is the workspace slot array [B][gridDim.x]; every CTA stores its partial
-template <bool DET>
-__global__ void __launch_bounds__(256) k_laplacian_fwd(const float* __restrict__ x, const int32_t* __restrict__ rowptr,
-                                                       const int32_t* __restrict__ col, const float* __restrict__ coef,
-                                                       float* __restrict__ y, float* __restrict__ loss, int V) {
+template <typename T, bool DET>
+__global__ void __launch_bounds__(256) k_laplacian_fwd(const T* __restrict__ x, const int32_t* __restrict__ rowptr,
+                                                       const int32_t* __restrict__ col, const T* __restrict__ coef,
+                                                       T* __restrict__ y, T* __restrict__ loss, int V) {
     const int b = blockIdx.y;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    float acc = 0.f;
+    T acc = 0;
     if (i < V) {
-        const float* xb = x + (size_t)b * V * 3;
-        float y0 = xb[i * 3], y1 = xb[i * 3 + 1], y2 = xb[i * 3 + 2];
+        const T* xb = x + (size_t)b * V * 3;
+        T y0 = xb[i * 3], y1 = xb[i * 3 + 1], y2 = xb[i * 3 + 2];
         for (int e = __ldg(rowptr + i); e < __ldg(rowptr + i + 1); ++e) {
             const int j = __ldg(col + e);
-            const float c = __ldg(coef + e);
+            const T c = __ldg(coef + e);
             y0 += c * xb[j * 3]; y1 += c * xb[j * 3 + 1]; y2 += c * xb[j * 3 + 2];
         }
-        float* yb = y + ((size_t)b * V + i) * 3;
+        T* yb = y + ((size_t)b * V + i) * 3;
         yb[0] = y0; yb[1] = y1; yb[2] = y2;
         acc = y0 * y0 + y1 * y1 + y2 * y2;
     }
     acc = warp_sum(acc);
-    __shared__ float s[8];
+    __shared__ T s[8];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (lane == 0) s[warp] = acc;
     __syncthreads();
     if (warp == 0) {
-        acc = lane < 8 ? s[lane] : 0.f;
+        acc = lane < 8 ? s[lane] : T(0);
         acc = warp_sum(acc);
         if (DET) {
             if (lane == 0) loss[(size_t)b * gridDim.x + blockIdx.x] = acc;
@@ -143,118 +146,117 @@ __global__ void __launch_bounds__(256) k_laplacian_fwd(const float* __restrict__
         }
     }
 }
-// deterministic finalize of the Laplacian / flatten sums: loss[b] = image b's n slots summed in ascending CTA order
-__global__ void k_mesh_loss_sum_det(const float* __restrict__ slots, float* __restrict__ loss, int B, int n) {
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b < B) loss[b] = sum_ascending(slots + (size_t)b * n, n);
-}
 // grad_x_j = 2 g_b (y_j + sum_{i : j in N(i)} coef[i,j] y_i); the neighbour relation is symmetric, so the transposed
 // entry of (j, i) is looked up through tcoef[e] = coef of row col[e] towards j (precomputed on the host)
-__global__ void __launch_bounds__(256) k_laplacian_bwd(const float* __restrict__ y, const int32_t* __restrict__ rowptr,
-                                                       const int32_t* __restrict__ col, const float* __restrict__ tcoef,
-                                                       const float* __restrict__ gl, float* __restrict__ gx, int V) {
+template <typename T>
+__global__ void __launch_bounds__(256) k_laplacian_bwd(const T* __restrict__ y, const int32_t* __restrict__ rowptr,
+                                                       const int32_t* __restrict__ col, const T* __restrict__ tcoef,
+                                                       const T* __restrict__ gl, T* __restrict__ gx, int V) {
     const int b = blockIdx.y;
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= V) return;
-    const float* yb = y + (size_t)b * V * 3;
-    float g0 = yb[j * 3], g1 = yb[j * 3 + 1], g2 = yb[j * 3 + 2];
+    const T* yb = y + (size_t)b * V * 3;
+    T g0 = yb[j * 3], g1 = yb[j * 3 + 1], g2 = yb[j * 3 + 2];
     for (int e = __ldg(rowptr + j); e < __ldg(rowptr + j + 1); ++e) {
         const int i = __ldg(col + e);
-        const float c = __ldg(tcoef + e);
+        const T c = __ldg(tcoef + e);
         g0 += c * yb[i * 3]; g1 += c * yb[i * 3 + 1]; g2 += c * yb[i * 3 + 2];
     }
-    const float k = 2.f * __ldg(gl + b);
-    float* o = gx + ((size_t)b * V + j) * 3;
+    const T k = T(2) * __ldg(gl + b);
+    T* o = gx + ((size_t)b * V + j) * 3;
     o[0] = k * g0; o[1] = k * g1; o[2] = k * g2;
 }
 
 // ---------------------------------------------------------------------------------------------
 // Flatten regulariser: per edge (v0, v1) with opposite corners v2, v3 (losses.py:71-108)
 // ---------------------------------------------------------------------------------------------
+template <typename T>
 struct Perp {  // forward values of one `perp(a, b)` block kept for the backward
-    float a[3], b[3], cb[3];
-    float al2, bl2, al1, bl1, ab, cosv, sinv, k, q, l;
+    T a[3], b[3], cb[3];
+    T al2, bl2, al1, bl1, ab, cosv, sinv, k, q, l;
 };
-__device__ __forceinline__ void perp_fwd(const float* a, const float* b, float eps, Perp& P) {
+template <typename T>
+__device__ __forceinline__ void perp_fwd(const T* a, const T* b, T eps, Perp<T>& P) {
 #pragma unroll
     for (int d = 0; d < 3; ++d) { P.a[d] = a[d]; P.b[d] = b[d]; }
     P.al2 = a[0] * a[0] + a[1] * a[1] + a[2] * a[2];
     P.bl2 = b[0] * b[0] + b[1] * b[1] + b[2] * b[2];
-    P.al1 = sqrtf(P.al2 + eps);
-    P.bl1 = sqrtf(P.bl2 + eps);
+    P.al1 = sqrt(P.al2 + eps);
+    P.bl1 = sqrt(P.bl2 + eps);
     P.ab = a[0] * b[0] + a[1] * b[1] + a[2] * b[2];
     P.q = P.al1 * P.bl1 + eps;
     P.cosv = P.ab / P.q;
-    P.sinv = sqrtf(1 - P.cosv * P.cosv + eps);
+    P.sinv = sqrt(1 - P.cosv * P.cosv + eps);
     P.k = P.ab / (P.al2 + eps);
 #pragma unroll
     for (int d = 0; d < 3; ++d) P.cb[d] = b[d] - a[d] * P.k;
     P.l = P.bl1 * P.sinv;
 }
 // reverse mode through perp(): inputs dcb[3], dl -> accumulates da[3], db[3]
-__device__ __forceinline__ void perp_bwd(const Perp& P, const float* dcb, float dl, float eps, float* da, float* db) {
-    float dbl1 = dl * P.sinv;
-    const float dsinv = dl * P.bl1;
-    float dk = 0.f;
+template <typename T>
+__device__ __forceinline__ void perp_bwd(const Perp<T>& P, const T* dcb, T dl, T eps, T* da, T* db) {
+    T dbl1 = dl * P.sinv;
+    const T dsinv = dl * P.bl1;
+    T dk = 0;
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
         db[d] += dcb[d];
         da[d] += -dcb[d] * P.k;
         dk += -dcb[d] * P.a[d];
     }
-    float dab = dk / (P.al2 + eps);
-    float dal2 = -dk * P.ab / ((P.al2 + eps) * (P.al2 + eps));
-    const float ds = dsinv / (2.f * P.sinv);
-    const float dcosv = -2.f * P.cosv * ds;
+    T dab = dk / (P.al2 + eps);
+    T dal2 = -dk * P.ab / ((P.al2 + eps) * (P.al2 + eps));
+    const T ds = dsinv / (T(2) * P.sinv);
+    const T dcosv = T(-2) * P.cosv * ds;
     dab += dcosv / P.q;
-    const float dq = -dcosv * P.ab / (P.q * P.q);
-    const float dal1 = dq * P.bl1;
+    const T dq = -dcosv * P.ab / (P.q * P.q);
+    const T dal1 = dq * P.bl1;
     dbl1 += dq * P.al1;
-    dal2 += dal1 / (2.f * P.al1);
-    const float dbl2 = dbl1 / (2.f * P.bl1);
+    dal2 += dal1 / (T(2) * P.al1);
+    const T dbl2 = dbl1 / (T(2) * P.bl1);
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
-        da[d] += dab * P.b[d] + 2.f * dal2 * P.a[d];
-        db[d] += dab * P.a[d] + 2.f * dbl2 * P.b[d];
+        da[d] += dab * P.b[d] + T(2) * dal2 * P.a[d];
+        db[d] += dab * P.a[d] + T(2) * dbl2 * P.b[d];
     }
 }
 // DET forward: `loss` is the workspace slot array [B][gridDim.x].  DET backward: `gverts` is the per-edge term array
-// [B][E][4][3] (roles v0..v3), summed per vertex by k_flatten_gather.
-template <bool BWD, bool DET>
-__global__ void __launch_bounds__(128) k_flatten(const float* __restrict__ verts, const int32_t* __restrict__ edges,
-                                                 float* __restrict__ loss, const float* __restrict__ gl,
-                                                 float* __restrict__ gverts, int V, int E, float eps) {
+// [B][E][4][3] (roles v0..v3), summed per vertex by k_gather3.  Float64 runs only the DET forms.
+template <typename T, bool BWD, bool DET>
+__global__ void __launch_bounds__(128) k_flatten(const T* __restrict__ verts, const int32_t* __restrict__ edges,
+                                                 T* __restrict__ loss, const T* __restrict__ gl,
+                                                 T* __restrict__ gverts, int V, int E, T eps) {
     const int b = blockIdx.y;
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    float acc = 0.f;
+    T acc = 0;
     if (e < E) {
-        const float* vb = verts + (size_t)b * V * 3;
+        const T* vb = verts + (size_t)b * V * 3;
         const int i0 = __ldg(edges + e * 4), i1 = __ldg(edges + e * 4 + 1), i2 = __ldg(edges + e * 4 + 2), i3 = __ldg(edges + e * 4 + 3);
-        float a[3], b1[3], b2[3];
+        T a[3], b1[3], b2[3];
 #pragma unroll
         for (int d = 0; d < 3; ++d) {
-            const float p0 = vb[i0 * 3 + d];
+            const T p0 = vb[i0 * 3 + d];
             a[d] = vb[i1 * 3 + d] - p0;
             b1[d] = vb[i2 * 3 + d] - p0;
             b2[d] = vb[i3 * 3 + d] - p0;
         }
-        Perp P1, P2;
+        Perp<T> P1, P2;
         perp_fwd(a, b1, eps, P1);
         perp_fwd(a, b2, eps, P2);
-        const float num = P1.cb[0] * P2.cb[0] + P1.cb[1] * P2.cb[1] + P1.cb[2] * P2.cb[2];
-        const float den = P1.l * P2.l + eps;
-        const float cosd = num / den;
+        const T num = P1.cb[0] * P2.cb[0] + P1.cb[1] * P2.cb[1] + P1.cb[2] * P2.cb[2];
+        const T den = P1.l * P2.l + eps;
+        const T cosd = num / den;
         acc = (cosd + 1) * (cosd + 1);
         if (BWD) {
-            const float dcos = 2.f * (cosd + 1) * __ldg(gl + b);
-            const float dnum = dcos / den, dden = -dcos * num / (den * den);
-            float dcb1[3], dcb2[3], da[3] = {0, 0, 0}, db1[3] = {0, 0, 0}, db2[3] = {0, 0, 0};
+            const T dcos = T(2) * (cosd + 1) * __ldg(gl + b);
+            const T dnum = dcos / den, dden = -dcos * num / (den * den);
+            T dcb1[3], dcb2[3], da[3] = {0, 0, 0}, db1[3] = {0, 0, 0}, db2[3] = {0, 0, 0};
 #pragma unroll
             for (int d = 0; d < 3; ++d) { dcb1[d] = dnum * P2.cb[d]; dcb2[d] = dnum * P1.cb[d]; }
             perp_bwd(P1, dcb1, dden * P2.l, eps, da, db1);
             perp_bwd(P2, dcb2, dden * P1.l, eps, da, db2);
             if (DET) {
-                float* t = gverts + ((size_t)b * E + e) * 12;
+                T* t = gverts + ((size_t)b * E + e) * 12;
 #pragma unroll
                 for (int d = 0; d < 3; ++d) {
                     t[d] = -(da[d] + db1[d] + db2[d]);
@@ -263,7 +265,7 @@ __global__ void __launch_bounds__(128) k_flatten(const float* __restrict__ verts
                     t[9 + d] = db2[d];
                 }
             } else {
-                float* gb = gverts + (size_t)b * V * 3;
+                T* gb = gverts + (size_t)b * V * 3;
 #pragma unroll
                 for (int d = 0; d < 3; ++d) {
                     atomicAdd(gb + i1 * 3 + d, da[d]);
@@ -276,12 +278,16 @@ __global__ void __launch_bounds__(128) k_flatten(const float* __restrict__ verts
     }
     if (!BWD) {
         acc = warp_sum(acc);
-        __shared__ float s[4];
+        __shared__ T s[4];
         const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
         if (lane == 0) s[warp] = acc;
         __syncthreads();
-        if (warp == 0) {
-            acc = lane < 4 ? s[lane] : 0.f;
+        // the four warp sums meet as (s0 + s2) + (s1 + s3) in float32 (warp_sum) and as ((s0 + s1) + s2) + s3 in float64:
+        // each precision keeps the bits it always had
+        if constexpr (std::is_same<T, double>::value) {
+            if (threadIdx.x == 0) loss[(size_t)b * gridDim.x + blockIdx.x] = ((s[0] + s[1]) + s[2]) + s[3];
+        } else if (warp == 0) {
+            acc = lane < 4 ? s[lane] : T(0);
             acc = warp_sum(acc);
             if (DET) {
                 if (lane == 0) loss[(size_t)b * gridDim.x + blockIdx.x] = acc;
@@ -291,24 +297,6 @@ __global__ void __launch_bounds__(128) k_flatten(const float* __restrict__ verts
         }
     }
 }
-// grad_vertices[b][v] = sum of v's per-edge terms over the transposed incidence table: vrowptr [V+1], vinc [4E] lists
-// edge * 4 + role in ascending order, so the sum order is fixed; a vertex on no edge gets 0
-__global__ void __launch_bounds__(256) k_flatten_gather(const float* __restrict__ terms, const int32_t* __restrict__ vrowptr,
-                                                        const int32_t* __restrict__ vinc, float* __restrict__ gverts, int V,
-                                                        int E) {
-    const int b = blockIdx.y;
-    const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    const float* tb = terms + (size_t)b * E * 12;
-    float g0 = 0.f, g1 = 0.f, g2 = 0.f;
-    for (int k = __ldg(vrowptr + v); k < __ldg(vrowptr + v + 1); ++k) {
-        const float* t = tb + (size_t)__ldg(vinc + k) * 3;
-        g0 += t[0]; g1 += t[1]; g2 += t[2];
-    }
-    float* o = gverts + ((size_t)b * V + v) * 3;
-    o[0] = g0; o[1] = g1; o[2] = g2;
-}
-
 // ---------------------------------------------------------------------------------------------
 // exact Euclidean distance transform + barrier sigmoid (utils/image.py:130-141)
 //   pass 1 (per column): g(y, x) = distance along the column to the nearest FEATURE pixel (inf if none)
@@ -419,16 +407,22 @@ extern "C" int umr_laplacian_forward(const float* x, const int32_t* rowptr, cons
     cudaError_t e = cudaMemsetAsync(loss, 0, (size_t)B * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     count_launch();
-    k_laplacian_fwd<false><<<dim3((V + 255) / 256, B), 256, 0, st>>>(x, rowptr, col, coef, y, loss, V);
+    k_laplacian_fwd<float, false><<<dim3((V + 255) / 256, B), 256, 0, st>>>(x, rowptr, col, coef, y, loss, V);
+    UMR_RET();
+}
+// float32 (default and deterministic mode: one writer per element) and float64
+template <typename T>
+static int laplacian_backward(const T* y, const int32_t* rowptr, const int32_t* col, const T* tcoef, const T* grad_loss,
+                              T* grad_x, int32_t B, int32_t V, void* stream_) {
+    if (!y || !rowptr || !col || !tcoef || !grad_loss || !grad_x || B <= 0 || V <= 0) return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    count_launch();
+    k_laplacian_bwd<T><<<dim3((V + 255) / 256, B), 256, 0, (cudaStream_t)stream_>>>(y, rowptr, col, tcoef, grad_loss, grad_x, V);
     UMR_RET();
 }
 extern "C" int umr_laplacian_backward(const float* y, const int32_t* rowptr, const int32_t* col, const float* tcoef,
                                       const float* grad_loss, float* grad_x, int32_t B, int32_t V, void* stream_) {
-    if (!y || !rowptr || !col || !tcoef || !grad_loss || !grad_x || B <= 0 || V <= 0) return UMR_ERR_BAD_ARG;
-    if (B > 65535) return UMR_ERR_TOO_LARGE;
-    count_launch();
-    k_laplacian_bwd<<<dim3((V + 255) / 256, B), 256, 0, (cudaStream_t)stream_>>>(y, rowptr, col, tcoef, grad_loss, grad_x, V);
-    UMR_RET();
+    return laplacian_backward(y, rowptr, col, tcoef, grad_loss, grad_x, B, V, stream_);
 }
 
 extern "C" int umr_flatten_forward(const float* vertices, const int32_t* edges, float* loss, int32_t B, int32_t V, int32_t E,
@@ -439,7 +433,7 @@ extern "C" int umr_flatten_forward(const float* vertices, const int32_t* edges, 
     cudaError_t e = cudaMemsetAsync(loss, 0, (size_t)B * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     count_launch();
-    k_flatten<false, false><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, loss, nullptr, nullptr, V, E, eps);
+    k_flatten<float, false, false><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, loss, nullptr, nullptr, V, E, eps);
     UMR_RET();
 }
 extern "C" int umr_flatten_backward(const float* vertices, const int32_t* edges, const float* grad_loss, float* grad_vertices,
@@ -450,7 +444,7 @@ extern "C" int umr_flatten_backward(const float* vertices, const int32_t* edges,
     cudaError_t e = cudaMemsetAsync(grad_vertices, 0, (size_t)B * V * 3 * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     count_launch();
-    k_flatten<true, false><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, nullptr, grad_loss, grad_vertices, V, E, eps);
+    k_flatten<float, true, false><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, nullptr, grad_loss, grad_vertices, V, E, eps);
     UMR_RET();
 }
 
@@ -472,58 +466,108 @@ extern "C" int umr_dt_barrier(const float* mask, float* dt, void* workspace, int
 }
 
 // ---------------------------------------------------------------------------------------------
-// deterministic mode (include/umr_b200.h, DESIGN.md §2): per-CTA partials stored in workspace slots and summed in
-// ascending CTA order; the flatten backward writes per-edge terms and gathers them per vertex
+// deterministic float32 and float64 (include/umr_b200.h, DESIGN.md §2, §10): per-CTA partials stored in workspace slots
+// and summed in ascending CTA order; the flatten backward writes per-edge terms and gathers them per vertex.  One launcher
+// per op serves both precisions.
 // ---------------------------------------------------------------------------------------------
-extern "C" size_t umr_laplacian_workspace_bytes_deterministic(int32_t B, int32_t V) {
+template <typename T>
+static size_t laplacian_workspace_bytes(int32_t B, int32_t V) {
     if (B <= 0 || V <= 0) return 0;
-    return (size_t)B * ((V + 255) / 256) * sizeof(float);
+    return (size_t)B * ((V + 255) / 256) * sizeof(T);
 }
-extern "C" int umr_laplacian_forward_deterministic(const float* x, const int32_t* rowptr, const int32_t* col, const float* coef,
-                                                   float* y, float* loss, int32_t B, int32_t V, void* workspace, void* stream_) {
+template <typename T>
+static int laplacian_forward_slots(const T* x, const int32_t* rowptr, const int32_t* col, const T* coef, T* y, T* loss,
+                                   int32_t B, int32_t V, void* workspace, void* stream_) {
     if (!x || !rowptr || !col || !coef || !y || !loss || !workspace || B <= 0 || V <= 0) return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     cudaStream_t st = (cudaStream_t)stream_;
     const int gx = (V + 255) / 256;
-    float* slots = (float*)workspace;
+    T* slots = (T*)workspace;
     count_launch(2);
-    k_laplacian_fwd<true><<<dim3(gx, B), 256, 0, st>>>(x, rowptr, col, coef, y, slots, V);
-    k_mesh_loss_sum_det<<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, gx);
+    k_laplacian_fwd<T, true><<<dim3(gx, B), 256, 0, st>>>(x, rowptr, col, coef, y, slots, V);
+    k_sum_slot_rows<T><<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, gx);
     UMR_RET();
 }
-
-extern "C" size_t umr_flatten_forward_workspace_bytes_deterministic(int32_t B, int32_t E) {
+template <typename T>
+static size_t flatten_forward_workspace_bytes(int32_t B, int32_t E) {
     if (B <= 0 || E <= 0) return 0;
-    return (size_t)B * ((E + 127) / 128) * sizeof(float);
+    return (size_t)B * ((E + 127) / 128) * sizeof(T);
 }
-extern "C" int umr_flatten_forward_deterministic(const float* vertices, const int32_t* edges, float* loss, int32_t B, int32_t V,
-                                                 int32_t E, float eps, void* workspace, void* stream_) {
+template <typename T>
+static int flatten_forward_slots(const T* vertices, const int32_t* edges, T* loss, int32_t B, int32_t V, int32_t E, T eps,
+                                 void* workspace, void* stream_) {
     if (!vertices || !edges || !loss || !workspace || B <= 0 || V <= 0 || E <= 0) return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     cudaStream_t st = (cudaStream_t)stream_;
     const int gx = (E + 127) / 128;
-    float* slots = (float*)workspace;
+    T* slots = (T*)workspace;
     count_launch(2);
-    k_flatten<false, true><<<dim3(gx, B), 128, 0, st>>>(vertices, edges, slots, nullptr, nullptr, V, E, eps);
-    k_mesh_loss_sum_det<<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, gx);
+    k_flatten<T, false, true><<<dim3(gx, B), 128, 0, st>>>(vertices, edges, slots, nullptr, nullptr, V, E, eps);
+    k_sum_slot_rows<T><<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, gx);
     UMR_RET();
 }
-
-extern "C" size_t umr_flatten_backward_workspace_bytes_deterministic(int32_t B, int32_t E) {
+template <typename T>
+static size_t flatten_backward_workspace_bytes(int32_t B, int32_t E) {
     if (B <= 0 || E <= 0) return 0;
-    return (size_t)B * E * 12 * sizeof(float);
+    return (size_t)B * E * 12 * sizeof(T);
 }
-extern "C" int umr_flatten_backward_deterministic(const float* vertices, const int32_t* edges, const int32_t* vert_rowptr,
-                                                  const int32_t* vert_incidence, const float* grad_loss, float* grad_vertices,
-                                                  int32_t B, int32_t V, int32_t E, float eps, void* workspace, void* stream_) {
+template <typename T>
+static int flatten_backward_gather(const T* vertices, const int32_t* edges, const int32_t* vert_rowptr,
+                                   const int32_t* vert_incidence, const T* grad_loss, T* grad_vertices, int32_t B, int32_t V,
+                                   int32_t E, T eps, void* workspace, void* stream_) {
     if (!vertices || !edges || !vert_rowptr || !vert_incidence || !grad_loss || !grad_vertices || !workspace || B <= 0 ||
         V <= 0 || E <= 0)
         return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     cudaStream_t st = (cudaStream_t)stream_;
-    float* terms = (float*)workspace;
+    T* terms = (T*)workspace;
     count_launch(2);
-    k_flatten<true, true><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, nullptr, grad_loss, terms, V, E, eps);
-    k_flatten_gather<<<dim3((V + 255) / 256, B), 256, 0, st>>>(terms, vert_rowptr, vert_incidence, grad_vertices, V, E);
+    k_flatten<T, true, true><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, nullptr, grad_loss, terms, V, E, eps);
+    k_gather3<T><<<dim3((V + 255) / 256, B), 256, 0, st>>>(terms, vert_rowptr, vert_incidence, grad_vertices, V, (int64_t)E * 4);
     UMR_RET();
+}
+
+extern "C" size_t umr_laplacian_workspace_bytes_deterministic(int32_t B, int32_t V) { return laplacian_workspace_bytes<float>(B, V); }
+extern "C" int umr_laplacian_forward_deterministic(const float* x, const int32_t* rowptr, const int32_t* col, const float* coef,
+                                                   float* y, float* loss, int32_t B, int32_t V, void* workspace, void* stream_) {
+    return laplacian_forward_slots(x, rowptr, col, coef, y, loss, B, V, workspace, stream_);
+}
+extern "C" size_t umr_flatten_forward_workspace_bytes_deterministic(int32_t B, int32_t E) {
+    return flatten_forward_workspace_bytes<float>(B, E);
+}
+extern "C" int umr_flatten_forward_deterministic(const float* vertices, const int32_t* edges, float* loss, int32_t B, int32_t V,
+                                                 int32_t E, float eps, void* workspace, void* stream_) {
+    return flatten_forward_slots(vertices, edges, loss, B, V, E, eps, workspace, stream_);
+}
+extern "C" size_t umr_flatten_backward_workspace_bytes_deterministic(int32_t B, int32_t E) {
+    return flatten_backward_workspace_bytes<float>(B, E);
+}
+extern "C" int umr_flatten_backward_deterministic(const float* vertices, const int32_t* edges, const int32_t* vert_rowptr,
+                                                  const int32_t* vert_incidence, const float* grad_loss, float* grad_vertices,
+                                                  int32_t B, int32_t V, int32_t E, float eps, void* workspace, void* stream_) {
+    return flatten_backward_gather(vertices, edges, vert_rowptr, vert_incidence, grad_loss, grad_vertices, B, V, E, eps,
+                                   workspace, stream_);
+}
+
+// float64 (include/umr_b200.h, "float64 loss kernels"): the deterministic structure is the only one
+extern "C" size_t umr_laplacian_workspace_bytes_f64(int32_t B, int32_t V) { return laplacian_workspace_bytes<double>(B, V); }
+extern "C" int umr_laplacian_forward_f64(const double* x, const int32_t* rowptr, const int32_t* col, const double* coef,
+                                         double* y, double* loss, int32_t B, int32_t V, void* workspace, void* stream_) {
+    return laplacian_forward_slots(x, rowptr, col, coef, y, loss, B, V, workspace, stream_);
+}
+extern "C" int umr_laplacian_backward_f64(const double* y, const int32_t* rowptr, const int32_t* col, const double* tcoef,
+                                          const double* grad_loss, double* grad_x, int32_t B, int32_t V, void* stream_) {
+    return laplacian_backward(y, rowptr, col, tcoef, grad_loss, grad_x, B, V, stream_);
+}
+extern "C" size_t umr_flatten_forward_workspace_bytes_f64(int32_t B, int32_t E) { return flatten_forward_workspace_bytes<double>(B, E); }
+extern "C" int umr_flatten_forward_f64(const double* vertices, const int32_t* edges, double* loss, int32_t B, int32_t V,
+                                       int32_t E, double eps, void* workspace, void* stream_) {
+    return flatten_forward_slots(vertices, edges, loss, B, V, E, eps, workspace, stream_);
+}
+extern "C" size_t umr_flatten_backward_workspace_bytes_f64(int32_t B, int32_t E) { return flatten_backward_workspace_bytes<double>(B, E); }
+extern "C" int umr_flatten_backward_f64(const double* vertices, const int32_t* edges, const int32_t* vert_rowptr,
+                                        const int32_t* vert_incidence, const double* grad_loss, double* grad_vertices,
+                                        int32_t B, int32_t V, int32_t E, double eps, void* workspace, void* stream_) {
+    return flatten_backward_gather(vertices, edges, vert_rowptr, vert_incidence, grad_loss, grad_vertices, B, V, E, eps,
+                                   workspace, stream_);
 }

@@ -274,15 +274,6 @@ __device__ __forceinline__ void sample_texture(const double* __restrict__ tx, do
     }
 }
 
-__device__ __forceinline__ double warp_sum(double v) {
-    v += __shfl_xor_sync(0xffffffffu, v, 16);
-    v += __shfl_xor_sync(0xffffffffu, v, 8);
-    v += __shfl_xor_sync(0xffffffffu, v, 4);
-    v += __shfl_xor_sync(0xffffffffu, v, 2);
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
-    return v;
-}
-
 __device__ __forceinline__ void red_add_u64(unsigned long long* addr, unsigned long long v) {
     asm volatile("red.global.add.u64 [%0], %1;" ::"l"(addr), "l"(v) : "memory");
 }

@@ -14,21 +14,28 @@
 //
 // Compiled with -fmad=false and written in the reference's operation order, so the forward is
 // bit-identical to the torch-op chain (every torch elementwise op rounds to fp32).
+//
+// CorrLossChamfer's kernels are templated on the scalar type; the float64 entry points at the end of this file
+// (DESIGN.md §10) run their double instantiations with the deterministic float32 launchers.
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "umr_b200.h"
 
 namespace umr {
 
+template <typename T>
 struct Cam {
-    float s, tx, ty, q0, q1, q2, q3;
+    T s, tx, ty, q0, q1, q2, q3;
 };
 
-__device__ __forceinline__ Cam load_cam(const float* __restrict__ cams, int b) {
-    const float* c = cams + (size_t)b * 7;
-    Cam k;
+template <typename T>
+__device__ __forceinline__ Cam<T> load_cam(const T* __restrict__ cams, int b) {
+    const T* c = cams + (size_t)b * 7;
+    Cam<T> k;
     k.s = __ldg(c); k.tx = __ldg(c + 1); k.ty = __ldg(c + 2);
     k.q0 = __ldg(c + 3); k.q1 = __ldg(c + 4); k.q2 = __ldg(c + 5); k.q3 = __ldg(c + 6);
     return k;
@@ -36,14 +43,15 @@ __device__ __forceinline__ Cam load_cam(const float* __restrict__ cams, int b) {
 
 // quat_rotate (geom_utils.py:147-165): r = q (x) (0, X) (x) conj(q), products written out in the
 // reference's order (hamilton_product, :119-144).
-__device__ __forceinline__ void quat_rotate(const Cam& k, float x, float y, float z, float& r1, float& r2, float& r3) {
-    const float b0 = k.q0, b1 = -k.q1, b2 = -k.q2, b3 = -k.q3;  // conjugate
-    const float a0 = x * 0.f;                                    // X[:, :, [0]] * 0
+template <typename T>
+__device__ __forceinline__ void quat_rotate(const Cam<T>& k, T x, T y, T z, T& r1, T& r2, T& r3) {
+    const T b0 = k.q0, b1 = -k.q1, b2 = -k.q2, b3 = -k.q3;  // conjugate
+    const T a0 = x * T(0);                                   // X[:, :, [0]] * 0
     // t = (0, X) (x) conj(q)
-    const float t0 = a0 * b0 - x * b1 - y * b2 - z * b3;
-    const float t1 = a0 * b1 + x * b0 + y * b3 - z * b2;
-    const float t2 = a0 * b2 - x * b3 + y * b0 + z * b1;
-    const float t3 = a0 * b3 + x * b2 - y * b1 + z * b0;
+    const T t0 = a0 * b0 - x * b1 - y * b2 - z * b3;
+    const T t1 = a0 * b1 + x * b0 + y * b3 - z * b2;
+    const T t2 = a0 * b2 - x * b3 + y * b0 + z * b1;
+    const T t3 = a0 * b3 + x * b2 - y * b1 + z * b0;
     // r = q (x) t
     r1 = k.q0 * t1 + k.q1 * t0 + k.q2 * t3 - k.q3 * t2;
     r2 = k.q0 * t2 - k.q1 * t3 + k.q2 * t0 + k.q3 * t1;
@@ -59,7 +67,7 @@ struct ProjCfg {
 
 // raster-space position of one vertex; also returns the pre-look_at position (used for normals,
 // mesh.py:112-118 takes them before the transform)
-__device__ __forceinline__ void project(const Cam& k, const ProjCfg& c, float x, float y, float z, float* out,
+__device__ __forceinline__ void project(const Cam<float>& k, const ProjCfg& c, float x, float y, float z, float* out,
                                         float* pre) {
     float r1, r2, r3;
     quat_rotate(k, x, y, z, r1, r2, r3);
@@ -88,7 +96,7 @@ __global__ void __launch_bounds__(256) k_project_faces(const float* __restrict__
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
     const int b = blockIdx.y;
     if (f >= F) return;
-    const Cam k = load_cam(cams, b);
+    const auto k = load_cam(cams, b);
     const int vb = b / H;  // vertex / face batch item: H consecutive renders (camera hypotheses) share one mesh
     const int32_t* fi = faces + (size_t)vb * faces_bstride + (size_t)f * 3;
     float out[9], pre[9];
@@ -160,7 +168,7 @@ __global__ void __launch_bounds__(256) k_scatter_face_grads(const float* __restr
         const float* gl = glight + ((size_t)b * F + f) * 3;
         const float gc = lc.id * (lc.cd[0] * __ldg(gl) + lc.cd[1] * __ldg(gl + 1) + lc.cd[2] * __ldg(gl + 2));
         if (gc != 0.f) {
-            const Cam k = load_cam(cams, b);
+            const auto k = load_cam(cams, b);
             float out[9], pre[9];
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
@@ -220,7 +228,7 @@ __global__ void __launch_bounds__(256) k_project_backward(const float* __restric
     const int vb = b / H;  // H consecutive renders (camera hypotheses) share one vertex set
     float gc[7] = {0, 0, 0, 0, 0, 0, 0};
     if (v < V) {
-        const Cam k = load_cam(cams, b);
+        const auto k = load_cam(cams, b);
         const float* p = verts + ((size_t)vb * V + v) * 3;
         const float X = __ldg(p), Y = __ldg(p + 1), Z = __ldg(p + 2);
         const float* gp = gproj + ((size_t)b * V + v) * 3;
@@ -335,42 +343,45 @@ __global__ void k_cam_finalize(const float* __restrict__ slots, float* __restric
 // CTA per render: project the NS selected vertices (same arithmetic as k_project_faces: quat_rotate, scale, translate),
 // nearest target of the vertex's own part in the defined fp32 order of k_chamfer_nn (losses.cu), weighted mean.
 // ---------------------------------------------------------------------------------------------
+template <typename T>
 struct CorrCfg {
-    const float* tgt[4];   // [B, m[g], 2] target points of part g
-    int m[4];              // target counts
-    int end[4];            // exclusive end of part g in the concatenated vertex selection (loss_utils.py:211-216 `nums`)
-    float w[4];            // per-part weights (loss_utils.py:210: [1, 1, 0, 0])
+    const T* tgt[4];   // [B, m[g], 2] target points of part g
+    int m[4];          // target counts
+    int end[4];        // exclusive end of part g in the concatenated vertex selection (loss_utils.py:211-216 `nums`)
+    T w[4];            // per-part weights (loss_utils.py:210: [1, 1, 0, 0])
 };
 
-__device__ __forceinline__ int corr_part(const CorrCfg& c, int j) { return j < c.end[0] ? 0 : (j < c.end[1] ? 1 : (j < c.end[2] ? 2 : 3)); }
+template <typename T>
+__device__ __forceinline__ int corr_part(const CorrCfg<T>& c, int j) { return j < c.end[0] ? 0 : (j < c.end[1] ? 1 : (j < c.end[2] ? 2 : 3)); }
 
-__global__ void __launch_bounds__(256) k_corr_fwd(const float* __restrict__ verts, int64_t verts_bstride, const float* __restrict__ cams,
-                                                  const int32_t* __restrict__ sel, CorrCfg c, float* __restrict__ vert2d,
-                                                  int32_t* __restrict__ nn, float* __restrict__ loss, int NS) {
-    __shared__ float s_part[8];
+template <typename T>
+__global__ void __launch_bounds__(256) k_corr_fwd(const T* __restrict__ verts, int64_t verts_bstride, const T* __restrict__ cams,
+                                                  const int32_t* __restrict__ sel, CorrCfg<T> c, T* __restrict__ vert2d,
+                                                  int32_t* __restrict__ nn, T* __restrict__ loss, int NS) {
+    __shared__ T s_part[8];
     const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const Cam k = load_cam(cams, b);
-    float acc = 0.f;  // meaningful in lane 0
+    const auto k = load_cam(cams, b);
+    T acc = 0;  // meaningful in lane 0
     for (int j = warp; j < NS; j += 8) {
-        const float* p = verts + (size_t)b * verts_bstride + (size_t)__ldg(sel + j) * 3;
-        float r1, r2, r3;
+        const T* p = verts + (size_t)b * verts_bstride + (size_t)__ldg(sel + j) * 3;
+        T r1, r2, r3;
         quat_rotate(k, __ldg(p), __ldg(p + 1), __ldg(p + 2), r1, r2, r3);
-        const float qx = k.s * r1 + k.tx, qy = k.s * r2 + k.ty;   // orthographic_proj_withz(...)[:, :, :2] (geom_utils.py:74-91)
+        const T qx = k.s * r1 + k.tx, qy = k.s * r2 + k.ty;   // orthographic_proj_withz(...)[:, :, :2] (geom_utils.py:74-91)
         const int g = corr_part(c, j);
-        const float* tb = c.tgt[g] + (size_t)b * c.m[g] * 2;
-        const float qq = __fadd_rn(__fmul_rn(qx, qx), __fmul_rn(qy, qy));
-        float best = __int_as_float(0x7f800000);
+        const T* tb = c.tgt[g] + (size_t)b * c.m[g] * 2;
+        const T qq = add_rn(mul_rn(qx, qx), mul_rn(qy, qy));
+        T best = (T)INFINITY;
         int bi = 0x7fffffff;
         for (int t = lane; t < c.m[g]; t += 32) {
-            const float kx = __ldg(tb + 2 * t), ky = __ldg(tb + 2 * t + 1);
-            const float kk = __fadd_rn(__fmul_rn(kx, kx), __fmul_rn(ky, ky));
-            const float zz = __fadd_rn(__fmul_rn(qx, kx), __fmul_rn(qy, ky));
-            const float P = __fsub_rn(__fadd_rn(qq, kk), __fmul_rn(2.f, zz));  // chamfer_python.py:63, as k_chamfer_nn
+            const T kx = __ldg(tb + 2 * t), ky = __ldg(tb + 2 * t + 1);
+            const T kk = add_rn(mul_rn(kx, kx), mul_rn(ky, ky));
+            const T zz = add_rn(mul_rn(qx, kx), mul_rn(qy, ky));
+            const T P = sub_rn(add_rn(qq, kk), mul_rn(T(2), zz));  // chamfer_python.py:63, as k_chamfer_nn
             if (P < best) { best = P; bi = t; }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
-            const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const T ob = __shfl_xor_sync(0xffffffffu, best, o);
             const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
             if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
         }
@@ -384,75 +395,79 @@ __global__ void __launch_bounds__(256) k_corr_fwd(const float* __restrict__ vert
     if (lane == 0) s_part[warp] = acc;
     __syncthreads();
     if (threadIdx.x == 0) {
-        float t = 0.f;
+        T t = 0;
         for (int w = 0; w < 8; ++w) t += s_part[w];   // fixed order: deterministic
-        loss[b] = t / (float)NS;                      // torch.mean(torch.cat(terms, 1), 1) (:239)
+        loss[b] = t / (T)NS;                          // torch.mean(torch.cat(terms, 1), 1) (:239)
     }
 }
 
-// per-vertex backward of r = quat_rotate(q, X); p = s r + t given G = dL/dp (dL/dpz = gz): adds to gc[7] (scale, tx, ty, q0..q3)
-// and returns dL/dX (the derivation of k_project_backward).
-__device__ __forceinline__ void project_point_backward(const Cam& k, float X, float Y, float Z, float gx, float gy, float gz,
-                                                       float* gc, float& o0, float& o1, float& o2) {
-    float r1, r2, r3;
+// per-vertex backward of r = quat_rotate(q, X); p = s r + t given G = dL/dp with dL/dpz = 0: adds to gc[7] (scale, tx, ty,
+// q0..q3) and returns dL/dX (the derivation of k_project_backward).  float32 carries the zero z gradient through (s * 0 and
+// a 0 * r3 term), float64 uses an exact 0 with no r3 term; they differ only for a non-finite scale or r3 and in the sign
+// of a zero, and each precision keeps its bits.
+template <typename T>
+__device__ __forceinline__ void project_point_backward(const Cam<T>& k, T X, T Y, T Z, T gx, T gy, T* gc, T& o0, T& o1, T& o2) {
+    constexpr bool F32 = std::is_same<T, float>::value;
+    T r1, r2, r3;
     quat_rotate(k, X, Y, Z, r1, r2, r3);
-    gc[0] += gx * r1 + gy * r2 + gz * r3;
+    gc[0] += F32 ? gx * r1 + gy * r2 + T(0) * r3 : gx * r1 + gy * r2;
     gc[1] += gx;
     gc[2] += gy;
-    const float Gx = k.s * gx, Gy = k.s * gy, Gz = k.s * gz;
-    const float vx = k.q1, vy = k.q2, vz = k.q3, q0 = k.q0;
-    const float vv = vx * vx + vy * vy + vz * vz;
-    const float vG = vx * Gx + vy * Gy + vz * Gz;
-    const float vX = vx * X + vy * Y + vz * Z;
-    const float XG = X * Gx + Y * Gy + Z * Gz;
-    const float c0 = q0 * q0 - vv;
-    const float cx = vy * Gz - vz * Gy, cy = vz * Gx - vx * Gz, cz = vx * Gy - vy * Gx;  // v x G
-    o0 = c0 * Gx + 2.f * vG * vx - 2.f * q0 * cx;
-    o1 = c0 * Gy + 2.f * vG * vy - 2.f * q0 * cy;
-    o2 = c0 * Gz + 2.f * vG * vz - 2.f * q0 * cz;
-    const float wx = vy * Z - vz * Y, wy = vz * X - vx * Z, wz = vx * Y - vy * X;  // v x X
-    gc[3] += 2.f * (q0 * XG + (Gx * wx + Gy * wy + Gz * wz));
-    const float ex = Y * Gz - Z * Gy, ey = Z * Gx - X * Gz, ez = X * Gy - Y * Gx;  // X x G
-    gc[4] += 2.f * (-XG * vx + vG * X + vX * Gx + q0 * ex);
-    gc[5] += 2.f * (-XG * vy + vG * Y + vX * Gy + q0 * ey);
-    gc[6] += 2.f * (-XG * vz + vG * Z + vX * Gz + q0 * ez);
+    const T Gx = k.s * gx, Gy = k.s * gy, Gz = F32 ? k.s * T(0) : T(0);
+    const T vx = k.q1, vy = k.q2, vz = k.q3, q0 = k.q0;
+    const T vv = vx * vx + vy * vy + vz * vz;
+    const T vG = vx * Gx + vy * Gy + vz * Gz;
+    const T vX = vx * X + vy * Y + vz * Z;
+    const T XG = X * Gx + Y * Gy + Z * Gz;
+    const T c0 = q0 * q0 - vv;
+    const T cx = vy * Gz - vz * Gy, cy = vz * Gx - vx * Gz, cz = vx * Gy - vy * Gx;  // v x G
+    o0 = c0 * Gx + T(2) * vG * vx - T(2) * q0 * cx;
+    o1 = c0 * Gy + T(2) * vG * vy - T(2) * q0 * cy;
+    o2 = c0 * Gz + T(2) * vG * vz - T(2) * q0 * cz;
+    const T wx = vy * Z - vz * Y, wy = vz * X - vx * Z, wz = vx * Y - vy * X;  // v x X
+    gc[3] += T(2) * (q0 * XG + (Gx * wx + Gy * wy + Gz * wz));
+    const T ex = Y * Gz - Z * Gy, ey = Z * Gx - X * Gz, ez = X * Gy - Y * Gx;  // X x G
+    gc[4] += T(2) * (-XG * vx + vG * X + vX * Gx + q0 * ex);
+    gc[5] += T(2) * (-XG * vy + vG * Y + vX * Gy + q0 * ey);
+    gc[6] += T(2) * (-XG * vz + vG * Z + vX * Gz + q0 * ez);
 }
 
 // backward: grad_loss [B] (per render), optional grad_vert2d [B,NS,2] -> grad_verts [B,V,3] (zero-filled by the host,
 // atomics: a vertex may sit in several parts) and grad_cams [B,7].  Targets are constants (the reference's are data).
-// DET: `gverts` is the per-(render, j) term array [B,NS,3] (plain stores), summed per vertex by k_corr_gather.
-template <bool DET>
-__global__ void __launch_bounds__(256) k_corr_bwd(const float* __restrict__ verts, int64_t verts_bstride, const float* __restrict__ cams,
-                                                  const int32_t* __restrict__ sel, CorrCfg c, const float* __restrict__ vert2d,
-                                                  const int32_t* __restrict__ nn, const float* __restrict__ grad_loss,
-                                                  const float* __restrict__ grad_vert2d, float* __restrict__ gverts,
-                                                  float* __restrict__ gcams, int NS, int V) {
-    __shared__ float s[8][7];
+// DET: `gverts` is the per-(render, j) term array [B,NS,3] (plain stores), summed per vertex by k_gather3.  Float64 runs
+// only the DET form.
+template <typename T, bool DET>
+__global__ void __launch_bounds__(256) k_corr_bwd(const T* __restrict__ verts, int64_t verts_bstride, const T* __restrict__ cams,
+                                                  const int32_t* __restrict__ sel, CorrCfg<T> c, const T* __restrict__ vert2d,
+                                                  const int32_t* __restrict__ nn, const T* __restrict__ grad_loss,
+                                                  const T* __restrict__ grad_vert2d, T* __restrict__ gverts,
+                                                  T* __restrict__ gcams, int NS, int V) {
+    __shared__ T s[8][7];
     const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const Cam k = load_cam(cams, b);
-    const float gl = __ldg(grad_loss + b) / (float)NS;
-    float gc[7] = {0, 0, 0, 0, 0, 0, 0};
+    const auto k = load_cam(cams, b);
+    const T gl = __ldg(grad_loss + b) / (T)NS;
+    T gc[7] = {0, 0, 0, 0, 0, 0, 0};
     for (int j = threadIdx.x; j < NS; j += 256) {
         const int g = corr_part(c, j);
         const int vi = __ldg(sel + j);
-        const float* p = verts + (size_t)b * verts_bstride + (size_t)vi * 3;
-        const float qx = __ldg(vert2d + ((size_t)b * NS + j) * 2), qy = __ldg(vert2d + ((size_t)b * NS + j) * 2 + 1);
-        const float* t = c.tgt[g] + ((size_t)b * c.m[g] + __ldg(nn + (size_t)b * NS + j)) * 2;
-        const float gd = gl * c.w[g];
+        const T* p = verts + (size_t)b * verts_bstride + (size_t)vi * 3;
+        const T qx = __ldg(vert2d + ((size_t)b * NS + j) * 2), qy = __ldg(vert2d + ((size_t)b * NS + j) * 2 + 1);
+        const T* t = c.tgt[g] + ((size_t)b * c.m[g] + __ldg(nn + (size_t)b * NS + j)) * 2;
+        const T gd = gl * c.w[g];
         // d/dq of (|q|^2 + |t|^2 - 2 q.t) = 2 q - 2 t (chamfer_python.py:63; the argmin is piecewise constant)
-        float gx = gd * (2.f * qx - 2.f * __ldg(t)), gy = gd * (2.f * qy - 2.f * __ldg(t + 1));
+        T gx = gd * (T(2) * qx - T(2) * __ldg(t)), gy = gd * (T(2) * qy - T(2) * __ldg(t + 1));
         if (grad_vert2d != nullptr) {
             gx += __ldg(grad_vert2d + ((size_t)b * NS + j) * 2);
             gy += __ldg(grad_vert2d + ((size_t)b * NS + j) * 2 + 1);
         }
-        float o0, o1, o2;
-        project_point_backward(k, __ldg(p), __ldg(p + 1), __ldg(p + 2), gx, gy, 0.f, gc, o0, o1, o2);
+        T o0, o1, o2;
+        project_point_backward(k, __ldg(p), __ldg(p + 1), __ldg(p + 2), gx, gy, gc, o0, o1, o2);
         if (gverts != nullptr) {
             if (DET) {
-                float* o = gverts + ((size_t)b * NS + j) * 3;
+                T* o = gverts + ((size_t)b * NS + j) * 3;
                 o[0] = o0; o[1] = o1; o[2] = o2;
             } else {
-                float* o = gverts + ((size_t)b * V + vi) * 3;
+                T* o = gverts + ((size_t)b * V + vi) * 3;
                 atomicAdd(o, o0); atomicAdd(o + 1, o1); atomicAdd(o + 2, o2);
             }
         }
@@ -460,31 +475,15 @@ __global__ void __launch_bounds__(256) k_corr_bwd(const float* __restrict__ vert
     if (gcams == nullptr) return;
 #pragma unroll
     for (int i = 0; i < 7; ++i) {
-        const float r = warp_sum(gc[i]);
+        const T r = warp_sum(gc[i]);
         if (lane == 0) s[warp][i] = r;
     }
     __syncthreads();
     if (threadIdx.x < 7) {
-        float r = 0.f;
+        T r = 0;
         for (int w = 0; w < 8; ++w) r += s[w][threadIdx.x];
         gcams[(size_t)b * 7 + threadIdx.x] = r;   // one CTA per render: plain store
     }
-}
-// grad_verts[b][v] = sum of v's (render, j) terms over the transposed selection table: vrowptr [V+1], vsel [NS] lists the
-// j with selection[j] == v in ascending order, so the sum order is fixed; an unselected vertex gets 0
-__global__ void __launch_bounds__(256) k_corr_gather(const float* __restrict__ terms, const int32_t* __restrict__ vrowptr,
-                                                     const int32_t* __restrict__ vsel, float* __restrict__ gverts, int NS, int V) {
-    const int b = blockIdx.y;
-    const int v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= V) return;
-    const float* tb = terms + (size_t)b * NS * 3;
-    float g0 = 0.f, g1 = 0.f, g2 = 0.f;
-    for (int k = __ldg(vrowptr + v); k < __ldg(vrowptr + v + 1); ++k) {
-        const float* t = tb + (size_t)__ldg(vsel + k) * 3;
-        g0 += t[0]; g1 += t[1]; g2 += t[2];
-    }
-    float* o = gverts + ((size_t)b * V + v) * 3;
-    o[0] = g0; o[1] = g1; o[2] = g2;
 }
 
 }  // namespace umr
@@ -588,8 +587,9 @@ extern "C" int umr_project_faces_backward_deterministic(const float* vertices, c
     return (int)cudaGetLastError();
 }
 
-static int make_corr_cfg(CorrCfg& c, const float* const* targets, const int32_t* target_counts, const int32_t* part_ends,
-                         const float* weights, int NS) {
+template <typename T>
+static int make_corr_cfg(CorrCfg<T>& c, const T* const* targets, const int32_t* target_counts, const int32_t* part_ends,
+                         const T* weights, int NS) {
     int prev = 0;
     for (int g = 0; g < 4; ++g) {
         if (!targets[g] || target_counts[g] <= 0 || part_ends[g] < prev) return UMR_ERR_BAD_ARG;
@@ -599,19 +599,29 @@ static int make_corr_cfg(CorrCfg& c, const float* const* targets, const int32_t*
     return prev == NS ? UMR_OK : UMR_ERR_BAD_ARG;
 }
 
+// float32 and float64
+template <typename T>
+static int corr_chamfer_forward(const T* vertices, int64_t vertices_batch_stride, const T* cams, const int32_t* selection,
+                                const T* const* targets, const int32_t* target_counts, const int32_t* part_ends,
+                                const T* weights, T* vert2d, int32_t* nearest, T* loss, int32_t B, int32_t NS, void* stream_) {
+    if (!vertices || !cams || !selection || !targets || !target_counts || !part_ends || !weights || !vert2d || !nearest ||
+        !loss || B <= 0 || NS <= 0)
+        return UMR_ERR_BAD_ARG;
+    CorrCfg<T> c;
+    const int rc = make_corr_cfg(c, targets, target_counts, part_ends, weights, NS);
+    if (rc) return rc;
+    count_launch();
+    k_corr_fwd<T><<<B, 256, 0, (cudaStream_t)stream_>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest,
+                                                        loss, NS);
+    return (int)cudaGetLastError();
+}
+
 extern "C" int umr_corr_chamfer_forward(const float* vertices, int64_t vertices_batch_stride, const float* cams,
                                         const int32_t* selection, const float* const* targets, const int32_t* target_counts,
                                         const int32_t* part_ends, const float* weights, float* vert2d, int32_t* nearest,
                                         float* loss, int32_t B, int32_t NS, void* stream_) {
-    if (!vertices || !cams || !selection || !targets || !target_counts || !part_ends || !weights || !vert2d || !nearest ||
-        !loss || B <= 0 || NS <= 0)
-        return UMR_ERR_BAD_ARG;
-    CorrCfg c;
-    const int rc = make_corr_cfg(c, targets, target_counts, part_ends, weights, NS);
-    if (rc) return rc;
-    count_launch();
-    k_corr_fwd<<<B, 256, 0, (cudaStream_t)stream_>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, loss, NS);
-    return (int)cudaGetLastError();
+    return corr_chamfer_forward(vertices, vertices_batch_stride, cams, selection, targets, target_counts, part_ends, weights,
+                                vert2d, nearest, loss, B, NS, stream_);
 }
 
 extern "C" int umr_corr_chamfer_backward(const float* vertices, int64_t vertices_batch_stride, const float* cams,
@@ -622,7 +632,7 @@ extern "C" int umr_corr_chamfer_backward(const float* vertices, int64_t vertices
     if (!vertices || !cams || !selection || !targets || !target_counts || !part_ends || !weights || !vert2d || !nearest ||
         !grad_loss || B <= 0 || NS <= 0 || V <= 0)
         return UMR_ERR_BAD_ARG;
-    CorrCfg c;
+    CorrCfg<float> c;
     const int rc = make_corr_cfg(c, targets, target_counts, part_ends, weights, NS);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream_;
@@ -631,16 +641,45 @@ extern "C" int umr_corr_chamfer_backward(const float* vertices, int64_t vertices
         if (e != cudaSuccess) return (int)e;
     }
     count_launch();
-    k_corr_bwd<false><<<B, 256, 0, st>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss, grad_vert2d,
-                                  grad_vertices, grad_cams, NS, V);
+    k_corr_bwd<float, false><<<B, 256, 0, st>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss,
+                                                grad_vert2d, grad_vertices, grad_cams, NS, V);
     return (int)cudaGetLastError();
 }
 
-// Deterministic backward (include/umr_b200.h): k_corr_bwd<true> stores the per-(render, j) vertex terms in the workspace,
-// k_corr_gather sums them per vertex in ascending j.  grad_cams is the default kernel's plain store.
-extern "C" size_t umr_corr_chamfer_workspace_bytes_deterministic(int32_t B, int32_t NS) {
+// Deterministic float32 and float64 backward (include/umr_b200.h): k_corr_bwd<T, true> stores the per-(render, j) vertex
+// terms in the workspace, k_gather3 sums them per vertex in ascending j.  grad_cams is the kernel's plain store.
+template <typename T>
+static size_t corr_chamfer_workspace_bytes(int32_t B, int32_t NS) {
     if (B <= 0 || NS <= 0) return 0;
-    return (size_t)B * NS * 3 * sizeof(float);
+    return (size_t)B * NS * 3 * sizeof(T);
+}
+template <typename T>
+static int corr_chamfer_backward_gather(const T* vertices, int64_t vertices_batch_stride, const T* cams, const int32_t* selection,
+                                        const T* const* targets, const int32_t* target_counts, const int32_t* part_ends,
+                                        const T* weights, const T* vert2d, const int32_t* nearest, const T* grad_loss,
+                                        const T* grad_vert2d, T* grad_vertices, T* grad_cams, int32_t B, int32_t NS, int32_t V,
+                                        const int32_t* vert_rowptr, const int32_t* vert_selection, void* workspace,
+                                        void* stream_) {
+    if (!vertices || !cams || !selection || !targets || !target_counts || !part_ends || !weights || !vert2d || !nearest ||
+        !grad_loss || B <= 0 || NS <= 0 || V <= 0)
+        return UMR_ERR_BAD_ARG;
+    if (grad_vertices && (!vert_rowptr || !vert_selection || !workspace)) return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    CorrCfg<T> c;
+    const int rc = make_corr_cfg(c, targets, target_counts, part_ends, weights, NS);
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream_;
+    T* terms = grad_vertices ? (T*)workspace : nullptr;
+    count_launch(grad_vertices ? 2 : 1);
+    k_corr_bwd<T, true><<<B, 256, 0, st>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss,
+                                           grad_vert2d, terms, grad_cams, NS, V);
+    if (grad_vertices)
+        k_gather3<T><<<dim3((V + 255) / 256, B), 256, 0, st>>>(terms, vert_rowptr, vert_selection, grad_vertices, V, (int64_t)NS);
+    return (int)cudaGetLastError();
+}
+
+extern "C" size_t umr_corr_chamfer_workspace_bytes_deterministic(int32_t B, int32_t NS) {
+    return corr_chamfer_workspace_bytes<float>(B, NS);
 }
 extern "C" int umr_corr_chamfer_backward_deterministic(const float* vertices, int64_t vertices_batch_stride, const float* cams,
                                                        const int32_t* selection, const float* const* targets,
@@ -650,20 +689,29 @@ extern "C" int umr_corr_chamfer_backward_deterministic(const float* vertices, in
                                                        float* grad_cams, int32_t B, int32_t NS, int32_t V,
                                                        const int32_t* vert_rowptr, const int32_t* vert_selection,
                                                        void* workspace, void* stream_) {
-    if (!vertices || !cams || !selection || !targets || !target_counts || !part_ends || !weights || !vert2d || !nearest ||
-        !grad_loss || B <= 0 || NS <= 0 || V <= 0)
-        return UMR_ERR_BAD_ARG;
-    if (grad_vertices && (!vert_rowptr || !vert_selection || !workspace)) return UMR_ERR_BAD_ARG;
-    if (B > 65535) return UMR_ERR_TOO_LARGE;
-    CorrCfg c;
-    const int rc = make_corr_cfg(c, targets, target_counts, part_ends, weights, NS);
-    if (rc) return rc;
-    cudaStream_t st = (cudaStream_t)stream_;
-    float* terms = grad_vertices ? (float*)workspace : nullptr;
-    count_launch(grad_vertices ? 2 : 1);
-    k_corr_bwd<true><<<B, 256, 0, st>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss, grad_vert2d,
-                                        terms, grad_cams, NS, V);
-    if (grad_vertices)
-        k_corr_gather<<<dim3((V + 255) / 256, B), 256, 0, st>>>(terms, vert_rowptr, vert_selection, grad_vertices, NS, V);
-    return (int)cudaGetLastError();
+    return corr_chamfer_backward_gather(vertices, vertices_batch_stride, cams, selection, targets, target_counts, part_ends,
+                                        weights, vert2d, nearest, grad_loss, grad_vert2d, grad_vertices, grad_cams, B, NS, V,
+                                        vert_rowptr, vert_selection, workspace, stream_);
+}
+
+// float64 (include/umr_b200.h, "float64 loss kernels")
+extern "C" int umr_corr_chamfer_forward_f64(const double* vertices, int64_t vertices_batch_stride, const double* cams,
+                                            const int32_t* selection, const double* const* targets,
+                                            const int32_t* target_counts, const int32_t* part_ends, const double* weights,
+                                            double* vert2d, int32_t* nearest, double* loss, int32_t B, int32_t NS,
+                                            void* stream_) {
+    return corr_chamfer_forward(vertices, vertices_batch_stride, cams, selection, targets, target_counts, part_ends, weights,
+                                vert2d, nearest, loss, B, NS, stream_);
+}
+extern "C" size_t umr_corr_chamfer_workspace_bytes_f64(int32_t B, int32_t NS) { return corr_chamfer_workspace_bytes<double>(B, NS); }
+extern "C" int umr_corr_chamfer_backward_f64(const double* vertices, int64_t vertices_batch_stride, const double* cams,
+                                             const int32_t* selection, const double* const* targets,
+                                             const int32_t* target_counts, const int32_t* part_ends, const double* weights,
+                                             const double* vert2d, const int32_t* nearest, const double* grad_loss,
+                                             const double* grad_vert2d, double* grad_vertices, double* grad_cams, int32_t B,
+                                             int32_t NS, int32_t V, const int32_t* vert_rowptr, const int32_t* vert_selection,
+                                             void* workspace, void* stream_) {
+    return corr_chamfer_backward_gather(vertices, vertices_batch_stride, cams, selection, targets, target_counts, part_ends,
+                                        weights, vert2d, nearest, grad_loss, grad_vert2d, grad_vertices, grad_cams, B, NS, V,
+                                        vert_rowptr, vert_selection, workspace, stream_);
 }
