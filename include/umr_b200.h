@@ -234,7 +234,9 @@ int umr_project_faces_backward(const float* vertices, const float* cams, const i
  * image [B,C,H,W], flow [B,N,2] (x,y in [-1,1]) -> out [B,N,C] (i.e. already permuted to the
  * `B x F x T x T x C` order sample_textures returns).  Backward: gradient w.r.t. flow only
  * (grad_flow [B,N,2], fully written) -- and optionally w.r.t. image (grad_image [B,C,H,W],
- * zero-filled by the call then accumulated; NULL to skip). */
+ * zero-filled by the call then accumulated; NULL to skip).  flow and grad_flow are read / written as (x,y) pairs:
+ * their addresses must be multiples of 2 * sizeof(element) (8 bytes here, 16 in the _f64 forms), else UMR_ERR_BAD_ARG;
+ * the same holds for umr_bilinear_sample_cells and every _deterministic / _f64 form. */
 int umr_bilinear_sample_forward(const float* image, const float* flow, float* out, int32_t B,
                                 int32_t C, int32_t H, int32_t W, int32_t N, void* stream);
 int umr_bilinear_sample_backward(const float* image, const float* flow, const float* grad_out,
@@ -310,7 +312,9 @@ int umr_corr_chamfer_backward(const float* vertices, int64_t vertices_batch_stri
 /* TexCycle (loss_utils.py:152-182).  flow [B,F,T2,2], prob [B,F,2], face_ids [B,P] (the hard
  * renderer's aggrs_info[:,1] plane as float, -1 = background which marks face F-1 visible like the
  * reference's negative index does).  visible [B,F] (uint8 scratch, written), loss[1].
- * Backward: grad_flow [B,F,T2,2] = grad_loss * dloss/dflow. */
+ * Backward: grad_flow [B,F,T2,2] = grad_loss * dloss/dflow.  flow, prob and grad_flow are read / written as (x,y) pairs:
+ * their addresses must be multiples of 2 * sizeof(element) (8 bytes here, 16 in the _f64 forms), else UMR_ERR_BAD_ARG,
+ * in every form.  B * F > INT32_MAX returns UMR_ERR_TOO_LARGE. */
 int umr_texcycle_forward(const float* flow, const float* prob, const float* face_ids,
                          uint8_t* visible, float* loss, int32_t B, int32_t F, int32_t T2,
                          int64_t P, void* stream);

@@ -14,9 +14,10 @@ Each function cites the reference lines it follows:
   flatten_ref       SoftRas/losses.py:39-114 `FlattenLoss`
   edt_sq_brute / dt_barrier_ref   utils/image.py:130-141 `compute_dt_barrier` (scipy's distance_transform_edt)
 
-Two places keep float32 on purpose:
-* The sampler's coordinate map is computed in float32, as torch and the kernel do: `floor` of it then falls on the same
-  side of a texel boundary, and everything after it is float64.  Its gradient is the exact (W - 1) / 2.
+Two places keep the kernel's precision on purpose:
+* The sampler's coordinate map is computed in the kernel's precision (float32 by default, as torch and the float32
+  kernel do; `map_dtype=torch.float64` for the float64 kernel): `floor` of it then falls on the same side of a texel
+  boundary, and everything after it is float64.  Its gradient is the exact (W - 1) / 2.
 * Chamfer: the caller may pass the kernel's nearest indices after checking that each differing one is a near-tie; the
   distances and gradients then follow that choice.
 
@@ -29,9 +30,9 @@ bound from the sensitivity of the result to a relative perturbation of every rou
 import numpy as np
 import torch
 
-from vertex_ref import U32, gamma
+from vertex_ref import U32, U64, gamma
 
-__all__ = ["U32", "gamma", "sample_ref", "sample_magnitude", "iou_ref", "masked_l1_ref", "loss_head_ref", "chamfer_ref",
+__all__ = ["U32", "U64", "gamma", "sample_ref", "sample_magnitude", "iou_ref", "masked_l1_ref", "loss_head_ref", "chamfer_ref",
            "near_tie", "visible_ref", "texcycle_ref", "laplacian_ref", "flatten_ref", "flatten_error_bound", "spiked_uv_sphere",
            "edt_sq_brute", "dt_barrier_ref"]
 
@@ -39,24 +40,25 @@ __all__ = ["U32", "gamma", "sample_ref", "sample_magnitude", "iou_ref", "masked_
 # -------------------------------------------------------------------------------------------------
 # bilinear sampler
 # -------------------------------------------------------------------------------------------------
-def _coords(flow, W, H):
-    """float32 pixel coordinates of flow [B,N,2] exactly as torch / k_sample_* compute them, as float64 tensors that
-    carry the map's exact derivative (W - 1) / 2 when `flow` requires grad."""
-    f = flow.detach().float()
-    ix32 = ((f[..., 0] + 1) / 2) * (W - 1)
-    iy32 = ((f[..., 1] + 1) / 2) * (H - 1)
-    ix, iy = ix32.double(), iy32.double()
+def _coords(flow, W, H, map_dtype):
+    """Pixel coordinates of flow [B,N,2] in `map_dtype` exactly as torch / k_sample_* compute them, ((x + 1) / 2) * (W - 1)
+    with each operation rounded once, and as float64 tensors that carry the map's exact derivative (W - 1) / 2 when
+    `flow` requires grad."""
+    f = flow.detach().to(map_dtype)
+    ixm = ((f[..., 0] + 1) / 2) * (W - 1)
+    iym = ((f[..., 1] + 1) / 2) * (H - 1)
+    ix, iy = ixm.double(), iym.double()
     if flow.requires_grad:
         fx, fy = flow[..., 0].double(), flow[..., 1].double()
         ix = ix + (fx * ((W - 1) / 2) - (fx * ((W - 1) / 2)).detach())
         iy = iy + (fy * ((H - 1) / 2) - (fy * ((H - 1) / 2)).detach())
-    return ix32, iy32, ix, iy
+    return ixm, iym, ix, iy
 
 
-def _corners(image, ix32, iy32):
+def _corners(image, ixm, iym):
     """The four corners of every sample: [(x, y, valid [B,N], value [B,C,N])] in the order 00, 10, 01, 11."""
     B, C, H, W = image.shape
-    x0, y0 = torch.floor(ix32).double(), torch.floor(iy32).double()
+    x0, y0 = torch.floor(ixm).double(), torch.floor(iym).double()
     out = []
     for dx, dy in ((0, 0), (1, 0), (0, 1), (1, 1)):
         x, y = x0 + dx, y0 + dy
@@ -67,23 +69,24 @@ def _corners(image, ix32, iy32):
     return out
 
 
-def sample_ref(image, flow):
-    """grid_sample(image, flow, bilinear, zeros, align_corners=True): image [B,C,H,W] float64, flow [B,N,2] (float32
-    values; float64 leaves for gradients) -> [B,N,C] float64."""
+def sample_ref(image, flow, map_dtype=torch.float32):
+    """grid_sample(image, flow, bilinear, zeros, align_corners=True): image [B,C,H,W] float64, flow [B,N,2] (values of
+    `map_dtype`, the precision of the kernel's coordinate map; float64 leaves for gradients) -> [B,N,C] float64."""
     B, C, H, W = image.shape
-    ix32, iy32, ix, iy = _coords(flow, W, H)
-    (x0, y0, _, a00), (x1, _, _, a10), (_, y1, _, a01), (_, _, _, a11) = _corners(image, ix32, iy32)
+    ixm, iym, ix, iy = _coords(flow, W, H, map_dtype)
+    (x0, y0, _, a00), (x1, _, _, a10), (_, y1, _, a01), (_, _, _, a11) = _corners(image, ixm, iym)
     wx1, wx0, wy1, wy0 = x1 - ix, ix - x0, y1 - iy, iy - y0
     out = a00 * (wx1 * wy1)[:, None] + a10 * (wx0 * wy1)[:, None] + a01 * (wx1 * wy0)[:, None] + a11 * (wx0 * wy0)[:, None]
     return out.permute(0, 2, 1)
 
 
-def sample_magnitude(image, flow, g):
+def sample_magnitude(image, flow, g, map_dtype=torch.float32):
     """Magnitudes of the sampler's outputs for the error bounds: (out [B,N,C], grad_flow [B,N,2], grad_image [B,C,H,W],
-    the largest number of corner terms one pixel receives).  g [B,N,C] is the upstream gradient."""
+    the largest number of corner terms one pixel receives).  g [B,N,C] is the upstream gradient; `map_dtype` as in
+    `sample_ref`."""
     B, C, H, W = image.shape
-    ix32, iy32, ix, iy = _coords(flow.detach(), W, H)
-    cs = _corners(image.abs(), ix32, iy32)
+    ixm, iym, ix, iy = _coords(flow.detach(), W, H, map_dtype)
+    cs = _corners(image.abs(), ixm, iym)
     (x0, y0, k00, a00), (x1, _, k10, a10), (_, y1, k01, a01), (_, _, k11, a11) = cs
     wx1, wx0, wy1, wy0 = x1 - ix, ix - x0, y1 - iy, iy - y0
     w = (wx1 * wy1, wx0 * wy1, wx1 * wy0, wx0 * wy0)
@@ -156,14 +159,15 @@ def chamfer_ref(a, b, idx_ab=None, idx_ba=None, magnitude=False):
     return d_ab, d_ba, idx_ab, idx_ba
 
 
-def near_tie(a, b, idx_kernel, idx_ref, dim):
+def near_tie(a, b, idx_kernel, idx_ref, dim, n=6, u=U32):
     """True where the kernel's nearest index is the float64 one or a near-tie of it: the two float64 distances differ
-    by no more than both distances' float32 rounding bound (the rule of test_losses_gpu.py::test_chamfer, with the
-    bound gamma_6 * magnitude of the expanded form instead of a fixed 4.8e-7)."""
+    by no more than both distances' rounding bound gamma_n(u) * magnitude of the expanded form (the rule of
+    test_losses_gpu.py::test_chamfer, with that bound instead of a fixed 4.8e-7).  The default n = 6, u = 2^-24 suits
+    the float32 kernel; a float64 kernel against this float64 reference counts both evaluations' roundings."""
     P, Pm = _sqdist(a, b), _sqdist(a.abs(), b.abs(), magnitude=True)
     pick = lambda X, i: torch.gather(X, dim, i.long().unsqueeze(dim)).squeeze(dim)   # noqa: E731
     diff = (pick(P, idx_kernel) - pick(P, idx_ref)).abs()
-    return (idx_kernel.long() == idx_ref.long()) | (diff <= gamma(6) * (pick(Pm, idx_kernel) + pick(Pm, idx_ref)))
+    return (idx_kernel.long() == idx_ref.long()) | (diff <= gamma(n, u) * (pick(Pm, idx_kernel) + pick(Pm, idx_ref)))
 
 
 # -------------------------------------------------------------------------------------------------
@@ -253,8 +257,9 @@ def flatten_ref(vertices, edges, eps=1e-6):
     return _flatten_terms(P, eps, _Rounder(False)).sum(1)
 
 
-def flatten_error_bound(vertices, edges, eps, grad_loss, reduce_depth):
-    """First-order bounds on k_flatten's float32 error: (loss [B], grad_vertices [B,V,3]).
+def flatten_error_bound(vertices, edges, eps, grad_loss, reduce_depth, u=U32):
+    """First-order bounds on k_flatten's error at unit roundoff u (U32 for the float32 kernel, U64 for the float64 one):
+    (loss [B], grad_vertices [B,V,3]).
 
     Every rounded operation of the kernel is one `_Rounder` perturbation of relative size <= u, so the error of an
     edge's term is at most u * sum |d term / d delta| to first order.  The forward is one perturbation per operation,
@@ -272,20 +277,20 @@ def flatten_error_bound(vertices, edges, eps, grad_loss, reduce_depth):
     G, = torch.autograd.grad((t * gl).sum(), P, create_graph=True)                 # [B,E,4,3] per-edge terms
     per_edge = lambda ds: sum(d.abs().reshape(B, E, -1).sum(-1) for d in ds if d is not None)   # noqa: E731
     sens_t = per_edge(torch.autograd.grad(t.sum(), r.deltas, retain_graph=True, allow_unused=True))
-    loss_bound = 2 * U32 * sens_t.sum(1) + gamma(reduce_depth) * t.detach().abs().sum(1)
+    loss_bound = 2 * u * sens_t.sum(1) + gamma(reduce_depth, u) * t.detach().abs().sum(1)
     sens_g = torch.zeros(B, E, 4, 3, dtype=torch.float64)
     for k in range(4):
         for d in range(3):
             ds = torch.autograd.grad(G[:, :, k, d].sum(), r.deltas, retain_graph=True, allow_unused=True)
             sens_g[:, :, k, d] = per_edge(ds)
     Gd = G.detach()
-    term_bound = 8 * U32 * sens_g
-    term_bound[:, :, 0] += gamma(2) * Gd[:, :, 1:].abs().sum(2)
+    term_bound = 8 * u * sens_g
+    term_bound[:, :, 0] += gamma(2, u) * Gd[:, :, 1:].abs().sum(2)
     count = torch.bincount(idx.reshape(-1), minlength=V).max().item()
     flat = idx.reshape(-1)
     gb = torch.zeros(B, V, 3, dtype=torch.float64).index_add_(1, flat, term_bound.reshape(B, E * 4, 3))
     ga = torch.zeros(B, V, 3, dtype=torch.float64).index_add_(1, flat, Gd.abs().reshape(B, E * 4, 3))
-    return loss_bound, gb + gamma(count + 2) * ga
+    return loss_bound, gb + gamma(count + 2, u) * ga
 
 
 def spiked_uv_sphere(n_lat, n_lon, n_spikes):

@@ -97,11 +97,13 @@ def project_faces_ref(vertices, cams, faces, offset_z=5.0, eye_z=-2.732, viewing
 
 
 U32 = 2.0 ** -24   # unit roundoff of float32
+U64 = 2.0 ** -53   # unit roundoff of float64
 
 
-def gamma(n):
-    """gamma_n = n u / (1 - n u): the relative error bound of n float32 roundings in a chain."""
-    return n * U32 / (1 - n * U32)
+def gamma(n, u=U32):
+    """gamma_n = n u / (1 - n u): the relative error bound of n roundings in a chain at unit roundoff u (float32 by
+    default, U64 for float64)."""
+    return n * u / (1 - n * u)
 
 
 def normal_conditioning(vertices, cams, faces, offset_z, flip_y, exact_corners=False):

@@ -413,6 +413,59 @@ def run_entry(name, mode):
     return outs, leaves
 
 
+def _odd_offset(t):
+    """A contiguous view of `t` one element into a fresh buffer: aligned to the element, never to an (x, y) pair."""
+    buf = torch.zeros(t.numel() + 1, dtype=t.dtype)
+    v = buf[1:].view(t.shape)
+    v.copy_(t.detach())
+    assert v.data_ptr() % (2 * v.element_size()) != 0
+    return v.requires_grad_(t.requires_grad)
+
+
+# symbol prefix -> the positions of its (x, y)-pair pointer arguments (include/umr_b200.h)
+PAIR_ARGS = {"umr_bilinear_sample_forward": (1,), "umr_bilinear_sample_cells": (0,), "umr_bilinear_sample_backward": (1, 3),
+             "umr_texcycle_forward": (0, 1), "umr_texcycle_backward": (0, 1, 4)}
+
+
+@pytest.mark.parametrize("mode", ["f32", "det", "f64", "mixed"])
+@pytest.mark.parametrize("op", ["sample", "texcycle"])
+def test_odd_offset_pairs_reach_the_library_aligned(fake, op, mode):
+    """Contiguous flow / prob views at an odd element offset: every pair pointer the library receives, forward and
+    backward, is a multiple of 2 * sizeof(element), and an input already aligned in the compute dtype is passed in place."""
+    dt = _dtypes(mode)
+    det = torch.are_deterministic_algorithms_enabled()
+    torch.use_deterministic_algorithms(mode == "det")
+    try:
+        if op == "sample":
+            img, flow = _rand((2, 3, 4, 5), dt(0), True), _odd_offset(_rand((2, 6, 2), dt(1), True))
+            aligned = _rand((2, 6, 2), dt(1), True)
+            ops.bilinear_sample(img, flow).sum().backward()
+            ops.bilinear_sample(img, aligned).sum().backward()
+        else:
+            flow, prob = _odd_offset(_rand((2, 3, 4, 2), dt(0), True)), _odd_offset(_rand((2, 3, 2), dt(1)))
+            vis = torch.tensor([[1, 0, 1], [1, 1, 0]], dtype=torch.uint8)
+            aligned = _rand((2, 3, 4, 2), dt(0), True)
+            ops.tex_cycle(flow, prob, None, vis).backward()
+            ops.tex_cycle(aligned, prob, None, vis).backward()
+    finally:
+        torch.use_deterministic_algorithms(det)
+    assert flow.grad is not None and flow.grad.dtype == flow.dtype
+    seen = 0
+    for name, args in fake.calls:
+        pos = [p for prefix, p in PAIR_ARGS.items() if name.startswith(prefix)]
+        if not pos:
+            continue
+        size = 8 if name.endswith("_f64") else 4
+        for k in pos[0]:
+            assert args[k].value % (2 * size) == 0, "%s: argument %d at %#x" % (name, k, args[k].value)
+            seen += 1
+    assert seen >= (6 if op == "sample" else 10)
+    # the second call's flow reaches the library in place when it already has the compute dtype
+    forwards = [args for name, args in fake.calls if name.startswith(("umr_bilinear_sample_forward", "umr_texcycle_forward"))]
+    if aligned.dtype == (torch.float64 if mode in ("f64", "mixed") else torch.float32):
+        assert forwards[-1][1 if op == "sample" else 0].value == aligned.data_ptr()
+
+
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("name", sorted(ENTRIES))
 def test_dispatch(fake, name, mode):

@@ -82,6 +82,46 @@ def test_bad_arguments_refused():
                                              9, N0, N0, N0, None) == UMR_ERR_TOO_LARGE
 
 
+def test_misaligned_vector_pointers_refused():
+    """The sampler's flow / grad_flow and TexCycle's flow / prob / grad_flow are read as (x, y) vector pairs: a pointer
+    that is not a multiple of 2 * sizeof(element) is refused with UMR_ERR_BAD_ARG in every precision, before any launch
+    (ops.py copies such an input to aligned storage first: test_dispatch_cpu.py::test_odd_offset_pairs_reach_the_library_aligned)."""
+    lib = _lib.load()
+    N0 = ctypes.c_void_p(0)
+    for suffix, step in (("", 4), ("_deterministic", 4), ("_f64", 8)):
+        odd = ctypes.c_void_p(FAKE.value + step)   # aligned to the element, not to the pair
+        fwd = getattr(lib, "umr_bilinear_sample_forward" + ("_f64" if suffix == "_f64" else ""))
+        assert fwd(FAKE, odd, FAKE, 1, 3, 4, 4, 10, None) == UMR_ERR_BAD_ARG, suffix
+        cells = getattr(lib, "umr_bilinear_sample_cells" + ("_f64" if suffix == "_f64" else ""))
+        assert cells(odd, FAKE, 1, 4, 4, 10, None) == UMR_ERR_BAD_ARG, suffix
+        bwd = getattr(lib, "umr_bilinear_sample_backward" + suffix)
+        table = () if suffix == "" else (N0, N0)
+        for flow, gflow in ((odd, FAKE), (FAKE, odd)):
+            assert bwd(FAKE, flow, FAKE, gflow, N0, 1, 3, 4, 4, 10, *table, None) == UMR_ERR_BAD_ARG, suffix
+        tfwd = getattr(lib, "umr_texcycle_forward" + suffix)
+        ws = () if suffix == "" else (FAKE,)
+        for flow, prob in ((odd, FAKE), (FAKE, odd)):
+            assert tfwd(flow, prob, N0, FAKE, FAKE, 2, 4, 9, 0, *ws, None) == UMR_ERR_BAD_ARG, suffix
+        if suffix != "_deterministic":   # the deterministic mode uses the default TexCycle backward
+            tbwd = getattr(lib, "umr_texcycle_backward" + suffix)
+            for flow, prob, gflow in ((odd, FAKE, FAKE), (FAKE, odd, FAKE), (FAKE, FAKE, odd)):
+                assert tbwd(flow, prob, FAKE, FAKE, gflow, 2, 4, 9, None) == UMR_ERR_BAD_ARG, suffix
+
+
+def test_texcycle_size_limit_in_every_precision():
+    """B * F is the kernels' int32 (image, face) index: every TexCycle entry point refuses B * F > INT32_MAX."""
+    lib = _lib.load()
+    N0 = ctypes.c_void_p(0)
+    B, F = 65535, 32769   # B * F = 2^31 + 32767
+    for suffix in ("", "_deterministic", "_f64"):
+        ws = () if suffix == "" else (FAKE,)
+        assert getattr(lib, "umr_texcycle_forward" + suffix)(FAKE, FAKE, N0, FAKE, FAKE, B, F, 9, 0, *ws,
+                                                             None) == UMR_ERR_TOO_LARGE, suffix
+    for suffix in ("", "_f64"):
+        assert getattr(lib, "umr_texcycle_backward" + suffix)(FAKE, FAKE, FAKE, FAKE, FAKE, B, F, 9,
+                                                              None) == UMR_ERR_TOO_LARGE, suffix
+
+
 def test_dtype_rule():
     f32, f64, f16 = torch.zeros(1), torch.zeros(1, dtype=torch.float64), torch.zeros(1, dtype=torch.float16)
     assert ops._is_f64(f32, f64) and ops._is_f64(f64) and ops._is_f64(None, f64)

@@ -282,10 +282,9 @@ def _mesh(kind, B):
             edges = mod.edge_table.cpu()
             ref = R.flatten_ref(xr, edges)
             (ref * w).sum().backward()
-            lb, gb = R.flatten_error_bound(verts, edges, 1e-6, w, edges.shape[0] // 128 + 16)
-            s = 8 * 2.0 ** -29   # the float32 first-order bounds scaled to float64 rounding, doubled twice for the reference
-            _within("flatten value", loss, ref, lb * s)
-            _within("flatten grad", gx, xr.grad, gb * s)
+            lb, gb = R.flatten_error_bound(verts, edges, 1e-6, w, edges.shape[0] // 128 + 16, R.U64)
+            _within("flatten value", loss, ref, lb)
+            _within("flatten grad", gx, xr.grad, gb)
     return fn, _leaves(verts), check
 
 

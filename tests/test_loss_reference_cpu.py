@@ -5,11 +5,12 @@ one-pixel-thin, empty, full and non-binary masks."""
 import numpy as np
 import pytest
 import torch
+import torch.nn.functional as TF
 
 import loss_ref as R
 import losses as O
 import mesh_oracle as MO
-from loss_ref import gamma
+from loss_ref import U32, U64, gamma
 from umr_b200 import synth
 from umr_b200 import soft_renderer as sr
 
@@ -32,6 +33,42 @@ def test_sampler_matches_grid_sample():
         out = R.sample_ref(img.double(), flow)
         mag, _, _, _ = R.sample_magnitude(img.double(), flow, torch.ones(2, 37, C))
         _within("sampler C=%d %dx%d" % (C, H, W), ref32, out, gamma(9) * mag)
+
+
+def test_sampler_double_map_matches_grid_sample_in_double():
+    """The float64 kernel's coordinate map (map_dtype=float64) against torch's CPU grid_sample in double.  On dyadic
+    coordinates the pixel coordinate is exact in either expression order ((x + 1) / 2 * (W - 1) here, (x + 1) * ((W - 1)
+    / 2) in torch), so the two differ only in how the four corner products are rounded and summed: gamma_8 at u = 2^-53.
+    The float32 map stays the default, unchanged: on random coordinates it is ~u32 * |ix| away from the double one."""
+    g = torch.Generator().manual_seed(8)
+    for C, H, W in ((1, 5, 7), (3, 1, 6), (4, 6, 1), (2, 9, 9), (3, 17, 23)):
+        img = torch.rand(2, C, H, W, generator=g, dtype=torch.float64) * 2 - 1
+        flow = torch.randint(-1200, 1200, (2, 301, 2), generator=g).double() / 1024   # dyadic, some outside [-1, 1]
+        flow[0, :4] = torch.tensor([[-1.0, -1.0], [1.0, 1.0], [1.0, -1.0], [0.0, 0.0]])
+        ref = TF.grid_sample(img, flow[:, :, None], mode="bilinear", padding_mode="zeros",
+                             align_corners=True)[..., 0].permute(0, 2, 1)
+        mag, _, _, _ = R.sample_magnitude(img, flow, torch.ones(2, 301, C, dtype=torch.float64), torch.float64)
+        _within("sampler double map C=%d %dx%d" % (C, H, W), R.sample_ref(img, flow, torch.float64), ref,
+                gamma(8, U64) * mag)
+        rand = torch.rand(2, 301, 2, generator=g, dtype=torch.float64) * 2.4 - 1.2
+        f32 = R.sample_ref(img, rand)
+        assert torch.equal(f32, R.sample_ref(img, rand, torch.float32))
+        assert torch.equal(f32, R.sample_ref(img, rand.float()))
+        assert (f32 - R.sample_ref(img, rand, torch.float64)).abs().max() > 1e3 * gamma(8, U64)
+
+
+def test_unit_roundoff_defaults_are_float32():
+    assert U32 == 2.0 ** -24 and U64 == 2.0 ** -53
+    assert gamma(7) == gamma(7, U32) == 7 * U32 / (1 - 7 * U32)
+    assert gamma(7, U64) == 7 * U64 / (1 - 7 * U64)
+    v, f = R.spiked_uv_sphere(5, 6, 2)
+    x = torch.from_numpy(v[None].astype(np.float32))
+    edges = sr.FlattenLoss(torch.from_numpy(f)).edge_table
+    b32 = R.flatten_error_bound(x, edges, 1e-6, torch.ones(1), 20)
+    for a, b in zip(b32, R.flatten_error_bound(x, edges, 1e-6, torch.ones(1), 20, U32)):
+        assert torch.equal(a, b)
+    for a, b in zip(b32, R.flatten_error_bound(x, edges, 1e-6, torch.ones(1), 20, U64)):
+        assert torch.allclose(b, a * (U64 / U32), rtol=1e-6, atol=0)   # first order in u: the bound scales with it
 
 
 def test_sampler_gradients():

@@ -87,7 +87,8 @@ using namespace umr;
 
 extern "C" int umr_bilinear_sample_forward(const float* image, const float* flow, float* out, int32_t B,
                                            int32_t C, int32_t H, int32_t W, int32_t N, void* stream_) {
-    if (!image || !flow || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0) return UMR_ERR_BAD_ARG;
+    if (!image || !flow || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 || vec2_misaligned(flow))
+        return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     cudaStream_t st = (cudaStream_t)stream_;
     const dim3 grid((N + 255) / 256, B);
@@ -106,7 +107,8 @@ extern "C" int umr_bilinear_sample_forward(const float* image, const float* flow
 extern "C" int umr_bilinear_sample_backward(const float* image, const float* flow, const float* grad_out,
                                             float* grad_flow, float* grad_image, int32_t B, int32_t C,
                                             int32_t H, int32_t W, int32_t N, void* stream_) {
-    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0)
+    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 ||
+        vec2_misaligned(flow) || vec2_misaligned(grad_flow))
         return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     cudaStream_t st = (cudaStream_t)stream_;
@@ -183,8 +185,10 @@ extern "C" int umr_chamfer_backward(const float* a, const float* b, const int32_
 extern "C" int umr_texcycle_forward(const float* flow, const float* prob, const float* face_ids, uint8_t* visible,
                                     float* loss, int32_t B, int32_t F, int32_t T2, int64_t P, void* stream_) {
     // face_ids == NULL: `visible` was already filled by umr_raster_visibility (its visible_faces output)
-    if (!flow || !prob || !visible || !loss || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0)) return UMR_ERR_BAD_ARG;
-    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    if (!flow || !prob || !visible || !loss || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0) ||
+        vec2_misaligned(flow) || vec2_misaligned(prob))
+        return UMR_ERR_BAD_ARG;
+    if (B > 65535 || (int64_t)B * F > INT_MAX) return UMR_ERR_TOO_LARGE;
     cudaStream_t st = (cudaStream_t)stream_;
     cudaError_t e = cudaMemsetAsync(loss, 0, sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
@@ -203,7 +207,10 @@ extern "C" int umr_texcycle_forward(const float* flow, const float* prob, const 
 
 extern "C" int umr_texcycle_backward(const float* flow, const float* prob, const uint8_t* visible, const float* grad_loss,
                                      float* grad_flow, int32_t B, int32_t F, int32_t T2, void* stream_) {
-    if (!flow || !prob || !visible || !grad_loss || !grad_flow || B <= 0 || F <= 0 || T2 <= 0) return UMR_ERR_BAD_ARG;
+    if (!flow || !prob || !visible || !grad_loss || !grad_flow || B <= 0 || F <= 0 || T2 <= 0 || vec2_misaligned(flow) ||
+        vec2_misaligned(prob) || vec2_misaligned(grad_flow))
+        return UMR_ERR_BAD_ARG;
+    if ((int64_t)B * F > INT_MAX) return UMR_ERR_TOO_LARGE;
     return texcycle_backward(flow, prob, visible, grad_loss, grad_flow, B, F, T2, stream_);
 }
 
@@ -274,9 +281,10 @@ extern "C" size_t umr_texcycle_workspace_bytes_deterministic(int32_t B, int32_t 
 extern "C" int umr_texcycle_forward_deterministic(const float* flow, const float* prob, const float* face_ids, uint8_t* visible,
                                                   float* loss, int32_t B, int32_t F, int32_t T2, int64_t P, void* workspace,
                                                   void* stream_) {
-    if (!flow || !prob || !visible || !loss || !workspace || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0))
+    if (!flow || !prob || !visible || !loss || !workspace || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0) ||
+        vec2_misaligned(flow) || vec2_misaligned(prob))
         return UMR_ERR_BAD_ARG;
-    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    if (B > 65535 || (int64_t)B * F > INT_MAX) return UMR_ERR_TOO_LARGE;
     return texcycle_forward_slots(flow, prob, face_ids, visible, loss, B, F, T2, P, workspace, stream_);
 }
 
@@ -305,7 +313,8 @@ extern "C" int umr_bilinear_sample_backward_deterministic(const float* image, co
                                                           float* grad_flow, float* grad_image, int32_t B, int32_t C, int32_t H,
                                                           int32_t W, int32_t N, const int32_t* cell_rowptr,
                                                           const int32_t* cell_samples, void* stream_) {
-    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0)
+    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 ||
+        vec2_misaligned(flow) || vec2_misaligned(grad_flow))
         return UMR_ERR_BAD_ARG;
     if (grad_image && (!cell_rowptr || !cell_samples)) return UMR_ERR_BAD_ARG;
     if (cells_too_large(B, H, W)) return UMR_ERR_TOO_LARGE;

@@ -583,9 +583,16 @@ static inline bool cells_too_large(int32_t B, int32_t H, int32_t W) {
     return B > 65535 || (int64_t)B * ((int64_t)H + 1) * ((int64_t)W + 1) > INT_MAX;
 }
 
+// The sampler's flow and TexCycle's flow / prob / grad_flow are read and written as vec2_t<T> (float2 / double2), which
+// needs an address aligned to 2 * sizeof(T); a misaligned one would fault on the device.  NULL passes.
+template <typename T>
+static inline bool vec2_misaligned(const T* p) {
+    return ((uintptr_t)p & (2 * sizeof(T) - 1)) != 0;
+}
+
 template <typename T>
 static int sample_cells(const T* flow, int32_t* cells, int32_t B, int32_t H, int32_t W, int32_t N, void* stream_) {
-    if (!flow || !cells || B <= 0 || H <= 0 || W <= 0 || N <= 0) return UMR_ERR_BAD_ARG;
+    if (!flow || !cells || B <= 0 || H <= 0 || W <= 0 || N <= 0 || vec2_misaligned(flow)) return UMR_ERR_BAD_ARG;
     if (cells_too_large(B, H, W)) return UMR_ERR_TOO_LARGE;
     count_launch();
     k_sample_cells<T><<<dim3((N + 255) / 256, B), 256, 0, (cudaStream_t)stream_>>>(

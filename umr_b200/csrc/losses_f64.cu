@@ -24,7 +24,8 @@ using namespace umr;
 
 extern "C" int umr_bilinear_sample_forward_f64(const double* image, const double* flow, double* out, int32_t B, int32_t C,
                                                int32_t H, int32_t W, int32_t N, void* stream_) {
-    if (!image || !flow || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0) return UMR_ERR_BAD_ARG;
+    if (!image || !flow || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 || vec2_misaligned(flow))
+        return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     if (C > 4) return UMR_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream_;
@@ -49,7 +50,8 @@ extern "C" int umr_bilinear_sample_backward_f64(const double* image, const doubl
                                                 double* grad_flow, double* grad_image, int32_t B, int32_t C, int32_t H,
                                                 int32_t W, int32_t N, const int32_t* cell_rowptr,
                                                 const int32_t* cell_samples, void* stream_) {
-    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0)
+    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 ||
+        vec2_misaligned(flow) || vec2_misaligned(grad_flow))
         return UMR_ERR_BAD_ARG;
     if (grad_image && (!cell_rowptr || !cell_samples)) return UMR_ERR_BAD_ARG;
     if (cells_too_large(B, H, W)) return UMR_ERR_TOO_LARGE;
@@ -109,14 +111,17 @@ extern "C" size_t umr_texcycle_workspace_bytes_f64(int32_t B, int32_t F) { retur
 extern "C" int umr_texcycle_forward_f64(const double* flow, const double* prob, const float* face_ids, uint8_t* visible,
                                         double* loss, int32_t B, int32_t F, int32_t T2, int64_t P, void* workspace,
                                         void* stream_) {
-    if (!flow || !prob || !visible || !loss || !workspace || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0))
+    if (!flow || !prob || !visible || !loss || !workspace || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0) ||
+        vec2_misaligned(flow) || vec2_misaligned(prob))
         return UMR_ERR_BAD_ARG;
     if (B > 65535 || (int64_t)B * F > INT_MAX) return UMR_ERR_TOO_LARGE;
     return texcycle_forward_slots(flow, prob, face_ids, visible, loss, B, F, T2, P, workspace, stream_);
 }
 extern "C" int umr_texcycle_backward_f64(const double* flow, const double* prob, const uint8_t* visible, const double* grad_loss,
                                          double* grad_flow, int32_t B, int32_t F, int32_t T2, void* stream_) {
-    if (!flow || !prob || !visible || !grad_loss || !grad_flow || B <= 0 || F <= 0 || T2 <= 0) return UMR_ERR_BAD_ARG;
+    if (!flow || !prob || !visible || !grad_loss || !grad_flow || B <= 0 || F <= 0 || T2 <= 0 || vec2_misaligned(flow) ||
+        vec2_misaligned(prob) || vec2_misaligned(grad_flow))
+        return UMR_ERR_BAD_ARG;
     if (B > 65535 || (int64_t)B * F > INT_MAX) return UMR_ERR_TOO_LARGE;
     return texcycle_backward(flow, prob, visible, grad_loss, grad_flow, B, F, T2, stream_);
 }

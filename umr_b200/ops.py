@@ -80,6 +80,13 @@ def _as(t, mode):
     return t.detach().contiguous().to(mode.dtype)
 
 
+def _pairs(t):
+    """`t` itself when its address is a multiple of 2 * itemsize, else an aligned copy: the kernels read the sampler's
+    flow and TexCycle's flow / prob as (x, y) vector pairs, which a contiguous view at an odd element offset (e.g.
+    `buf[1:].view(B, N, 2)`) would misalign.  The library refuses such a pointer."""
+    return t if t.data_ptr() % (2 * t.element_size()) == 0 else t.clone()
+
+
 # -------------------------------------------------------------------------------------------------
 # bilinear texture-flow sampler
 # -------------------------------------------------------------------------------------------------
@@ -91,7 +98,7 @@ class BilinearSampleFunction(torch.autograd.Function):
     def forward(ctx, images, flow):
         _need_cuda(images, flow)
         m = KernelMode(_is_f64(images, flow))   # the forward has no atomics; the backward's mode
-        img, fl = _as(images, m), _as(flow, m)
+        img, fl = _as(images, m), _pairs(_as(flow, m))
         B, C, H, W = img.shape
         N = fl.shape[1]
         with torch.cuda.device(img.device):
@@ -326,7 +333,7 @@ class TexCycleFunction(torch.autograd.Function):
     def forward(ctx, flow, prob, face_ids, visible=None):
         _need_cuda(flow, prob) if face_ids is None else _need_cuda(flow, prob, face_ids)
         m = KernelMode(_is_f64(flow, prob, face_ids))
-        fl, pr = _as(flow, m), _as(prob, m)
+        fl, pr = _pairs(_as(flow, m)), _pairs(_as(prob, m))
         B, F, T2 = fl.shape[0], fl.shape[1], fl.shape[2]
         if visible is not None:
             if visible.dtype != torch.uint8 or tuple(visible.shape) != (B, F) or not visible.is_cuda:
