@@ -88,7 +88,10 @@ def _p(a):
 
 
 def standard_grid(image_size, dtype=np.float32):
-    """`affine_grid(identity, (1,1,S,S))` of torch 1.1 (== align_corners=True): [S,S,2] (x,y)."""
+    """`affine_grid(identity, (1,1,S,S))` of torch 1.1 (== align_corners=True): [S,S,2] (x,y).  At S = 1 torch 1.1 takes
+    linspace(-1, 1, 1) = [-1], so the one pixel is (-1, -1); torch >= 1.3 returns 0 there instead."""
+    if int(image_size) == 1:
+        return np.full((1, 1, 2), -1.0, dtype)
     import torch
     theta = torch.tensor([[1, 0, 0], [0, 1, 0]], dtype=torch.float)
     g = torch.nn.functional.affine_grid(theta.unsqueeze(0), (1, 1, image_size, image_size),

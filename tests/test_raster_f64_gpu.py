@@ -22,6 +22,7 @@ import softras
 from umr_b200 import _lib, raster, synth
 from umr_b200 import soft_renderer as sr
 from umr_b200.nnutils import geom_utils, smr
+from raster_range_scenes import kernel_grid
 from util import rel_report, scene
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
@@ -34,18 +35,6 @@ SOFT = dict(sigma_val=1e-4, dist_eps=1e-4, gamma_val=1e-3)
 RTOL, ATOL_PLANE, ATOL_GRAD_REL = 1e-11, 1e-13, 1e-11
 BG = (0.25, 0.5, 0.75)   # exact in float32: UmrRasterParams carries the background as float
 _REF_NOFMA = rc.load("soft_rasterize_ref_nofma")
-
-
-def kernel_grid(S, dtype=np.float64):
-    """The p2f grid of the kernels: torch's float32 linspace(-1, 1, S) by its per-element definition (start + step * i in the
-    lower half, end - step * (S - 1 - i) in the upper), widened.  torch's vectorised CPU linspace, which
-    softras.standard_grid calls, rounds some elements one float ulp away from it, so the oracle is handed this grid."""
-    step = np.float32(2.0) / np.float32(S - 1)
-    i = np.arange(S)
-    lo = (np.float32(-1.0) + step * i.astype(np.float32)).astype(np.float32)
-    hi = (np.float32(1.0) - step * (S - 1 - i).astype(np.float32)).astype(np.float32)
-    x = np.where(i * 2 < S, lo, hi)
-    return np.ascontiguousarray(np.stack(np.broadcast_arrays(x[None, :], x[:, None]), axis=-1).astype(dtype))
 
 
 @pytest.fixture(autouse=True)
@@ -440,7 +429,7 @@ def test_non_finite_vertices_render_as_the_oracle_does(bad):
             assert np.allclose(got[k][fin], ref[k][fin], rtol=1e-9, atol=1e-9 * (np.abs(ref[k][fin]).max() if fin.any() else 1)), (k, rgb)
 
 
-@pytest.mark.parametrize("tex_res", [1, 6, 17])
+@pytest.mark.parametrize("tex_res", [1, 6, 17, 257])
 def test_texture_resolutions(tex_res):
     rng = np.random.default_rng(129)
     v, f = synth.icosphere(1)

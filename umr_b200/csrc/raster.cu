@@ -660,7 +660,8 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
 
     const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
     // torch-1.1 affine_grid (align_corners=True) coordinates of this pixel: linspace(-1, 1, S)
-    const float gstep = 2.f / (float)(S - 1);
+    // S = 1: torch 1.1's affine_grid takes linspace(-1, 1, 1) = [-1] (DESIGN.md §2), where 2 / 0 would give -1 + inf * 0 = NaN
+    const float gstep = S > 1 ? 2.f / (float)(S - 1) : 0.f;
     const float gx = (px * 2 < S) ? (-1.f + gstep * px) : (1.f - gstep * (S - 1 - px));
     const float gy = (py * 2 < S) ? (-1.f + gstep * py) : (1.f - gstep * (S - 1 - py));
 
@@ -1594,7 +1595,7 @@ __global__ void k_p2f_finalize_det(const unsigned long long* __restrict__ acc, f
 __device__ __forceinline__ void det_span(float lo, float hi, int S, int& i0, int& i1) {
     const double a = ((double)lo * S + (S - 1)) * 0.5, c = ((double)hi * S + (S - 1)) * 0.5;
     i0 = a > 0.0 ? (a < (double)S ? (int)a - 1 : S) : 0;
-    i1 = c < (double)(S - 1) ? (c >= 0.0 ? (int)c + 1 : -1) : S - 1;
+    i1 = c < (double)(S - 1) ? (c > -1.0 ? (int)c + 1 : -1) : S - 1;  // c in (-1, 0): pixel 0 may still lie in the box
     i0 = max(i0, 0);
     i1 = min(i1, S - 1);
 }
@@ -2236,10 +2237,10 @@ extern "C" int umr_raster_backward_deterministic(const float* face_vertices, con
                                                  const UmrRasterParams* p, void* workspace, void* stream_) {
     int rc = check_params(p);
     if (rc) return rc;
+    if ((int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;  // as the forward
     if (!face_vertices || !textures || !soft_colors || !aggrs_info || !grad_images || !workspace) return UMR_ERR_BAD_ARG;
     if (!grad_faces && !grad_textures) return UMR_ERR_BAD_ARG;
     if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
-    if ((int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;
     const bool gen = is_generic(p);
     const bool nc4 = p->color_channels == 4;
     if (nc4 && grad_textures) return UMR_ERR_UNSUPPORTED;  // part maps are constants (loss_utils.py:367-381)

@@ -411,7 +411,8 @@ __global__ void __launch_bounds__(CTA, 2) k_raster_fwd_f64(const double* __restr
     const double* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
     // the float32 affine_grid (align_corners=True) coordinates of this pixel, widened: soft_rasterize.py:58-62 builds
     // the grid from a float theta
-    const float gstep = 2.f / (float)(S - 1);
+    // S = 1: torch 1.1's affine_grid takes linspace(-1, 1, 1) = [-1] (DESIGN.md §2), where 2 / 0 would give -1 + inf * 0 = NaN
+    const float gstep = S > 1 ? 2.f / (float)(S - 1) : 0.f;
     const double gx = (double)((px * 2 < S) ? (-1.f + gstep * px) : (1.f - gstep * (S - 1 - px)));
     const double gy = (double)((py * 2 < S) ? (-1.f + gstep * py) : (1.f - gstep * (S - 1 - py)));
 
@@ -584,7 +585,7 @@ __global__ void __launch_bounds__(CTA, 2) k_raster_fwd_f64(const double* __restr
 __device__ __forceinline__ void box_span(double lo, double hi, int S, int& i0, int& i1) {
     const double a = (lo * S + (S - 1)) * 0.5, c = (hi * S + (S - 1)) * 0.5;
     i0 = a > 0.0 ? (a < (double)S ? (int)a - 1 : S) : 0;
-    i1 = c < (double)(S - 1) ? (c >= 0.0 ? (int)c + 1 : -1) : S - 1;
+    i1 = c < (double)(S - 1) ? (c > -1.0 ? (int)c + 1 : -1) : S - 1;  // c in (-1, 0): pixel 0 may still lie in the box
     i0 = max(i0, 0);
     i1 = min(i1, S - 1);
 }

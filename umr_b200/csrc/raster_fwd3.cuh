@@ -166,7 +166,8 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
     float zmin = 10000000.f;
     int fid = -1;
     // torch-1.1 affine_grid (align_corners=True) coordinates of this pixel: linspace(-1, 1, S)
-    const float gstep = 2.f / (float)(S - 1);
+    // S = 1: torch 1.1's affine_grid takes linspace(-1, 1, 1) = [-1] (DESIGN.md §2), where 2 / 0 would give -1 + inf * 0 = NaN
+    const float gstep = S > 1 ? 2.f / (float)(S - 1) : 0.f;
     const float gx = (px * 2 < S) ? (-1.f + gstep * px) : (1.f - gstep * (S - 1 - px));
     const float gy = (py * 2 < S) ? (-1.f + gstep * py) : (1.f - gstep * (S - 1 - py));
 

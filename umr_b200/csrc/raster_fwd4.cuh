@@ -195,7 +195,8 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
     };
     const bool slow = nc > LC;  // uniform: the bin's list does not fit the shared tile list -> windowed static path below
     float* wst = s_wrec + warp * (2 * WG4 * REC_F);
-    const float gstep = 2.f / (float)(S - 1);
+    // S = 1: torch 1.1's affine_grid takes linspace(-1, 1, 1) = [-1] (DESIGN.md §2), where 2 / 0 would give -1 + inf * 0 = NaN
+    const float gstep = S > 1 ? 2.f / (float)(S - 1) : 0.f;
 
     struct PixelState { float acc_a, ssum, smax, c0, c1, c2, zmin; int fid; };
     auto init_state = [&](PixelState& st) {  // kernel.cu:335-348
