@@ -175,6 +175,22 @@ int umr_raster_backward_deterministic(const float* face_vertices, const float* t
                                       float* grad_textures, const UmrRasterParams* params, void* workspace,
                                       void* stream);
 
+/* Split backward (DESIGN.md §11): one backward of one render that serves two losses -- a mask loss on the alpha plane whose
+ * gradient reaches the geometry, and a texture loss on the RGB planes of the same render whose geometry is detached.  Same
+ * arguments as umr_raster_backward / umr_raster_backward_deterministic (and the same workspace).  grad_faces receives only the
+ * terms driven by the alpha plane of grad_images -- bitwise what the plain call gives with the RGB planes of grad_images set
+ * to zero -- and grad_textures the texel gradients of the RGB planes, bitwise what the plain call gives with grad_faces ==
+ * NULL (in the deterministic variant; the default one sums with float atomics).  Both outputs are required; UMR's
+ * configuration only (euclidean / prod / surface, 3 colour channels, softmax or hard colours, shared textures, any F up to
+ * UMR_RASTER_MAX_FACES, every pair-buffer state): anything else returns UMR_ERR_BAD_ARG.  No host synchronisation. */
+int umr_raster_backward_split(const float* face_vertices, const float* textures, const float* soft_colors,
+                              const float* aggrs_info, const float* grad_images, float* grad_faces, float* grad_textures,
+                              const UmrRasterParams* params, void* workspace, void* stream);
+int umr_raster_backward_split_deterministic(const float* face_vertices, const float* textures, const float* soft_colors,
+                                            const float* aggrs_info, const float* grad_images, float* grad_faces,
+                                            float* grad_textures, const UmrRasterParams* params, void* workspace,
+                                            void* stream);
+
 /* Double precision (DESIGN.md §9).  The arguments, outputs, validation and error codes of umr_raster_forward /
  * umr_raster_backward with every buffer in double: an operation-for-operation twin of the reference kernels' `scalar_t =
  * double` instantiation (every operation one IEEE binary64 rounding; the scalars of UmrRasterParams stay float, as in the

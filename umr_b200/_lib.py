@@ -70,6 +70,11 @@ EXPORTS = {
                                                                       ctypes.c_void_p]),
     "umr_raster_backward_deterministic": (ctypes.c_int, [c_f32p] * 7 + [ctypes.POINTER(UmrRasterParams), ctypes.c_void_p,
                                                                        ctypes.c_void_p]),
+    # split backward: alpha adjoint -> grad_faces, RGB adjoint -> grad_textures (the arguments of umr_raster_backward)
+    "umr_raster_backward_split": (ctypes.c_int, [c_f32p] * 7 + [ctypes.POINTER(UmrRasterParams), ctypes.c_void_p,
+                                                               ctypes.c_void_p]),
+    "umr_raster_backward_split_deterministic": (ctypes.c_int, [c_f32p] * 7 + [ctypes.POINTER(UmrRasterParams), ctypes.c_void_p,
+                                                                             ctypes.c_void_p]),
     # double-precision rasteriser: the arguments of umr_raster_forward / umr_raster_backward with double buffers
     "umr_raster_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32] * 4),
     "umr_raster_forward_f64": (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.POINTER(UmrRasterParams), ctypes.c_void_p,

@@ -1261,7 +1261,10 @@ __device__ __forceinline__ bool bwd_pair(const float* __restrict__ rc, float xp,
 // Register-lean variant used by the pair-parallel kernel: the 10 per-pixel inputs stay in shared memory
 // (sp = &s_pix[0][pix], plane stride PT*PT) and are fetched where they are consumed, and the 9 gradients are
 // added straight into the caller's accumulators -- this keeps the kernel at <= 64 registers (4 CTAs/SM).
-template <int RGB, bool TEXGRAD, int NC = 3, class Sink = TexRedSink>
+// SPLIT (the split backward, softmax only): the vertex gradients keep only the terms driven by the alpha adjoint g3; the texel
+// gradients are formed from the colour adjoints as always.  Skipping the colour terms leaves every other expression as it is,
+// so the vertex gradients equal, bit for bit, those of the same pairs with zero colour adjoints.
+template <int RGB, bool TEXGRAD, int NC = 3, class Sink = TexRedSink, bool SPLIT = false>
 __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float xp, float yp, const Consts& K,
                                              const float* __restrict__ sp, int f, const float* __restrict__ tex_img,
                                              float* __restrict__ gtex_img, float* acc, Sink sink = Sink()) {
@@ -1309,16 +1312,18 @@ __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float
                         for (int c = 0; c < NC; ++c) red_add_global(gtex_img + to + c, s * g[c]);
                     }
                 }
-                float Crgb = 0.f;
+                if (!SPLIT) {
+                    float Crgb = 0.f;
 #pragma unroll
-                for (int c = 0; c < NC; ++c) Crgb += g[c] * (__ldg(tex_img + to + c) - sp[(NPL + c) * NP]);
-                Crgb *= s;
-                if (Crgb != 0.f) {
-                    Cxy += Crgb / fr.D;
-                    const float Cz = Crgb / K.gamma / (K.near_ - K.far_) * zp * zp;
-                    acc[2] += Cz * k0 / rc[2] / rc[2];
-                    acc[5] += Cz * k1 / rc[5] / rc[5];
-                    acc[8] += Cz * k2 / rc[8] / rc[8];
+                    for (int c = 0; c < NC; ++c) Crgb += g[c] * (__ldg(tex_img + to + c) - sp[(NPL + c) * NP]);
+                    Crgb *= s;
+                    if (Crgb != 0.f) {
+                        Cxy += Crgb / fr.D;
+                        const float Cz = Crgb / K.gamma / (K.near_ - K.far_) * zp * zp;
+                        acc[2] += Cz * k0 / rc[2] / rc[2];
+                        acc[5] += Cz * k1 / rc[5] / rc[5];
+                        acc[8] += Cz * k2 / rc[8] / rc[8];
+                    }
                 }
             }
         }
@@ -1335,8 +1340,8 @@ __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float
 }
 
 // One PT x PT tile of the recompute backward (bx, by, b = tile column / row / image).  Every early exit is CTA-uniform.
-// `bar_phase` carries the mbarrier parity across the tiles a CTA processes (list-driven launch).
-template <int RGB, bool TEXGRAD, int NC = 3>
+// `bar_phase` carries the mbarrier parity across the tiles a CTA processes (list-driven launch).  SPLIT: see bwd_pair_acc.
+template <int RGB, bool TEXGRAD, int NC = 3, bool SPLIT = false>
 __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all, const float4* __restrict__ box_all,
                                                const float* __restrict__ textures, const float* __restrict__ colors_hi,
                                                const float* __restrict__ aggrs, const float* __restrict__ grad_images,
@@ -1498,7 +1503,8 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
                     const int col = cx0 + (local - lr * w);
                     const int row = ry0 + lr;
                     const int pix = row * PT + col;
-                    if (bwd_pair_acc<RGB, TEXGRAD, NC>(rc, s_xp[col], s_yp[row], K, &s_pix[0][pix], f, tex_img, gtex_img, acc))
+                    if (bwd_pair_acc<RGB, TEXGRAD, NC, TexRedSink, SPLIT>(rc, s_xp[col], s_yp[row], K, &s_pix[0][pix], f, tex_img,
+                                                                          gtex_img, acc))
                         acc_any = true;
                 }
                 if (__any_sync(0xffffffffu, acc_any)) {
@@ -1523,7 +1529,7 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
 
 
 // full grid: one CTA per tile (no pair buffer: every tile is recomputed)
-template <int RGB, bool TEXGRAD, int NC = 3>
+template <int RGB, bool TEXGRAD, int NC = 3, bool SPLIT = false>
 __global__ void __launch_bounds__(CTA, 3) k_raster_bwd_pairs(const float* __restrict__ rec_all, const float4* __restrict__ box_all,
                                                              const float* __restrict__ textures, const float* __restrict__ colors_hi,
                                                              const float* __restrict__ aggrs, const float* __restrict__ grad_images,
@@ -1535,14 +1541,14 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd_pairs(const float* __rest
         fence_mbar_init();
     }
     uint32_t phase = 0;  // (bwd_pairs_tile synchronises the CTA before the barrier is first used)
-    bwd_pairs_tile<RGB, TEXGRAD, NC>(rec_all, box_all, textures, colors_hi, aggrs, grad_images, grad_faces, grad_tex, ubox, K,
-                                 (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z, &s_bar, phase);
+    bwd_pairs_tile<RGB, TEXGRAD, NC, SPLIT>(rec_all, box_all, textures, colors_hi, aggrs, grad_images, grad_faces, grad_tex, ubox,
+                                        K, (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z, &s_bar, phase);
 }
 
 // list-driven: with a pair buffer, only the tiles the forward could NOT save are recomputed.  The forward appended
 // their ids to `ulist` (count in *ucount); a small persistent grid walks the list, so a render whose tiles were all
 // saved pays one near-empty launch instead of one CTA per tile (35 us at C2 with the full grid).
-template <int RGB, bool TEXGRAD, int NC = 3>
+template <int RGB, bool TEXGRAD, int NC = 3, bool SPLIT = false>
 __global__ void __launch_bounds__(CTA, 3) k_raster_bwd_pairs_list(const float* __restrict__ rec_all, const float4* __restrict__ box_all,
                                                                   const float* __restrict__ textures, const float* __restrict__ colors_hi,
                                                                   const float* __restrict__ aggrs, const float* __restrict__ grad_images,
@@ -1561,8 +1567,8 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd_pairs_list(const float* _
     for (uint32_t i = blockIdx.x; i < nu; i += gridDim.x) {
         const int t = __ldg(ulist + i);
         const int bx = t % tiles_x, by = (t / tiles_x) % tiles_y, b = t / (tiles_x * tiles_y);
-        bwd_pairs_tile<RGB, TEXGRAD, NC>(rec_all, box_all, textures, colors_hi, aggrs, grad_images, grad_faces, grad_tex, ubox, K,
-                                     bx, by, b, &s_bar, phase);
+        bwd_pairs_tile<RGB, TEXGRAD, NC, SPLIT>(rec_all, box_all, textures, colors_hi, aggrs, grad_images, grad_faces, grad_tex,
+                                            ubox, K, bx, by, b, &s_bar, phase);
     }
 }
 
@@ -1607,9 +1613,9 @@ __device__ __forceinline__ void det_span(float lo, float hi, int S, int& i0, int
 // Texel gradients: lanes that hit the same texel are summed in ascending lane order, and the lowest of them adds the sum into the
 // warp-owned texels of the face (plain load / store; __syncwarp orders the steps).  GEN: the generic modes (distance, alpha
 // and texture mode read at run time), evaluated with bwd_pair_generic -- k_raster_bwd's arithmetic; a vertex-texture pair adds
-// to the face's 9 corner colours, which the warp sums the same way.
+// to the face's 9 corner colours, which the warp sums the same way.  SPLIT (UMR's configuration only): see bwd_pair_acc.
 constexpr int DET_WARPS = CTA / 32;
-template <int RGB, bool TEXGRAD, int NC = 3, bool GEN = false>
+template <int RGB, bool TEXGRAD, int NC = 3, bool GEN = false, bool SPLIT = false>
 __global__ void __launch_bounds__(CTA) k_raster_bwd_det(const float* __restrict__ rec_all, const float* __restrict__ textures,
                                                         const float* __restrict__ colors_hi, const float* __restrict__ aggrs,
                                                         const float* __restrict__ grad_images, float* __restrict__ grad_faces,
@@ -1675,8 +1681,8 @@ __global__ void __launch_bounds__(CTA) k_raster_bwd_det(const float* __restrict_
                             for (int k = 0; k < 9; ++k) acc[k] += gv[k];
                         }
                     } else {
-                        bwd_pair_acc<RGB, TEXGRAD, NC, TexTakeSink>(rc, xp, yp, K, sp, f, tex_img, gtex_img, acc,
-                                                                     TexTakeSink{&taddr, tval});
+                        bwd_pair_acc<RGB, TEXGRAD, NC, TexTakeSink, SPLIT>(rc, xp, yp, K, sp, f, tex_img, gtex_img, acc,
+                                                                            TexTakeSink{&taddr, tval});
                     }
                 }
                 if (TEXGRAD) {
@@ -1731,15 +1737,17 @@ __global__ void __launch_bounds__(CTA) k_raster_bwd_det(const float* __restrict_
 using namespace umr;
 
 // k_raster_bwd2 instantiation for the call: texture-only (grad_faces == NULL) and warp-level texel pre-reduction variants
-// exist for the texture-gradient kernels only
-template <int RGBM, bool TG, int TS, typename IdxT>
+// exist for the texture-gradient kernels only; SP: the split backward (softmax, both gradients)
+template <int RGBM, bool TG, int TS, typename IdxT, bool SP = false>
 static void launch_bwd2(dim3 grid, cudaStream_t stream, bool pre, const float* rec, const float* textures, const float* soft_colors,
                         const float* aggrs_info, const float* grad_images, float* grad_faces, float* grad_textures,
                         const Consts& K, const PairBuf& pb) {
 #define UMR_BWD2_GO(GEOMV, PREV) \
-    k_raster_bwd2<RGBM, TG, TS, 3, GEOMV, PREV, IdxT><<<grid, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images, \
-                                                                                    grad_faces, grad_textures, K, pb)
-    if constexpr (TG && RGBM == 1) {
+    k_raster_bwd2<RGBM, TG, TS, 3, GEOMV, PREV, IdxT, SP><<<grid, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, \
+                                                                                        grad_images, grad_faces, grad_textures, K, pb)
+    if constexpr (SP) {
+        if (pre) UMR_BWD2_GO(true, true); else UMR_BWD2_GO(true, false);
+    } else if constexpr (TG && RGBM == 1) {
         if (pre) { if (grad_faces) UMR_BWD2_GO(true, true); else UMR_BWD2_GO(false, true); }
         else { if (grad_faces) UMR_BWD2_GO(true, false); else UMR_BWD2_GO(false, false); }
     } else if constexpr (TG) {
@@ -1885,6 +1893,7 @@ static int ensure_smem_attrs() {
     UMR_SET((k_raster_bwd_pairs<1, false>)) UMR_SET((k_raster_bwd_pairs<1, true>))
     UMR_SET((k_raster_bwd_pairs_list<0, false>)) UMR_SET((k_raster_bwd_pairs_list<0, true>))
     UMR_SET((k_raster_bwd_pairs_list<1, false>)) UMR_SET((k_raster_bwd_pairs_list<1, true>))
+    UMR_SET((k_raster_bwd_pairs<1, true, 3, true>)) UMR_SET((k_raster_bwd_pairs_list<1, true, 3, true>))
 #undef UMR_SET
     done[dev] = true;
     return 0;
@@ -2111,19 +2120,22 @@ extern "C" int umr_raster_visibility(const float* face_vertices, float* aggrs_in
     return (int)cudaGetLastError();
 }
 
-extern "C" int umr_raster_backward(const float* face_vertices, const float* textures,
-                                   const float* soft_colors, const float* aggrs_info,
-                                   const float* grad_images, float* grad_faces, float* grad_textures,
-                                   const UmrRasterParams* p, void* workspace, void* stream_) {
-    int rc = check_params(p);
-    if (rc) return rc;
+// The split backward takes both gradients and UMR's configuration with 3 colour channels only (see umr_raster_backward_split).
+static bool split_refused(const UmrRasterParams* p, const float* grad_faces, const float* grad_textures) {
+    return !grad_faces || !grad_textures || is_generic(p) || p->color_channels == 4;
+}
+
+// split: umr_raster_backward_split (the caller has checked split_refused)
+static int raster_backward(const float* face_vertices, const float* textures, const float* soft_colors, const float* aggrs_info,
+                           const float* grad_images, float* grad_faces, float* grad_textures, const UmrRasterParams* p,
+                           void* workspace, void* stream_, bool split) {
     if (!face_vertices || !textures || !soft_colors || !aggrs_info || !grad_images || !workspace) return UMR_ERR_BAD_ARG;
     if (!grad_faces && !grad_textures) return UMR_ERR_BAD_ARG;  // nothing to compute
     if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
     const bool nc4 = p->color_channels == 4;
     if (nc4 && grad_textures) return UMR_ERR_UNSUPPORTED;  // part maps are constants (loss_utils.py:367-381)
     cudaStream_t stream = (cudaStream_t)stream_;
-    rc = ensure_smem_attrs();
+    int rc = ensure_smem_attrs();
     if (rc) return rc;
     const int B = p->batch_size, F = p->num_faces;
     const Consts K = make_consts(p);
@@ -2140,11 +2152,11 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
     if (e != cudaSuccess) return (int)e;
     const bool gen = is_generic(p);
     const PairBuf pb = gen ? PairBuf{nullptr, nullptr, nullptr, nullptr, nullptr, 0u} : make_pairbuf(p, K.S);
-    // The streamed backward re-derives its z-gradient factors from the records whenever it forms vertex gradients; a
-    // texture-only backward with a pair buffer needs them only for the recompute fallback, so k_prep returns at once there
-    // when no tile is unsaved.
+    // The streamed backward re-derives its z-gradient factors from the records whenever it forms the colour terms of the
+    // vertex gradients; a texture-only or split backward with a pair buffer needs them only for the recompute fallback, so
+    // k_prep returns at once there when no tile is unsaved.
     k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, r,
-                                                         (pb.cap > 0 && !grad_faces) ? pb.ctrl + 1 : nullptr);
+                                                         (pb.cap > 0 && (!grad_faces || split)) ? pb.ctrl + 1 : nullptr);
     count_launch();
     if (grad_faces) {
         e = cudaMemsetAsync(grad_faces, 0, n * 9 * sizeof(float), stream);
@@ -2159,7 +2171,7 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
     const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
     const size_t smem = raster_dyn_smem(F);
     const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
-#define UMR_LAUNCH_BWD(RGBM, TG)                                                                              \
+#define UMR_LAUNCH_BWD(RGBM, TG, SP)                                                                          \
     do {                                                                                                      \
         if (gen)                                                                                              \
             k_raster_bwd<RGBM, TG><<<grid, CTA, smem, stream>>>(rec, box, textures, soft_colors, aggrs_info,    \
@@ -2168,25 +2180,25 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
             if (pb.cap > 0) {                                                                                 \
                 count_launch();                                                                               \
                 if (forward_impl(p->tile_mode) == 4 && wide)                                                  \
-                    launch_bwd2<RGBM, TG, 32, uint32_t>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
-                                                        grad_images, grad_faces, grad_textures, K, pb);       \
+                    launch_bwd2<RGBM, TG, 32, uint32_t, SP>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
+                                                            grad_images, grad_faces, grad_textures, K, pb);   \
                 else if (forward_impl(p->tile_mode) == 4)                                                     \
-                    launch_bwd2<RGBM, TG, 32, uint16_t>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
-                                                        grad_images, grad_faces, grad_textures, K, pb);       \
+                    launch_bwd2<RGBM, TG, 32, uint16_t, SP>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
+                                                            grad_images, grad_faces, grad_textures, K, pb);   \
                 else if (wide)                                                                                \
-                    launch_bwd2<RGBM, TG, 16, uint32_t>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
-                                                        grad_images, grad_faces, grad_textures, K, pb);       \
+                    launch_bwd2<RGBM, TG, 16, uint32_t, SP>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, \
+                                                            aggrs_info, grad_images, grad_faces, grad_textures, K, pb); \
                 else                                                                                          \
-                    launch_bwd2<RGBM, TG, 16, uint16_t>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
-                                                        grad_images, grad_faces, grad_textures, K, pb);       \
+                    launch_bwd2<RGBM, TG, 16, uint16_t, SP>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, \
+                                                            aggrs_info, grad_images, grad_faces, grad_textures, K, pb); \
             }                                                                                                 \
             if (pb.cap > 0)                                                                                   \
-                k_raster_bwd_pairs_list<RGBM, TG><<<list_grid, CTA, smem, stream>>>(                          \
+                k_raster_bwd_pairs_list<RGBM, TG, 3, SP><<<list_grid, CTA, smem, stream>>>(                   \
                     rec, box, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, ubox, K, \
                     pb.ctrl + 1, pb.ulist, (int)grid_pairs.x, (int)grid_pairs.y);                             \
             else                                                                                              \
-                k_raster_bwd_pairs<RGBM, TG><<<grid_pairs, CTA, smem, stream>>>(rec, box, textures, soft_colors, aggrs_info, \
-                                                                      grad_images, grad_faces, grad_textures, ubox, K); \
+                k_raster_bwd_pairs<RGBM, TG, 3, SP><<<grid_pairs, CTA, smem, stream>>>(rec, box, textures, soft_colors, \
+                                                              aggrs_info, grad_images, grad_faces, grad_textures, ubox, K); \
         }                                                                                                     \
     } while (0)
     const dim3 grid_pairs((K.S + PT - 1) / PT, (K.S + PT - 1) / PT, B);
@@ -2220,23 +2232,43 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
                                                                                grad_faces, grad_textures, ubox, K);
         }
     } else if (softmax) {
-        if (grad_textures) UMR_LAUNCH_BWD(1, true); else UMR_LAUNCH_BWD(1, false);
-    } else {
-        if (grad_textures) UMR_LAUNCH_BWD(0, true); else UMR_LAUNCH_BWD(0, false);
+        if (split) UMR_LAUNCH_BWD(1, true, true);
+        else if (grad_textures) UMR_LAUNCH_BWD(1, true, false);
+        else UMR_LAUNCH_BWD(1, false, false);
+    } else {  // hard colours: the vertex gradients have no colour terms, so the split backward is the full one
+        if (grad_textures) UMR_LAUNCH_BWD(0, true, false); else UMR_LAUNCH_BWD(0, false, false);
     }
 #undef UMR_LAUNCH_BWD
     if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
     return (int)cudaGetLastError();
 }
 
-// Deterministic backward: k_prep, then the face-parallel gather k_raster_bwd_det (no pair buffer, no atomics).  Same inputs
-// and outputs as umr_raster_backward; grad_faces == NULL (texture-only) is accepted.
-extern "C" int umr_raster_backward_deterministic(const float* face_vertices, const float* textures,
-                                                 const float* soft_colors, const float* aggrs_info,
-                                                 const float* grad_images, float* grad_faces, float* grad_textures,
-                                                 const UmrRasterParams* p, void* workspace, void* stream_) {
+extern "C" int umr_raster_backward(const float* face_vertices, const float* textures,
+                                   const float* soft_colors, const float* aggrs_info,
+                                   const float* grad_images, float* grad_faces, float* grad_textures,
+                                   const UmrRasterParams* p, void* workspace, void* stream_) {
     int rc = check_params(p);
     if (rc) return rc;
+    return raster_backward(face_vertices, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, p, workspace,
+                           stream_, false);
+}
+
+extern "C" int umr_raster_backward_split(const float* face_vertices, const float* textures,
+                                         const float* soft_colors, const float* aggrs_info,
+                                         const float* grad_images, float* grad_faces, float* grad_textures,
+                                         const UmrRasterParams* p, void* workspace, void* stream_) {
+    int rc = check_params(p);
+    if (rc) return rc;
+    if (split_refused(p, grad_faces, grad_textures)) return UMR_ERR_BAD_ARG;
+    return raster_backward(face_vertices, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, p, workspace,
+                           stream_, true);
+}
+
+// Deterministic backward: k_prep, then the face-parallel gather k_raster_bwd_det (no pair buffer, no atomics).  Same inputs
+// and outputs as umr_raster_backward; grad_faces == NULL (texture-only) is accepted.  split: see raster_backward.
+static int raster_backward_det(const float* face_vertices, const float* textures, const float* soft_colors,
+                               const float* aggrs_info, const float* grad_images, float* grad_faces, float* grad_textures,
+                               const UmrRasterParams* p, void* workspace, void* stream_, bool split) {
     if ((int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;  // as the forward
     if (!face_vertices || !textures || !soft_colors || !aggrs_info || !grad_images || !workspace) return UMR_ERR_BAD_ARG;
     if (!grad_faces && !grad_textures) return UMR_ERR_BAD_ARG;
@@ -2272,10 +2304,34 @@ extern "C" int umr_raster_backward_deterministic(const float* face_vertices, con
     } while (0)
     if (nc4) k_raster_bwd_det<1, false, 4><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images,
                                                                       grad_faces, grad_textures, K);
+    else if (split && softmax) k_raster_bwd_det<1, true, 3, false, true><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors,
+                                                                                                   aggrs_info, grad_images,
+                                                                                                   grad_faces, grad_textures, K);
     else if (softmax) { if (grad_textures) UMR_BWD_DET(1, true, 3); else UMR_BWD_DET(1, false, 3); }
-    else { if (grad_textures) UMR_BWD_DET(0, true, 3); else UMR_BWD_DET(0, false, 3); }
+    else { if (grad_textures) UMR_BWD_DET(0, true, 3); else UMR_BWD_DET(0, false, 3); }  // hard: split == full
 #undef UMR_BWD_DET
     if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
     count_launch(2);
     return (int)cudaGetLastError();
+}
+
+extern "C" int umr_raster_backward_deterministic(const float* face_vertices, const float* textures,
+                                                 const float* soft_colors, const float* aggrs_info,
+                                                 const float* grad_images, float* grad_faces, float* grad_textures,
+                                                 const UmrRasterParams* p, void* workspace, void* stream_) {
+    int rc = check_params(p);
+    if (rc) return rc;
+    return raster_backward_det(face_vertices, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, p,
+                               workspace, stream_, false);
+}
+
+extern "C" int umr_raster_backward_split_deterministic(const float* face_vertices, const float* textures,
+                                                       const float* soft_colors, const float* aggrs_info,
+                                                       const float* grad_images, float* grad_faces, float* grad_textures,
+                                                       const UmrRasterParams* p, void* workspace, void* stream_) {
+    int rc = check_params(p);
+    if (rc) return rc;
+    if (split_refused(p, grad_faces, grad_textures)) return UMR_ERR_BAD_ARG;
+    return raster_backward_det(face_vertices, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, p,
+                               workspace, stream_, true);
 }

@@ -274,7 +274,11 @@ constexpr int BWD2_THREADS = 256, BWD2_WARPS = BWD2_THREADS / 32;  // threads of
 // plain vector REDs are faster.
 // rec_all: the face records of k_prep (GEOM only): the z-gradient factors w_clip_k / z_k^2 are re-derived from them
 // IdxT: face-index width of the block headers (hdr_shift)
-template <int RGB, bool TEXGRAD, int TS, int NC = 3, bool GEOM = true, bool PRE = false, typename IdxT = uint16_t>  // NC colour channels; pixel planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
+// SPLIT = true (the split backward, softmax only): the vertex gradients keep only the terms driven by the alpha adjoint, the
+// texel gradients are formed from the colour adjoints as always -- one walk serves a mask loss on alpha and a texture loss on
+// RGB whose geometry is detached.  Without the colour terms no face record is read (no z-gradient factors).
+template <int RGB, bool TEXGRAD, int TS, int NC = 3, bool GEOM = true, bool PRE = false, typename IdxT = uint16_t,
+          bool SPLIT = false>  // NC colour channels; pixel planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
 __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const float* __restrict__ rec_all, const float* __restrict__ textures,
                                                         const float* __restrict__ colors_hi,
                                                         const float* __restrict__ aggrs, const float* __restrict__ grad_images,
@@ -284,6 +288,7 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
     __shared__ float s_pix[NV][TS * TS];  // g[NC], g_alpha, C[NC], alpha, ssum, smax (row-major tile pixels)
     __shared__ float s_xp[TS], s_yp[TS];  // pixel centres, built as the forward builds its tables (same bits)
     constexpr int NP = TS * TS;
+    constexpr bool ZGRAD = GEOM && !SPLIT;  // the colour terms of the vertex gradients (they read the face records)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.z;
     const int S = K.S, F = K.F;
@@ -291,7 +296,7 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
     const int32_t head = __ldg(pb.tile_head + tile_id);
     if (head < 0) return;  // empty, or unsaved (k_raster_bwd_pairs handles it)
     const int x0 = blockIdx.x * TS, y0 = blockIdx.y * TS;
-    if (GEOM) {
+    if (ZGRAD) {
         if (tid < TS) s_xp[tid] = pixel_coord(x0 + tid, S);
         else if (tid < 2 * TS) s_yp[tid - TS] = pixel_coord(S - 1 - (y0 + tid - TS), S);
     }
@@ -324,7 +329,7 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
     const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
     float* gtex_img = TEXGRAD ? grad_tex + (size_t)(b / K.tex_div) * K.tex_bs : nullptr;
     float* gf_img = grad_faces + (size_t)b * F * 9;
-    const float* rec_img = GEOM ? rec_all + (size_t)b * F * REC_F : nullptr;
+    const float* rec_img = ZGRAD ? rec_all + (size_t)b * F * REC_F : nullptr;
     // the 128-byte face record of a step is pulled into L1 one step ahead: lanes 1-3 take the 32-byte sectors that hold
     // R_INV and R_IZ2
     auto prefetch_face = [&](int f) {
@@ -427,13 +432,13 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
         const float4 *src_c = nullptr, *src_n = nullptr;
         bool have = plan(f_c, act_c, src_c);
         if (have) prefetch2(act_c, src_c);
-        if (GEOM && have) prefetch_face(f_c);
+        if (ZGRAD && have) prefetch_face(f_c);
         while (have) {
             const bool have_n = plan(f_n, act_n, src_n);
             if (have_n) prefetch2(act_n, src_n);
             const int f = f_c;  // (warp-uniform, like f_n and have_n)
             if (f != cur_f) { flush(); cur_f = f; }
-            if (GEOM && have_n && f_n != f) prefetch_face(f_n);
+            if (ZGRAD && have_n && f_n != f) prefetch_face(f_n);
             int pre_tix = -1;   // PRE: this lane's texel of face f and its NC gradient terms (set below when it contributes)
             float pre_v[NC];
 #pragma unroll
@@ -487,12 +492,12 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
                                 }
                             }
                             float Crgb = 0.f;
-                            if (GEOM) {
+                            if (ZGRAD) {
 #pragma unroll
                                 for (int c = 0; c < NC; ++c) Crgb += g[c] * (__ldg(tex_img + to + c) - sp[(NPL + c) * NP]);
                                 Crgb *= s;
                             }
-                            if (GEOM && Crgb != 0.f) {
+                            if (ZGRAD && Crgb != 0.f) {
                                 Cxy += __fdividef(Crgb, D);
                                 const float zp = K.far_ - zn * (K.far_ - K.near_);
                                 const float Cz = Crgb * K.r_gamma * K.r_nf * zp * zp;  // :624

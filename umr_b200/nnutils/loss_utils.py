@@ -314,7 +314,6 @@ class MultiTextureLoss(nn.Module):
 
     def forward(self, vs, fs, cams_all_hypo, cam_probs, proj_cam, rgbs, masks_gt, masks_pred, tx, tex_flow,
                 dts_barrier):
-        H = self.num_hypo_cams
         # textured softmax render of every hypothesis; vertices detached: only the texture learns here (:313)
         # ... and neither is the [B*8,F,T2,3] texture copy of loss_utils.py:305 (70.8 MB at batch 16): the raster kernels
         # read textures[b // 8] and accumulate the 8 hypotheses' texture gradients directly
@@ -325,6 +324,13 @@ class MultiTextureLoss(nn.Module):
         else:
             texture_rgba, _, _ = self.renderer.forward(vs.detach(), fs, cams_all_hypo.view(-1, 7), tx)
             texture_pred = texture_rgba[:, 0:3, :, :]
+        tex_loss, tex_dt_loss, tex_cycle_loss = self._losses(vs, fs, cam_probs, proj_cam, rgbs, masks_gt, masks_pred,
+                                                             texture_pred, tex_flow, dts_barrier)
+        return tex_loss, tex_dt_loss, tex_cycle_loss, texture_pred
+
+    def _losses(self, vs, fs, cam_probs, proj_cam, rgbs, masks_gt, masks_pred, texture_pred, tex_flow, dts_barrier):
+        """(tex_loss, tex_dt_loss, tex_cycle_loss) of the rendered `texture_pred` (loss_utils.py:320-331)."""
+        H = self.num_hypo_cams
         per_render = self.texture_loss(texture_pred, tile_hypotheses(rgbs, H), tile_hypotheses(masks_gt, H),
                                        masks_pred, avg=False)
         tex_loss = expected_over_hypotheses(per_render, cam_probs)
@@ -341,7 +347,50 @@ class MultiTextureLoss(nn.Module):
             p2f_info, aggr_info = self.hard_renderer.visibility(vs.detach(), fs, proj_cam.detach())
             face_ids = aggr_info[:, 1, :, :].reshape(vs.size(0), -1)
             tex_cycle_loss, _ = self.texture_cycle_fn(tex_flow, p2f_info.detach(), face_ids.detach())
-        return tex_loss, tex_dt_loss, tex_cycle_loss, texture_pred
+        return tex_loss, tex_dt_loss, tex_cycle_loss
+
+
+class MultiMaskTextureLoss(nn.Module):
+    """MultiMaskLoss and MultiTextureLoss of one train_s2 step (experiments/train_s2.py:226-248) from ONE render.  Both
+    render the same geometry from the same camera hypotheses in the same raster configuration, and alpha (prod) depends
+    on neither light nor texture, so the textured render's alpha plane is the mask render's.  `SoftRenderer.render_split`
+    renders once and splits the backward: the alpha plane's gradient reaches the geometry and cameras, the RGB planes'
+    the textures only.  Not a reference name -- an addition; it returns what
+
+        mask_loss, mask_all_hypo = MultiMaskLoss(...)(vs, fs, cams_all_hypo, cam_probs, masks_gt)
+        tex_loss, tex_dt_loss, tex_cycle_loss, texture_pred = MultiTextureLoss(...)(
+            vs.detach(), fs, cams_all_hypo.detach(), cam_probs.detach(), proj_cam, rgbs, masks_gt, mask_all_hypo, tx,
+            tex_flow, dts_barrier)
+
+    returns, with the same gradients (mask_all_hypo is the texture loss's `masks_pred`, undetached, as in the reference).
+    The constructor takes the union of the two modules' arguments; with renderer="nmr" the two modules run as above."""
+
+    def __init__(self, samples_per_gpu=32, num_hypo_cams=8, image_size=256, renderer_type="softmax",
+                 texture_loss_type="perceptual", renderer="smr"):
+        super().__init__()
+        self.mask_loss_fn = MultiMaskLoss(image_size, renderer_type, num_hypo_cams)
+        self.texture_loss_fn = MultiTextureLoss(samples_per_gpu, num_hypo_cams, image_size, renderer_type, texture_loss_type,
+                                                renderer)
+        self.num_hypo_cams = num_hypo_cams
+
+    def forward(self, vs, fs, cams_all_hypo, cam_probs, proj_cam, rgbs, masks_gt, tx, tex_flow, dts_barrier):
+        """-> (mask_loss, mask_all_hypo, tex_loss, tex_dt_loss, tex_cycle_loss, texture_pred)"""
+        tl = self.texture_loss_fn
+        if tl.which_renderer in "nmr":
+            mask_loss, mask_all_hypo = self.mask_loss_fn(vs, fs, cams_all_hypo, cam_probs, masks_gt)
+            out = tl(vs.detach(), fs, cams_all_hypo.detach(), cam_probs.detach(), proj_cam, rgbs, masks_gt, mask_all_hypo, tx,
+                     tex_flow, dts_barrier)
+            return (mask_loss, mask_all_hypo) + tuple(out)
+        H = self.num_hypo_cams
+        # the texture renderer's light (ambient only) colours the RGB planes; alpha is the mask render's
+        rgba, _, _ = tl.renderer.render_split(vs, fs, cams_all_hypo.view(-1, 7), tx)
+        mask_all_hypo = rgba[:, 3, :, :]
+        per_render = neg_iou_loss(mask_all_hypo, tile_hypotheses(masks_gt, H), avg=False)
+        mask_loss = expected_over_hypotheses(per_render, cam_probs)
+        texture_pred = rgba[:, 0:3, :, :]
+        tex_loss, tex_dt_loss, tex_cycle_loss = tl._losses(vs.detach(), fs, cam_probs.detach(), proj_cam, rgbs, masks_gt,
+                                                           mask_all_hypo, texture_pred, tex_flow, dts_barrier)
+        return mask_loss, mask_all_hypo, tex_loss, tex_dt_loss, tex_cycle_loss, texture_pred
 
 
 # ---------------------------------------------------------------------------------------------

@@ -99,6 +99,39 @@ class SoftRenderer(torch.nn.Module):
                 tex = textures * torch.tensor(c, dtype=torch.float32, device=fv.device)
         return r.rasterizer.rasterize(fv, tex)
 
+    def render_split(self, vertices, faces, cams, textures):
+        """One textured render whose gradient is split between two losses, as UMR's mask and texture branches use it
+        (experiments/train_s2.py: MultiMaskLoss on the live geometry, MultiTextureLoss on detached geometry and cameras):
+        images [B*H,4,is,is] (+ p2f_info, aggrs_info) with this renderer's light, cameras broadcast as in `forward`.  The
+        gradient of images[:, 3] (alpha, which depends on neither light nor texture) reaches `vertices` and `cams`; that of
+        images[:, :3] reaches `textures` only, as if the geometry of the RGB render were detached.
+
+        Fused configuration: one vertex kernel, one raster forward and one split raster backward.  Elsewhere (float64, CPU,
+        other raster modes) two ordinary renders: alpha from the live geometry, RGB from the detached one."""
+        r = self.renderer
+        if self._fusable(vertices) and r.rasterizer.supports_split():
+            tr = r.transform.transformer
+            amb, dl = r.lighting.ambient, r.lighting.directionals[0]
+            light_cfg = None
+            if float(dl.light_intensity) != 0.0:
+                light_cfg = (amb.light_intensity, amb.light_color, dl.light_intensity, dl.light_color, dl.light_direction)
+            fv, light = project_faces(vertices, cams, faces, offset_z=self.offset_z, eye_z=float(tr._eye[2]),
+                                      viewing_scale=tr.viewing_scale, flip_y=True, light=light_cfg)
+            B, F = fv.shape[:2]
+            if light is not None:
+                # the RGB planes' gradient must not reach the geometry through the light either
+                light = light.detach()
+                if textures.shape[0] not in (1, B):
+                    textures = textures.repeat_interleave(B // textures.shape[0], dim=0)
+                tex = textures * light[:, :, None, :]
+            else:
+                c = [float(amb.light_intensity) * float(k) for k in amb.light_color]
+                tex = textures if c == [1.0, 1.0, 1.0] else textures * torch.tensor(c, dtype=torch.float32, device=fv.device)
+            return r.rasterizer.rasterize_split(fv, tex)
+        alpha = self.forward(vertices, faces, cams)[0][:, 3:4]
+        rgba, p2f, aggrs = self.forward(vertices.detach(), faces, cams.detach(), textures)
+        return torch.cat((rgba[:, :3], alpha), dim=1), p2f, aggrs
+
     def visibility(self, vertices, faces, cams):
         """(p2f_info, aggrs_info) of this renderer WITHOUT the image: what `MultiTextureLoss` keeps of its hard render
         (loss_utils.py:327-329, `_, p2f_info, aggr_info = self.hard_renderer(...)`).  For the hard renderer on CUDA this

@@ -341,6 +341,66 @@ def soft_rasterize(face_vertices, textures, image_size=256, background_color=(0,
                                        aggr_func_rgb, aggr_func_alpha, texture_type, anti_aliasing)
 
 
+class SoftRasterizeSplitFunction(torch.autograd.Function):
+    """The forward of SoftRasterizeFunction; the backward sends the alpha plane's adjoint to `face_vertices` and the RGB
+    planes' adjoint to `textures` only (umr_raster_backward_split): one render serves a mask loss on alpha and a texture
+    loss on RGB whose geometry is detached.  float32 in UMR's configuration (euclidean / prod / surface, 3 colour channels)
+    only -- other calls raise; `SoftRenderer.render_split` composes two ordinary renders there.
+
+    Not a subclass of SoftRasterizeFunction: a subclass would inherit whatever `apply` is assigned on that class (a wrapper
+    that counts or captures its calls, say) and run the plain backward in place of the split one."""
+
+    @staticmethod
+    def forward(ctx, face_vertices, textures, image_size=256, background_color=(0, 0, 0), near=1,
+                far=100, fill_back=True, eps=1e-3, sigma_val=1e-5, dist_func="euclidean",
+                dist_eps=1e-4, gamma_val=1e-4, aggr_func_rgb="softmax", aggr_func_alpha="prod",
+                texture_type="surface", anti_aliasing=False):
+        if face_vertices.dtype == torch.float64:
+            raise ValueError("the split raster backward is float32 only: render float64 meshes twice (SoftRenderer.render_split)")
+        if dist_func != "euclidean" or aggr_func_alpha != "prod" or texture_type != "surface":
+            raise ValueError("the split raster backward covers euclidean distance, prod alpha and surface textures only")
+        if int(textures.shape[-1]) != 3:
+            raise ValueError("the split raster backward takes 3 colour channels, got %d" % int(textures.shape[-1]))
+        return SoftRasterizeFunction.forward(ctx, face_vertices, textures, image_size, background_color, near, far, fill_back,
+                                             eps, sigma_val, dist_func, dist_eps, gamma_val, aggr_func_rgb, aggr_func_alpha,
+                                             texture_type, anti_aliasing)
+
+    @staticmethod
+    def backward(ctx, grad_images, grad_p2f=None, grad_aggrs=None):
+        mode = ctx.mode
+        if ctx.has_pairs:
+            fv, tex, colors_hi, aggrs, pairs = ctx.saved_tensors
+            assert ctx.params.pair_buffer == pairs.data_ptr()
+        else:
+            fv, tex, colors_hi, aggrs = ctx.saved_tensors
+        dev = fv.device
+        B, F = fv.shape[:2]
+        g = grad_images.contiguous().to(mode.dtype)
+        _attach_events(ctx.params, "bwd")
+        with torch.cuda.device(dev):
+            # the split kernels take both outputs; one nobody asked for is scratch
+            grad_faces = torch.empty_like(fv)
+            grad_tex = torch.empty_like(tex)
+            ws_bytes, _ = mode.symbol("umr_raster_workspace_bytes", True)
+            ws = torch.empty(ws_bytes(B, F, ctx.params.image_size, ctx.params.anti_aliasing), device=dev, dtype=torch.uint8)
+            mode.call("umr_raster_backward_split", True, _ptr(fv), _ptr(tex), _ptr(colors_hi), _ptr(aggrs), _ptr(g),
+                      _ptr(grad_faces), _ptr(grad_tex), ctypes.byref(ctx.params), _ptr(ws), _stream_ptr(dev))
+        ctx.params.ev_kernel_start = ctx.params.ev_kernel_stop = None
+        return ((grad_faces.view(ctx.in_shape) if ctx.geom_needs_grad else None),
+                (grad_tex if ctx.tex_needs_grad else None)) + (None,) * 14
+
+
+def soft_rasterize_split(face_vertices, textures, image_size=256, background_color=(0, 0, 0), near=1, far=100,
+                         fill_back=True, eps=1e-3, sigma_val=1e-5, dist_func="euclidean", dist_eps=1e-4,
+                         gamma_val=1e-4, aggr_func_rgb="softmax", aggr_func_alpha="prod", texture_type="surface",
+                         anti_aliasing=False):
+    """`soft_rasterize` with the split gradient of SoftRasterizeSplitFunction: same arguments, same (images, p2f_info,
+    aggrs_info); the gradient of images[:, 3] reaches only `face_vertices`, that of images[:, :3] only `textures`."""
+    return SoftRasterizeSplitFunction.apply(face_vertices, textures, image_size, background_color, near, far,
+                                            fill_back, eps, sigma_val, dist_func, dist_eps, gamma_val,
+                                            aggr_func_rgb, aggr_func_alpha, texture_type, anti_aliasing)
+
+
 def visibility(face_vertices, image_size=256, near=1, far=100, fill_back=True, eps=1e-3, sigma_val=1e-5,
                dist_eps=1e-4, gamma_val=1e-4, anti_aliasing=False, want_faces=False):
     """The hard z-buffer's winner per raster pixel and nothing else: returns aggrs_info [B,2,S,S] = (depth_min,

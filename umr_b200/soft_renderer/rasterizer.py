@@ -2,7 +2,7 @@
 and error messages); the 2x supersampling + `avg_pool2d` of rasterizer.py:43,52-53 is fused into the kernels."""
 import torch.nn as nn
 
-from ..raster import soft_rasterize, visibility
+from ..raster import soft_rasterize, soft_rasterize_split, visibility
 from ._args import bind
 
 # (name, default) in the reference's positional order
@@ -35,6 +35,15 @@ class SoftRasterizer(nn.Module):
     def rasterize(self, face_vertices, face_textures):
         """Rasterise raster-space face vertices [B,F,3,3] with face textures [B,F,T2,3]."""
         return soft_rasterize(face_vertices, face_textures, *[getattr(self, k) for k in KERNEL_ARGS])
+
+    def rasterize_split(self, face_vertices, face_textures):
+        """`rasterize` whose backward sends the alpha plane's gradient to the geometry and the RGB planes' gradient to the
+        textures only (raster.soft_rasterize_split); see supports_split."""
+        return soft_rasterize_split(face_vertices, face_textures, *[getattr(self, k) for k in KERNEL_ARGS])
+
+    def supports_split(self):
+        """The split backward exists for UMR's configuration (euclidean / prod / surface), softmax or hard colours."""
+        return self.dist_func == "euclidean" and self.aggr_func_alpha == "prod" and self.texture_type == "surface"
 
     def supports_visibility(self):
         """The visibility-only kernel exists for UMR's configuration of the hard renderer (nnutils/smr.py:52-58)."""
