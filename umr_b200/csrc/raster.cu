@@ -36,22 +36,14 @@
 #include <stdint.h>
 
 #include "common.cuh"
+#include "raster_generic.cuh"
 #include "umr_b200.h"
 
 namespace umr {
 
-constexpr int TILE = 16;
-constexpr int CTA = TILE * TILE;  // 256 threads, one pixel each
 constexpr int CHUNK = 32;         // face records per TMA stage
 constexpr int NSTAGE = 2;
-constexpr int REC_F = 32;         // floats per record (128 B)
-
-// record layout (float index)
-constexpr int R_V = 0;     // 9 : x0 y0 z0 x1 y1 z1 x2 y2 z2
-constexpr int R_INV = 9;   // 9 : barycentric inverse, row-major
-constexpr int R_SYM = 18;  // 6 : s00 s01 s02 s11 s12 s22   (Gram + 1)
-constexpr int R_BOX = 24;  // 4 : xlo xhi ylo yhi (cull box, already expanded by r)
-constexpr int R_FLG = 28;  // 1 : bit0..2 obtuse corner, bit3 front-facing
+// float records (layout in raster_generic.cuh) also carry, after the flags:
 constexpr int R_IZ2 = 29;  // 3 : 1 / (z_k * z_k)  (backward z-gradient factor)
 
 // Face indices.  Meshes of up to NARROW_MAX_FACES faces keep them in 16 bits (coarse-bin lists, tile lists, pair-block
@@ -82,7 +74,7 @@ inline WorkspaceLayout ws_layout(int B, int F, int S) {
     const size_t ncb = (size_t)(S + COARSE_BIN - 1) / COARSE_BIN;
     const size_t nbin = (size_t)B * ncb * ncb;
     L.rec_off = 0;
-    L.box_off = align256(n * REC_F * sizeof(float));
+    L.box_off = align256(n * REC_LEN * sizeof(float));
     L.p2f_off = L.box_off + align256(n * sizeof(float4));
     L.ubox_off = L.p2f_off + align256(n * 4 * sizeof(float));
     L.ccount_off = L.ubox_off + align256((size_t)B * 4 * sizeof(uint32_t));
@@ -133,7 +125,7 @@ __global__ void __launch_bounds__(256) k_prep(const float* __restrict__ fv, floa
     // max(det, 1e-10) / min(det, -1e-10) are evaluated in double by the reference and stored as
     // float; a float select against the rounded constant is bit-identical (DESIGN.md §4).
     det = det > 0 ? fmaxf(det, 1e-10f) : fminf(det, -1e-10f);
-    float out[REC_F];
+    float out[REC_LEN];
 #pragma unroll
     for (int k = 0; k < 9; ++k) out[R_V + k] = v[k];
 #pragma unroll
@@ -172,9 +164,9 @@ __global__ void __launch_bounds__(256) k_prep(const float* __restrict__ fv, floa
     out[R_IZ2 + 1] = 1.f / (v[5] * v[5]);
     out[R_IZ2 + 2] = 1.f / (v[8] * v[8]);
     if (valid) {
-        float4* dst = reinterpret_cast<float4*>(rec + (size_t)i * REC_F);
+        float4* dst = reinterpret_cast<float4*>(rec + (size_t)i * REC_LEN);
 #pragma unroll
-        for (int k = 0; k < REC_F / 4; ++k)
+        for (int k = 0; k < REC_LEN / 4; ++k)
             dst[k] = make_float4(out[4 * k], out[4 * k + 1], out[4 * k + 2], out[4 * k + 3]);
         box[i] = make_float4(xlo, xhi, ylo, yhi);
     }
@@ -201,167 +193,6 @@ __device__ __forceinline__ bool tile_outside_union(const uint32_t* __restrict__ 
     const float yhi = __uint_as_float(u.z), ylo = -__uint_as_float(u.w);
     return s_ext[0] > xhi || s_ext[1] < xlo || s_ext[2] > yhi || s_ext[3] < ylo;
 }
-
-// ---------------------------------------------------------------------------------------------
-// shared per-(pixel, face) math
-// ---------------------------------------------------------------------------------------------
-struct Frag {
-    float w0, w1, w2;  // unclipped barycentrics
-    float t0, t1, t2;  // closest-point barycentrics minus w
-    float sign, dx, dy, dis, D;
-};
-
-// kernel.cu:325-326 evaluates (2.*i + 1. - S) / S in double and stores a float.  Numerator and
-// denominator are integers < 2^24 (exact in float), and rounding a correctly rounded binary64 quotient
-// to binary32 equals the correctly rounded binary32 quotient whenever the wide format carries at least
-// 2p+2 = 50 bits (Figueroa's double-rounding theorem; binary64 has 53).  So one IEEE float division is
-// bit-identical and ~4x cheaper than the double one.
-__device__ __forceinline__ float pixel_coord(int i, int S) {
-    return __fdiv_rn((float)(2 * i + 1 - S), (float)S);
-}
-
-// euclidean signed distance + sigmoid: kernel.cu:62-152, 380-383.  `rc` points at a staged record.
-// Returns false when the pair is culled (outside and farther than the threshold).
-__device__ __forceinline__ bool fragment(const float* __restrict__ rc, float xp, float yp, float thr,
-                                         float sigma, Frag& fr) {
-    const float w0 = rc[R_INV + 0] * xp + rc[R_INV + 1] * yp + rc[R_INV + 2];
-    const float w1 = rc[R_INV + 3] * xp + rc[R_INV + 4] * yp + rc[R_INV + 5];
-    const float w2 = rc[R_INV + 6] * xp + rc[R_INV + 7] * yp + rc[R_INV + 8];
-    fr.w0 = w0; fr.w1 = w1; fr.w2 = w2;
-    const float fx0 = rc[0], fy0 = rc[1], fx1 = rc[3], fy1 = rc[4], fx2 = rc[6], fy2 = rc[7];
-    const float s00 = rc[R_SYM + 0], s01 = rc[R_SYM + 1], s02 = rc[R_SYM + 2];
-    const float s11 = rc[R_SYM + 3], s12 = rc[R_SYM + 4], s22 = rc[R_SYM + 5];
-    // inside pixels (kernel.cu:76-110) keep the nearest of the three edges; outside pixels (:111-147) project on the ONE
-    // edge selected by the sign pattern of w (with the obtuse-corner correction) and clamp
-    float dx, dy, t0, t1, t2;
-    if (w0 > 0 && w1 > 0 && w2 > 0 && w0 < 1 && w1 < 1 && w2 < 1) {
-        float best = 100000000.f;
-        // edge k=0: v0=0,v1=1,v2=2    a = sym[0,:] - sym[1,:]
-        {
-            const float a0 = s00 - s01, a1 = s01 - s11, a2 = s02 - s12;
-            float u0 = (w0 * a0 + w1 * a1 + w2 * a2 - a1) / (a0 - a1);
-            float u1 = 1 - u0;
-            float u2 = 0;
-            u0 -= w0; u1 -= w1; u2 -= w2;
-            const float ex = u0 * fx0 + u1 * fx1 + u2 * fx2;
-            const float ey = u0 * fy0 + u1 * fy1 + u2 * fy2;
-            const float d = ex * ex + ey * ey;
-            dx = 0.f; dy = 0.f; t0 = t1 = t2 = 0.f;
-            if (d < best) { best = d; dx = ex; dy = ey; t0 = u0; t1 = u1; t2 = u2; }
-        }
-        // edge k=1: v0=1,v1=2,v2=0    a = sym[1,:] - sym[2,:]
-        {
-            const float a0 = s01 - s02, a1 = s11 - s12, a2 = s12 - s22;
-            float u1 = (w0 * a0 + w1 * a1 + w2 * a2 - a2) / (a1 - a2);
-            float u2 = 1 - u1;
-            float u0 = 0;
-            u0 -= w0; u1 -= w1; u2 -= w2;
-            const float ex = u0 * fx0 + u1 * fx1 + u2 * fx2;
-            const float ey = u0 * fy0 + u1 * fy1 + u2 * fy2;
-            const float d = ex * ex + ey * ey;
-            if (d < best) { best = d; dx = ex; dy = ey; t0 = u0; t1 = u1; t2 = u2; }
-        }
-        // edge k=2: v0=2,v1=0,v2=1    a = sym[2,:] - sym[0,:]
-        {
-            const float a0 = s02 - s00, a1 = s12 - s01, a2 = s22 - s02;
-            float u2 = (w0 * a0 + w1 * a1 + w2 * a2 - a0) / (a2 - a0);
-            float u0 = 1 - u2;
-            float u1 = 0;
-            u0 -= w0; u1 -= w1; u2 -= w2;
-            const float ex = u0 * fx0 + u1 * fx1 + u2 * fx2;
-            const float ey = u0 * fy0 + u1 * fy1 + u2 * fy2;
-            const float d = ex * ex + ey * ey;
-            if (d < best) { best = d; dx = ex; dy = ey; t0 = u0; t1 = u1; t2 = u2; }
-        }
-        fr.sign = 1.f;
-    } else {
-        const uint32_t flg = __float_as_uint(rc[R_FLG]);
-        int v0 = -1;
-        if (w1 <= 0 && w2 <= 0) {
-            v0 = 0;
-            if ((flg & 1u) && (xp - fx0) * (fx2 - fx0) + (yp - fy0) * (fy2 - fy0) > 0) v0 = 2;
-        } else if (w2 <= 0 && w0 <= 0) {
-            v0 = 1;
-            if ((flg & 2u) && (xp - fx1) * (fx0 - fx1) + (yp - fy1) * (fy0 - fy1) > 0) v0 = 0;
-        } else if (w0 <= 0 && w1 <= 0) {
-            v0 = 2;
-            if ((flg & 4u) && (xp - fx2) * (fx1 - fx2) + (yp - fy2) * (fy1 - fy2) > 0) v0 = 1;
-        } else if (w0 <= 0) v0 = 1;
-        else if (w1 <= 0) v0 = 2;
-        else if (w2 <= 0) v0 = 0;
-        // all w > 0 but some w >= 1 (rounding): undefined in the reference (kernel.cu:128-139 runs
-        // with v0 = -1).  Defined as "corner with the largest barycentric", like oracle B.
-        if (v0 < 0) v0 = w0 >= w1 ? (w0 >= w2 ? 0 : 2) : (w1 >= w2 ? 1 : 2);
-        float u0, u1, u2;
-        if (v0 == 0) {  // v1 = 1, v2 = 2
-            const float a0 = s00 - s01, a1 = s01 - s11, a2 = s02 - s12;
-            u0 = (w0 * a0 + w1 * a1 + w2 * a2 - a1) / (a0 - a1);
-            u1 = 1 - u0;
-            u2 = 0;
-        } else if (v0 == 1) {  // v1 = 2, v2 = 0
-            const float a0 = s01 - s02, a1 = s11 - s12, a2 = s12 - s22;
-            u1 = (w0 * a0 + w1 * a1 + w2 * a2 - a2) / (a1 - a2);
-            u2 = 1 - u1;
-            u0 = 0;
-        } else {  // v0 = 2, v1 = 0, v2 = 1
-            const float a0 = s02 - s00, a1 = s12 - s01, a2 = s22 - s02;
-            u2 = (w0 * a0 + w1 * a1 + w2 * a2 - a0) / (a2 - a0);
-            u0 = 1 - u2;
-            u1 = 0;
-        }
-        // min(max(t, 0.), 1.) in double then float == float clamp (values are only selected)
-        u0 = fminf(fmaxf(u0, 0.f), 1.f) - w0;
-        u1 = fminf(fmaxf(u1, 0.f), 1.f) - w1;
-        u2 = fminf(fmaxf(u2, 0.f), 1.f) - w2;
-        t0 = u0; t1 = u1; t2 = u2;
-        dx = t0 * fx0 + t1 * fx1 + t2 * fx2;
-        dy = t0 * fy0 + t1 * fy1 + t2 * fy2;
-        fr.sign = -1.f;
-    }
-    const float dis = dx * dx + dy * dy;
-    if (fr.sign < 0 && dis >= thr) return false;
-    fr.t0 = t0; fr.t1 = t1; fr.t2 = t2;
-    fr.dx = dx; fr.dy = dy; fr.dis = dis;
-    // 1. / (1. + exp(-sign * dis / sigma)): float exp, double add + divide, float result (:383)
-    const float e = expf(-fr.sign * dis / sigma);
-    fr.D = (float)(1. / (1. + (double)e));
-    return true;
-}
-
-// NaN-aware note: fmaxf/fminf return the non-NaN operand whereas the reference's comparisons
-// propagate differently; inputs with NaN coordinates are outside the supported domain.
-
-__device__ __forceinline__ void clip_bary(float& w0, float& w1, float& w2) {  // kernel.cu:54-59
-    const float hi = (float)(1 - 1e-5), lo = (float)1e-5;
-    w0 = fmaxf(fminf(w0, hi), lo);
-    w1 = fmaxf(fminf(w1, hi), lo);
-    w2 = fmaxf(fminf(w2, hi), lo);
-    const float s = fmaxf(w0 + w1 + w2, lo);
-    w0 /= s; w1 /= s; w2 /= s;
-}
-
-__device__ __forceinline__ float depth_of(const float* __restrict__ rc, float c0, float c1, float c2) {
-    // kernel.cu:403: 1. / (float sum) in double, stored as float == 1.f / sum in float (same theorem:
-    // both operands are floats, the binary64 quotient is rounded once more to binary32).
-    return __fdiv_rn(1.f, c0 / rc[2] + c1 / rc[5] + c2 / rc[8]);
-}
-
-__device__ __forceinline__ int texel_index(float c0, float c1, int R) {  // kernel.cu:180-190
-    const int wx = (int)(c0 * R);
-    const int wy = (int)(c1 * R);
-    if ((c0 + c1) * R - wx - wy <= 1) return wy * R + wx;
-    return (R - 1 - wy) * R + (R - 1 - wx);
-}
-
-struct Consts {
-    float thr, sigma, gamma, near_, far_, inv_unused;
-    float r_sigma, r_gamma, r_fn, r_nf;  // 1/sigma, 1/gamma, 1/(far-near), 1/(near-far): streamed backward only
-    int F, T2, R, S, IS, aa, double_side;
-    int dist, alpha, tex;  // mode ids (read only by the generic-mode kernels)
-    int vec_store;         // 1: forward may use the shared-staged 128-bit store epilogue (alignment checked on host)
-    size_t tex_bs;         // elements per texture (F*T2*3)
-    int tex_div;           // consecutive images sharing one texture (1: per-image, B: one batch-shared texture)
-};
 
 // ---------------------------------------------------------------------------------------------
 // Deterministic mode (umr_raster_*_deterministic, DESIGN.md §3): the forward adds its per-(warp, face) p2f partials as
@@ -407,96 +238,15 @@ __device__ __forceinline__ void red_p2f_fixed(unsigned long long* acc, float x, 
     red_fixed(acc + 2 * P2F_LIMBS, acc + 3 * P2F_LIMBS, w);
 }
 
-// Texel-gradient sinks of bwd_pair_acc: the recompute backward adds a pair's texel gradient with REDs; the deterministic
-// gather takes it out (address and values) and combines the warp's lanes in a fixed order instead.
-struct TexRedSink {
-    __device__ __forceinline__ void add3(float* p, float a, float b, float c) const { red_add3_global(p, a, b, c); }
-    __device__ __forceinline__ void add(float* p, float v) const { red_add_global(p, v); }
-};
-// A pair adds to at most 9 consecutive floats (a surface texel's 3 channels, or a vertex texture's 3 corner colours) at
-// ascending addresses: *addr = the first, val[k] = the value for *addr + k.
-struct TexTakeSink {
-    float** addr;
-    float* val;
-    __device__ __forceinline__ void add3(float* p, float a, float b, float c) const {
-        *addr = p; val[0] = a; val[1] = b; val[2] = c;
-    }
-    __device__ __forceinline__ void add(float* p, float v) const {
-        if (*addr == nullptr) *addr = p;
-        val[p - *addr] = v;
-    }
-};
-
-// ---------------------------------------------------------------------------------------------
-// Modes UMR does not exercise (SURVEY.md §8f-3): hard / barycentric distance, hard / sum alpha, per-vertex
-// textures.  They run through the generic per-pixel kernels k_raster_fwd / k_raster_bwd, which read the mode
-// ids from Consts at run time; the UMR configuration (euclidean, prod, surface) has its own kernels.
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool fragment_any(const float* __restrict__ rc, float xp, float yp, const Consts& K, Frag& fr) {
-    if (K.dist == UMR_DIST_EUCLIDEAN) return fragment(rc, xp, yp, K.thr, K.sigma, fr);
-    const float w0 = rc[R_INV + 0] * xp + rc[R_INV + 1] * yp + rc[R_INV + 2];
-    const float w1 = rc[R_INV + 3] * xp + rc[R_INV + 4] * yp + rc[R_INV + 5];
-    const float w2 = rc[R_INV + 6] * xp + rc[R_INV + 7] * yp + rc[R_INV + 8];
-    fr.w0 = w0; fr.w1 = w1; fr.w2 = w2;
-    fr.t0 = w0; fr.t1 = w1; fr.t2 = w2;  // kernel.cu:551 (barycentric backward uses the unclipped w)
-    fr.sign = 0.f; fr.dx = 0.f; fr.dy = 0.f; fr.dis = 0.f;
-    if (K.dist == UMR_DIST_HARD) {  // kernel.cu:370-372
-        const bool inside = w0 <= 1 && w0 >= 0 && w1 <= 1 && w1 >= 0 && w2 <= 1 && w2 >= 0;
-        fr.D = inside ? 1.f : 0.f;
-        return inside;
-    }
-    // barycentric distance, kernel.cu:156-159, 374-377
-    float m = w0 > w1 ? (w1 > w2 ? w2 : w1) : (w0 > w2 ? w2 : w0);
-    const float dis = m > 0 ? m * m : -(m * m);
-    if (-dis >= K.thr) return false;
-    fr.dis = dis;
-    fr.D = (float)(1. / (1. + (double)expf(-dis / K.sigma)));
-    return true;
-}
-
-// colour channel k of face texture `tx` (surface: [T2,3] texels; vertex: [3,3] corner colours), kernel.cu:179-195
-__device__ __forceinline__ void sample_texture(const float* __restrict__ tx, float c0, float c1, float c2, const Consts& K,
-                                               float& r, float& g, float& b) {
-    if (K.tex == UMR_TEX_SURFACE) {
-        const float* t = tx + (size_t)texel_index(c0, c1, K.R) * 3;
-        r = __ldg(t); g = __ldg(t + 1); b = __ldg(t + 2);
-    } else {
-        r = c0 * __ldg(tx + 0) + c1 * __ldg(tx + 3) + c2 * __ldg(tx + 6);
-        g = c0 * __ldg(tx + 1) + c1 * __ldg(tx + 4) + c2 * __ldg(tx + 7);
-        b = c0 * __ldg(tx + 2) + c1 * __ldg(tx + 5) + c2 * __ldg(tx + 8);
-    }
-}
-
-// texture gradient of one pair: adds wgt * (g0,g1,g2) to the sampled texel (surface) or w_j * wgt * g to the
-// three corner colours (vertex), kernel.cu:597-601 / 610-616 with the intended texel semantics (App. B-1)
-template <class Sink = TexRedSink>
-__device__ __forceinline__ void add_texture_grad(float* __restrict__ gt, float c0, float c1, float c2, const Consts& K,
-                                                 float wgt, float g0, float g1, float g2, bool weighted, Sink sink = Sink()) {
-    if (K.tex == UMR_TEX_SURFACE) {
-        float* t = gt + (size_t)texel_index(c0, c1, K.R) * 3;
-        sink.add(t + 0, weighted ? wgt * g0 : g0);
-        sink.add(t + 1, weighted ? wgt * g1 : g1);
-        sink.add(t + 2, weighted ? wgt * g2 : g2);
-    } else {
-        const float w[3] = {c0, c1, c2};
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-            sink.add(gt + 3 * j + 0, weighted ? wgt * (w[j] * g0) : w[j] * g0);
-            sink.add(gt + 3 * j + 1, weighted ? wgt * (w[j] * g1) : w[j] * g1);
-            sink.add(gt + 3 * j + 2, weighted ? wgt * (w[j] * g2) : w[j] * g2);
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------------------------
 // tile machinery shared by forward and backward
 // ---------------------------------------------------------------------------------------------
 constexpr int PT = 16;          // pixel-tile side of the pair-parallel backward kernel (32 is the A/B alternative)
+static_assert(PT * PT == CTA, "k_raster_bwd_det stages one per-pixel slot per thread; bwd_pair_acc reads them with stride PT * PT");
 constexpr int BOX_PIECE = 2048;  // cull boxes staged per TMA bulk copy (32 KB)
-constexpr int NWARP = CTA / 32;
 
 // dynamic shared memory: [ records NSTAGE*CHUNK*128 B | cull boxes min(F,BOX_PIECE)*16 B | list u16[F] ]
-__host__ __device__ inline size_t smem_box_off() { return (size_t)NSTAGE * CHUNK * REC_F * 4; }
+__host__ __device__ inline size_t smem_box_off() { return (size_t)NSTAGE * CHUNK * REC_LEN * 4; }
 __host__ __device__ inline size_t smem_list_off(int F) {
     return smem_box_off() + (size_t)(F < BOX_PIECE ? F : BOX_PIECE) * 16;
 }
@@ -566,7 +316,7 @@ __device__ __forceinline__ void issue_chunk(const float* __restrict__ rec_img, c
     const int idx = c * CHUNK + j;
     if (idx < n) {
         const int f = list[idx];
-        cp_async16(s_rec + ((size_t)(c % NSTAGE) * CHUNK + j) * REC_F + q * 4, rec_img + (size_t)f * REC_F + q * 4);
+        cp_async16(s_rec + ((size_t)(c % NSTAGE) * CHUNK + j) * REC_LEN + q * 4, rec_img + (size_t)f * REC_LEN + q * 4);
     }
     cp_async_commit();
 }
@@ -618,7 +368,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
                                                        const float* __restrict__ textures,
                                                        float* __restrict__ images, float* __restrict__ colors_hi,
                                                        float* __restrict__ aggrs, float* __restrict__ p2f_acc,
-                                                       const uint32_t* __restrict__ ubox, Consts K, float eps,
+                                                       const uint32_t* __restrict__ ubox, Consts<float> K, float eps,
                                                        float bg0, float bg1, float bg2) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float* s_rec = reinterpret_cast<float*>(smem_raw);
@@ -670,7 +420,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
                                   s_warp_cnt, &s_bar, bar_phase);
     // (build_tile_list ends with __syncthreads: the list is visible)
     any = any || n > 0;
-    const float* rec_img = rec_all + ((size_t)b * F + wb) * REC_F;
+    const float* rec_img = rec_all + ((size_t)b * F + wb) * REC_LEN;
     const int nchunk = (n + CHUNK - 1) / CHUNK;
     if (nchunk > 0) {
         issue_chunk(rec_img, s_list, n, 0, s_rec);
@@ -681,18 +431,18 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
         const int cnt = min(CHUNK, n - c * CHUNK);
         cp_async_wait<1>();  // chunk c has landed (c+1 may still be in flight)
         __syncthreads();     // ... for every thread
-        const float* chunk = s_rec + (size_t)st * CHUNK * REC_F;
+        const float* chunk = s_rec + (size_t)st * CHUNK * REC_LEN;
         // p2f partial sums of this warp: lane j owns chunk face j (registers, no shared traffic)
         float own_x = 0.f, own_y = 0.f, own_w = 0.f;
         float4 bb = *reinterpret_cast<const float4*>(chunk + R_BOX);
         for (int j = 0; j < cnt; ++j) {
-            const float* rc = chunk + j * REC_F;
+            const float* rc = chunk + j * REC_LEN;
             // prefetch the next cull box while this face is evaluated
-            const float4 bbn = *reinterpret_cast<const float4*>(chunk + (j + 1 < cnt ? j + 1 : j) * REC_F + R_BOX);
+            const float4 bbn = *reinterpret_cast<const float4*>(chunk + (j + 1 < cnt ? j + 1 : j) * REC_LEN + R_BOX);
             float a_x = 0.f, a_y = 0.f, a_w = 0.f;
             bool contrib = false;
             if (live && !(xp > bb.y || xp < bb.x || yp > bb.w || yp < bb.z)) {
-                Frag fr;
+                Frag<float> fr;
                 if (fragment_any(rc, xp, yp, K, fr)) {
                     if (K.alpha == UMR_ALPHA_PROD) {
                         acc_a = (float)((double)acc_a * (1. - (double)fr.D));  // kernel.cu:396
@@ -804,7 +554,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_fwd(const float* __restrict__
         // thread issues float4 stores of 64-byte row segments instead of scattered 4-byte stores.
         cp_async_wait<0>();
         __syncthreads();
-        float* st = s_rec;  // 6 * 256 + 4 * 64 = 1792 floats <= NSTAGE * CHUNK * REC_F = 2048
+        float* st = s_rec;  // 6 * 256 + 4 * 64 = 1792 floats <= NSTAGE * CHUNK * REC_LEN = 2048
         const int o = (py - ty0) * TILE + (px - tx0);
         st[0 * 256 + o] = o0; st[1 * 256 + o] = o1; st[2 * 256 + o] = o2; st[3 * 256 + o] = alpha;
         st[4 * 256 + o] = g0; st[5 * 256 + o] = g1;
@@ -873,98 +623,6 @@ __global__ void k_p2f_finalize(const float* __restrict__ acc, float* __restrict_
 // =============================================================================================
 // backward
 // =============================================================================================
-// One (pixel, face) pair of the generic-mode backward for the deterministic gather (k_raster_bwd_det<..., GEN>): the
-// per-pair body of k_raster_bwd (kernel.cu:577-654) statement for statement, with the texture gradient going to `sink`;
-// writes the 9 vertex gradients to gv (zeroed by the caller) and sets `contrib` for a pair inside the depth range.
-// k_raster_bwd keeps its inline copy: calling this function from it changes that kernel's SASS (its scheduling), and the
-// default kernels stay bit-for-bit what they were.  The GPU tests hold both to oracle B.
-// face_of() yields the face index (read where k_raster_bwd always read it: only for pairs inside the depth range).
-template <int RGB, bool TEXGRAD, class Sink = TexRedSink, class FaceOf>
-__device__ __forceinline__ void bwd_pair_generic(const float* __restrict__ rc, float xp, float yp, const Consts& K, FaceOf face_of,
-                                                 float g0, float g1, float g2, float g3, float C0, float C1, float C2,
-                                                 float C3, float ssum, float smax, const float* __restrict__ tex_img,
-                                                 float* __restrict__ gtex_img, float* gv, bool& contrib, Sink sink = Sink()) {
-    Frag fr;
-    if (fragment_any(rc, xp, yp, K, fr)) {
-        // alpha: kernel.cu:577-585 (hard alpha passes the raw gradient through, as the reference does)
-        const float one_m_a = 1 - C3;
-        float Cxy;
-        if (K.alpha == UMR_ALPHA_PROD) {
-            Cxy = (one_m_a == 0.f || g3 == 0.f)
-                      ? g3 * one_m_a
-                      : (float)((double)g3 * ((double)one_m_a / fmax((double)(1 - fr.D), 1e-6)));
-        } else if (K.alpha == UMR_ALPHA_SUM) {
-            Cxy = g3 / K.F;
-        } else {
-            Cxy = g3;
-        }
-        float k0 = fr.w0, k1 = fr.w1, k2 = fr.w2;
-        clip_bary(k0, k1, k2);
-        const float zp = depth_of(rc, k0, k1, k2);
-        if (!(zp < K.near_ || zp > K.far_)) {  // :592 drops the alpha gradient as well
-            contrib = true;
-            const uint32_t flg = __float_as_uint(rc[R_FLG]);
-            const bool front = (flg & 8u) != 0;
-            const int f = face_of();
-            float gz0 = 0.f, gz1 = 0.f, gz2 = 0.f;
-            if (RGB == 0) {
-                if ((float)f == smax) {  // aggrs[1] = winning face id (:596)
-                    if (TEXGRAD)
-                        add_texture_grad(gtex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, 1.f, g0, g1, g2, false, sink);
-                }
-            } else if ((front || K.double_side) && (g0 != 0.f || g1 != 0.f || g2 != 0.f)) {
-                const float zn = (K.far_ - zp) / (K.far_ - K.near_);
-                const float s = fr.D * expf((zn - smax) / K.gamma) / ssum;  // :608
-                if (s != 0.f) {
-                    if (TEXGRAD)
-                        add_texture_grad(gtex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, s, g0, g1, g2, true, sink);
-                    float t0, t1, t2;
-                    sample_texture(tex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, t0, t1, t2);
-                    float Crgb = 0.f;
-                    Crgb += g0 * (t0 - C0);
-                    Crgb += g1 * (t1 - C1);
-                    Crgb += g2 * (t2 - C2);
-                    Crgb *= s;
-                    if (Crgb != 0.f) {
-                        Cxy += Crgb / fr.D;
-                        const float Cz = Crgb / K.gamma / (K.near_ - K.far_) * zp * zp;  // :624
-                        gz0 = Cz * k0 / rc[2] / rc[2];
-                        gz1 = Cz * k1 / rc[5] / rc[5];
-                        gz2 = Cz * k2 / rc[8] / rc[8];
-                    }
-                }
-            }
-            Cxy *= fr.D * (1 - fr.D) / K.sigma;  // :632
-            gv[2] = gz0; gv[5] = gz1; gv[8] = gz2;
-            if (K.dist == UMR_DIST_EUCLIDEAN) {
-                const float q = 2 * fr.sign * Cxy;  // :640
-                gv[0] = q * (fr.t0 + fr.w0) * fr.dx;
-                gv[1] = q * (fr.t0 + fr.w0) * fr.dy;
-                gv[3] = q * (fr.t1 + fr.w1) * fr.dx;
-                gv[4] = q * (fr.t1 + fr.w1) * fr.dy;
-                gv[6] = q * (fr.t2 + fr.w2) * fr.dx;
-                gv[7] = q * (fr.t2 + fr.w2) * fr.dy;
-            } else if (K.dist == UMR_DIST_BARYCENTRIC) {  // kernel.cu:162-176
-                const float w0 = fr.t0, w1 = fr.t1, w2 = fr.t2;  // unclipped barycentrics
-                const int pidx = w0 > w1 ? (w1 > w2 ? 2 : 1) : (w0 > w2 ? 2 : 0);
-                const double scale = fr.dis > 0 ? (2. * (double)sqrtf(fr.dis)) : (2. * (double)sqrtf(-fr.dis));
-#pragma unroll
-                for (int l = 0; l < 2; ++l) {
-                    const float ip = rc[R_INV + 3 * pidx + l];
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        float gkl = 0.f;
-                        gkl += -ip * rc[R_INV + 3 * k + 0] * xp;
-                        gkl += -ip * rc[R_INV + 3 * k + 1] * yp;
-                        gkl += -ip * rc[R_INV + 3 * k + 2] * 1.f;
-                        gv[3 * k + l] = (float)((double)(gkl * Cxy) * scale);
-                    }
-                }
-            }
-        }
-    }
-}
-
 template <int RGB, bool TEXGRAD>
 __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__ rec_all,
                                                        const float4* __restrict__ box_all,
@@ -973,7 +631,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
                                                        const float* __restrict__ aggrs,
                                                        const float* __restrict__ grad_images,
                                                        float* __restrict__ grad_faces, float* __restrict__ grad_tex,
-                                                       const uint32_t* __restrict__ ubox, Consts K) {
+                                                       const uint32_t* __restrict__ ubox, Consts<float> K) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float* s_rec = reinterpret_cast<float*>(smem_raw);
     float4* s_box = reinterpret_cast<float4*>(smem_raw + smem_box_off());
@@ -1009,7 +667,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
     const int n = build_tile_list(box + wb, min(F - wb, FACE_WINDOW), s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, s_list,
                                   s_warp_cnt, &s_bar, bar_phase);
     if (n == 0) continue;  // uniform
-    const float* rec_img = rec_all + ((size_t)b * F + wb) * REC_F;
+    const float* rec_img = rec_all + ((size_t)b * F + wb) * REC_LEN;
 
     const int nchunk = (n + CHUNK - 1) / CHUNK;
     issue_chunk(rec_img, s_list, n, 0, s_rec);
@@ -1046,21 +704,21 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
         const int cnt = min(CHUNK, n - c * CHUNK);
         cp_async_wait<1>();
         __syncthreads();  // chunk c visible to all; s_g is zero again
-        const float* chunk = s_rec + (size_t)st * CHUNK * REC_F;
+        const float* chunk = s_rec + (size_t)st * CHUNK * REC_LEN;
         float own[9];  // vertex-gradient partial sums of this warp: lane j owns chunk face j
 #pragma unroll
         for (int k = 0; k < 9; ++k) own[k] = 0.f;
         bool own_any = false;
         float4 bb = *reinterpret_cast<const float4*>(chunk + R_BOX);
         for (int j = 0; j < cnt; ++j) {
-            const float* rc = chunk + j * REC_F;
-            const float4 bbn = *reinterpret_cast<const float4*>(chunk + (j + 1 < cnt ? j + 1 : j) * REC_F + R_BOX);
+            const float* rc = chunk + j * REC_LEN;
+            const float4 bbn = *reinterpret_cast<const float4*>(chunk + (j + 1 < cnt ? j + 1 : j) * REC_LEN + R_BOX);
             float gv[9];
 #pragma unroll
             for (int k = 0; k < 9; ++k) gv[k] = 0.f;
             bool contrib = false;
             if (live && !(xp > bb.y || xp < bb.x || yp > bb.w || yp < bb.z)) {
-                Frag fr;
+                Frag<float> fr;
                 if (fragment_any(rc, xp, yp, K, fr)) {
                     // alpha: kernel.cu:577-585 (hard alpha passes the raw gradient through, as the reference does)
                     const float one_m_a = 1 - C3;
@@ -1086,14 +744,14 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
                         if (RGB == 0) {
                             if ((float)f == smax) {  // aggrs[1] = winning face id (:596)
                                 if (TEXGRAD)
-                                    add_texture_grad(gtex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, 1.f, g0, g1, g2, false);
+                                    add_texture_grad(gtex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, 1.f, g0, g1, g2, false, TexRedSink());
                             }
                         } else if ((front || K.double_side) && (g0 != 0.f || g1 != 0.f || g2 != 0.f)) {
                             const float zn = (K.far_ - zp) / (K.far_ - K.near_);
                             const float s = fr.D * expf((zn - smax) / K.gamma) / ssum;  // :608
                             if (s != 0.f) {
                                 if (TEXGRAD)
-                                    add_texture_grad(gtex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, s, g0, g1, g2, true);
+                                    add_texture_grad(gtex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, s, g0, g1, g2, true, TexRedSink());
                                 float t0, t1, t2;
                                 sample_texture(tex_img + (size_t)f * K.T2 * 3, k0, k1, k2, K, t0, t1, t2);
                                 float Crgb = 0.f;
@@ -1185,90 +843,18 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
 // CTA carry the same load, and the 9 vertex gradients are combined by a segmented warp reduction (lanes
 // are sorted by face) followed by one shared atomic per (warp, face, component).
 // =============================================================================================
-template <int RGB, bool TEXGRAD>
-__device__ __forceinline__ bool bwd_pair(const float* __restrict__ rc, float xp, float yp, const Consts& K, float g0,
-                                         float g1, float g2, float g3, float C0, float C1, float C2, float C3,
-                                         float ssum, float smax, int f, const float* __restrict__ tex_img,
-                                         float* __restrict__ gtex_img, float* gv) {
-    Frag fr;
-    if (!fragment(rc, xp, yp, K.thr, K.sigma, fr)) return false;
-    // alpha (prod): kernel.cu:577-585
-    // g3 * ((1 - alpha) / max(1 - D, 1e-6)) in double (:584).  Interior pixels have alpha == 1: the quotient is
-    // then exactly 0 and the double division would take its (very long) special-operand path, so the zero
-    // cases are answered directly: x * 0 == 0 with the same sign rules.
-    const float one_m_a = 1 - C3;
-    float Cxy = (one_m_a == 0.f || g3 == 0.f)
-                    ? g3 * one_m_a
-                    : (float)((double)g3 * ((double)one_m_a / fmax((double)(1 - fr.D), 1e-6)));
-    float k0 = fr.w0, k1 = fr.w1, k2 = fr.w2;
-    clip_bary(k0, k1, k2);
-    const float zp = depth_of(rc, k0, k1, k2);
-    if (zp < K.near_ || zp > K.far_) return false;  // :592 drops the alpha gradient as well
-    const uint32_t flg = __float_as_uint(rc[R_FLG]);
-    const bool front = (flg & 8u) != 0;
-    float gz0 = 0.f, gz1 = 0.f, gz2 = 0.f;
-    if (RGB == 0) {
-        if ((float)f == smax) {  // aggrs[1] = winning face id (:596)
-            if (TEXGRAD) {
-                float* gt = gtex_img + ((size_t)f * K.T2 + texel_index(k0, k1, K.R)) * 3;
-                red_add_global(gt + 0, g0);
-                red_add_global(gt + 1, g1);
-                red_add_global(gt + 2, g2);
-            }
-        }
-    } else if ((front || K.double_side) && (g0 != 0.f || g1 != 0.f || g2 != 0.f)) {
-        // (no colour gradient at this pixel, e.g. silhouette-only losses: every term below is exactly 0)
-        const float zn = (K.far_ - zp) / (K.far_ - K.near_);
-        const float s = fr.D * expf((zn - smax) / K.gamma) / ssum;  // :608
-        // s == 0 (softmax weight of an occluded face underflowed): texture gradient, C_rgb and the z
-        // gradients are all exactly 0 -- skipping them also avoids ~9 IEEE divisions with zero numerators,
-        // each of which would take the division's slow special-operand path.
-        if (s != 0.f) {
-            const size_t to = ((size_t)f * K.T2 + texel_index(k0, k1, K.R)) * 3;
-            if (TEXGRAD) {
-                red_add_global(gtex_img + to + 0, s * g0);
-                red_add_global(gtex_img + to + 1, s * g1);
-                red_add_global(gtex_img + to + 2, s * g2);
-            }
-            float Crgb = 0.f;
-            Crgb += g0 * (__ldg(tex_img + to + 0) - C0);
-            Crgb += g1 * (__ldg(tex_img + to + 1) - C1);
-            Crgb += g2 * (__ldg(tex_img + to + 2) - C2);
-            Crgb *= s;
-            if (Crgb != 0.f) {
-                Cxy += Crgb / fr.D;
-                const float Cz = Crgb / K.gamma / (K.near_ - K.far_) * zp * zp;  // :624
-                gz0 = Cz * k0 / rc[2] / rc[2];
-                gz1 = Cz * k1 / rc[5] / rc[5];
-                gz2 = Cz * k2 / rc[8] / rc[8];
-            }
-        }
-    }
-    Cxy *= fr.D * (1 - fr.D) / K.sigma;  // :632
-    const float q = 2 * fr.sign * Cxy;      // :640
-    gv[0] = q * (fr.t0 + fr.w0) * fr.dx;
-    gv[1] = q * (fr.t0 + fr.w0) * fr.dy;
-    gv[2] = gz0;
-    gv[3] = q * (fr.t1 + fr.w1) * fr.dx;
-    gv[4] = q * (fr.t1 + fr.w1) * fr.dy;
-    gv[5] = gz1;
-    gv[6] = q * (fr.t2 + fr.w2) * fr.dx;
-    gv[7] = q * (fr.t2 + fr.w2) * fr.dy;
-    gv[8] = gz2;
-    return true;
-}
-
 // Register-lean variant used by the pair-parallel kernel: the 10 per-pixel inputs stay in shared memory
 // (sp = &s_pix[0][pix], plane stride PT*PT) and are fetched where they are consumed, and the 9 gradients are
 // added straight into the caller's accumulators -- this keeps the kernel at <= 64 registers (4 CTAs/SM).
 // SPLIT (the split backward, softmax only): the vertex gradients keep only the terms driven by the alpha adjoint g3; the texel
 // gradients are formed from the colour adjoints as always.  Skipping the colour terms leaves every other expression as it is,
 // so the vertex gradients equal, bit for bit, those of the same pairs with zero colour adjoints.
-template <int RGB, bool TEXGRAD, int NC = 3, class Sink = TexRedSink, bool SPLIT = false>
-__device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float xp, float yp, const Consts& K,
+// (Declared with its default arguments in raster_generic.cuh, for the deterministic gather.)
+template <int RGB, bool TEXGRAD, int NC, class Sink, bool SPLIT>
+__device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float xp, float yp, const Consts<float>& K,
                                              const float* __restrict__ sp, int f, const float* __restrict__ tex_img,
-                                             float* __restrict__ gtex_img, float* acc, Sink sink = Sink()) {
-    Frag fr;
+                                             float* __restrict__ gtex_img, float* acc, Sink sink) {
+    Frag<float> fr;
     if (!fragment(rc, xp, yp, K.thr, K.sigma, fr)) return false;
     constexpr int NP = PT * PT, NPL = NC + 1, NV = 2 * NPL + 2;  // planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
     const float g3 = sp[NC * NP];
@@ -1346,7 +932,7 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
                                                const float* __restrict__ textures, const float* __restrict__ colors_hi,
                                                const float* __restrict__ aggrs, const float* __restrict__ grad_images,
                                                float* __restrict__ grad_faces, float* __restrict__ grad_tex,
-                                               const uint32_t* __restrict__ ubox, const Consts& K, int bx, int by, int b,
+                                               const uint32_t* __restrict__ ubox, const Consts<float>& K, int bx, int by, int b,
                                                uint64_t* s_bar_p, uint32_t& bar_phase) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float* s_rec = reinterpret_cast<float*>(smem_raw);
@@ -1380,7 +966,7 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
     const int n = build_tile_list(box + wb, min(F - wb, FACE_WINDOW), s_ext[0], s_ext[1], s_ext[2], s_ext[3], s_box, s_list,
                                   s_warp_cnt, &s_bar, bar_phase);
     if (n == 0) continue;  // uniform
-    const float* rec_img = rec_all + ((size_t)b * F + wb) * REC_F;
+    const float* rec_img = rec_all + ((size_t)b * F + wb) * REC_LEN;
 
     const int nchunk = (n + CHUNK - 1) / CHUNK;
     issue_chunk(rec_img, s_list, n, 0, s_rec);
@@ -1421,12 +1007,12 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
         if (tid < CHUNK) { s_cm[tid] = 0u; s_rm[tid] = 0u; }
         cp_async_wait<1>();
         __syncthreads();  // chunk c (and s_pix on the first pass) visible; masks zeroed; s_g zero
-        const float* chunk = s_rec + (size_t)st * CHUNK * REC_F;
+        const float* chunk = s_rec + (size_t)st * CHUNK * REC_LEN;
         // ---- rectangles: thread (j = tid & 31, part = tid >> 5) tests 4 columns or 4 rows of face j
         {
             const int j = tid & 31, part = tid >> 5;
             if (j < cnt) {
-                const float4 bb = *reinterpret_cast<const float4*>(chunk + j * REC_F + R_BOX);
+                const float4 bb = *reinterpret_cast<const float4*>(chunk + j * REC_LEN + R_BOX);
                 unsigned m = 0;
                 constexpr int PER = PT / 4;  // columns (or rows) tested per thread
                 if (part < 4) {
@@ -1491,7 +1077,7 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
                 const uint32_t geo = s_geo[j];
                 const int cx0 = (int)(geo & 0xff), w = (int)((geo >> 8) & 0xff), ry0 = (int)(geo >> 16);
                 const uint32_t rcpw = s_rcpw[j];
-                const float* rc = chunk + j * REC_F;
+                const float* rc = chunk + j * REC_LEN;
                 const int f = wb + (int)s_list[c * CHUNK + j];
                 float acc[9];
 #pragma unroll
@@ -1534,7 +1120,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd_pairs(const float* __rest
                                                              const float* __restrict__ textures, const float* __restrict__ colors_hi,
                                                              const float* __restrict__ aggrs, const float* __restrict__ grad_images,
                                                              float* __restrict__ grad_faces, float* __restrict__ grad_tex,
-                                                             const uint32_t* __restrict__ ubox, Consts K) {
+                                                             const uint32_t* __restrict__ ubox, Consts<float> K) {
     __shared__ uint64_t s_bar;
     if (threadIdx.x == 0) {
         mbar_init(&s_bar, 1);
@@ -1553,7 +1139,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd_pairs_list(const float* _
                                                                   const float* __restrict__ textures, const float* __restrict__ colors_hi,
                                                                   const float* __restrict__ aggrs, const float* __restrict__ grad_images,
                                                                   float* __restrict__ grad_faces, float* __restrict__ grad_tex,
-                                                                  const uint32_t* __restrict__ ubox, Consts K,
+                                                                  const uint32_t* __restrict__ ubox, Consts<float> K,
                                                                   const uint32_t* __restrict__ ucount, const int32_t* __restrict__ ulist,
                                                                   int tiles_x, int tiles_y) {
     const uint32_t nu = __ldg(ucount);
@@ -1596,135 +1182,6 @@ __global__ void k_p2f_finalize_det(const unsigned long long* __restrict__ acc, f
     reinterpret_cast<float2*>(p2f)[i] = make_float2(x / d, y / d);
 }
 
-// Conservative index range [i0, i1] of the pixels whose centre coordinate pixel_coord(i, S) lies in [lo, hi] (monotone in i;
-// one index of slack on each side, the exact test runs per pixel).  NaN bounds keep every index, as the tile tests do.
-__device__ __forceinline__ void det_span(float lo, float hi, int S, int& i0, int& i1) {
-    const double a = ((double)lo * S + (S - 1)) * 0.5, c = ((double)hi * S + (S - 1)) * 0.5;
-    i0 = a > 0.0 ? (a < (double)S ? (int)a - 1 : S) : 0;
-    i1 = c < (double)(S - 1) ? (c > -1.0 ? (int)c + 1 : -1) : S - 1;  // c in (-1, 0): pixel 0 may still lie in the box
-    i0 = max(i0, 0);
-    i1 = min(i1, S - 1);
-}
-
-// Face-parallel backward without atomics.  A (pixel, face) pair's gradient depends only on per-pixel constants and the face
-// record, so every output gets exactly one writer: one warp owns a (texture group, face) pair and walks the group's images in
-// ascending order and, in each, the face's cull box row by row (lanes across a row segment of 32 pixels), evaluating each pair
-// with bwd_pair_acc -- the recompute backward's arithmetic.  Vertex gradients: a fixed shuffle tree, one plain store per image.
-// Texel gradients: lanes that hit the same texel are summed in ascending lane order, and the lowest of them adds the sum into the
-// warp-owned texels of the face (plain load / store; __syncwarp orders the steps).  GEN: the generic modes (distance, alpha
-// and texture mode read at run time), evaluated with bwd_pair_generic -- k_raster_bwd's arithmetic; a vertex-texture pair adds
-// to the face's 9 corner colours, which the warp sums the same way.  SPLIT (UMR's configuration only): see bwd_pair_acc.
-constexpr int DET_WARPS = CTA / 32;
-template <int RGB, bool TEXGRAD, int NC = 3, bool GEN = false, bool SPLIT = false>
-__global__ void __launch_bounds__(CTA) k_raster_bwd_det(const float* __restrict__ rec_all, const float* __restrict__ textures,
-                                                        const float* __restrict__ colors_hi, const float* __restrict__ aggrs,
-                                                        const float* __restrict__ grad_images, float* __restrict__ grad_faces,
-                                                        float* __restrict__ grad_tex, Consts K) {
-    constexpr int NPL = NC + 1, NV = 2 * NPL + 2, NP = PT * PT;
-    static_assert(NP == CTA, "bwd_pair_acc reads the per-pixel planes with stride PT * PT: one slot per thread");
-    __shared__ float s_pix[NV][NP];
-    __shared__ __align__(16) float s_rc[DET_WARPS][REC_F];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int f = blockIdx.x * DET_WARPS + warp;
-    if (f >= K.F) return;  // warp-uniform; the warps share no memory
-    const int grp = blockIdx.y, S = K.S, F = K.F;
-    const float* tex_img = textures + (size_t)grp * K.tex_bs;
-    float* gtex_img = TEXGRAD ? grad_tex + (size_t)grp * K.tex_bs : nullptr;
-    float* sp = &s_pix[0][threadIdx.x];
-    const float* rc = s_rc[warp];
-    const size_t np = (size_t)S * S;
-    for (int i = 0; i < K.tex_div; ++i) {
-        const int b = grp * K.tex_div + i;
-        __syncwarp();
-        s_rc[warp][lane] = __ldg(rec_all + ((size_t)b * F + f) * REC_F + lane);
-        __syncwarp();
-        const float4 bb = *reinterpret_cast<const float4*>(rc + R_BOX);
-        int c0, c1, j0, j1;
-        det_span(bb.x, bb.y, S, c0, c1);
-        det_span(bb.z, bb.w, S, j0, j1);  // j = S - 1 - row
-        float acc[9];
-#pragma unroll
-        for (int k = 0; k < 9; ++k) acc[k] = 0.f;
-        for (int py = S - 1 - j1; py <= S - 1 - j0; ++py) {
-            const float yp = pixel_coord(S - 1 - py, S);
-            if (yp > bb.w || yp < bb.z) continue;  // uniform
-            for (int x0 = c0; x0 <= c1; x0 += 32) {
-                const int px = x0 + lane;
-                const float xp = pixel_coord(px, S);
-                float* taddr = nullptr;
-                float tval[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                if (px <= c1 && !(xp > bb.y || xp < bb.x)) {
-                    const size_t p = (size_t)py * S + px;
-                    if (K.aa) {  // avg_pool2d backward: g / 4
-                        const size_t nq = (size_t)K.IS * K.IS;
-                        const size_t q = (size_t)(py >> 1) * K.IS + (px >> 1);
-#pragma unroll
-                        for (int k = 0; k < NPL; ++k) sp[k * NP] = __ldg(grad_images + ((size_t)b * NPL + k) * nq + q) * 0.25f;
-                    } else {
-#pragma unroll
-                        for (int k = 0; k < NPL; ++k) sp[k * NP] = __ldg(grad_images + ((size_t)b * NPL + k) * np + p);
-                    }
-#pragma unroll
-                    for (int k = 0; k < NPL; ++k) sp[(NPL + k) * NP] = __ldg(colors_hi + ((size_t)b * NPL + k) * np + p);
-                    sp[(NV - 2) * NP] = __ldg(aggrs + ((size_t)b * 2 + 0) * np + p);
-                    sp[(NV - 1) * NP] = __ldg(aggrs + ((size_t)b * 2 + 1) * np + p);
-                    if constexpr (GEN) {
-                        float gv[9];
-#pragma unroll
-                        for (int k = 0; k < 9; ++k) gv[k] = 0.f;
-                        bool hit = false;
-                        bwd_pair_generic<RGB, TEXGRAD, TexTakeSink>(rc, xp, yp, K, [=] { return f; }, sp[0], sp[NP], sp[2 * NP], sp[3 * NP],
-                                                                    sp[4 * NP], sp[5 * NP], sp[6 * NP], sp[7 * NP], sp[8 * NP],
-                                                                    sp[9 * NP], tex_img, gtex_img, gv, hit, TexTakeSink{&taddr, tval});
-                        if (hit) {
-#pragma unroll
-                            for (int k = 0; k < 9; ++k) acc[k] += gv[k];
-                        }
-                    } else {
-                        bwd_pair_acc<RGB, TEXGRAD, NC, TexTakeSink, SPLIT>(rc, xp, yp, K, sp, f, tex_img, gtex_img, acc,
-                                                                            TexTakeSink{&taddr, tval});
-                    }
-                }
-                if (TEXGRAD) {
-                    const bool has = taddr != nullptr;
-                    uint32_t rem = __ballot_sync(0xffffffffu, has);
-                    if (rem) {  // uniform
-                        const uint32_t peers = __match_any_sync(0xffffffffu, (unsigned long long)(uintptr_t)taddr);
-                        const bool vtx = GEN && K.tex != UMR_TEX_SURFACE;  // 9 corner-colour values instead of 3 texel channels
-                        float sum[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                        while (rem) {  // ascending lane order
-                            const int o = __ffs(rem) - 1;
-                            rem &= rem - 1u;
-                            const bool mine = (peers >> o) & 1u;
-#pragma unroll
-                            for (int k = 0; k < 9; ++k) {
-                                if (k < 3 || vtx) {
-                                    const float v = __shfl_sync(0xffffffffu, tval[k], o);
-                                    if (mine) sum[k] += v;
-                                }
-                            }
-                        }
-                        if (has && lane == __ffs(peers) - 1) {
-#pragma unroll
-                            for (int k = 0; k < 9; ++k)
-                                if (k < 3 || vtx) taddr[k] = taddr[k] + sum[k];
-                        }
-                        __syncwarp();
-                    }
-                }
-            }
-        }
-#pragma unroll
-        for (int k = 0; k < 9; ++k) acc[k] = warp_sum(acc[k]);
-        if (grad_faces != nullptr && lane < 9) {
-            float v = acc[0];
-#pragma unroll
-            for (int k = 1; k < 9; ++k) v = (lane == k) ? acc[k] : v;
-            grad_faces[((size_t)b * F + f) * 9 + lane] = v;
-        }
-    }
-}
-
 }  // namespace umr
 
 #include "raster_stream.cuh"
@@ -1741,7 +1198,7 @@ using namespace umr;
 template <int RGBM, bool TG, int TS, typename IdxT, bool SP = false>
 static void launch_bwd2(dim3 grid, cudaStream_t stream, bool pre, const float* rec, const float* textures, const float* soft_colors,
                         const float* aggrs_info, const float* grad_images, float* grad_faces, float* grad_textures,
-                        const Consts& K, const PairBuf& pb) {
+                        const Consts<float>& K, const PairBuf& pb) {
 #define UMR_BWD2_GO(GEOMV, PREV) \
     k_raster_bwd2<RGBM, TG, TS, 3, GEOMV, PREV, IdxT, SP><<<grid, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, \
                                                                                         grad_images, grad_faces, grad_textures, K, pb)
@@ -1838,8 +1295,8 @@ static bool is_generic(const UmrRasterParams* p) {
            p->texture_sample_type != UMR_TEX_SURFACE;
 }
 
-static Consts make_consts(const UmrRasterParams* p) {
-    Consts K;
+static Consts<float> make_consts(const UmrRasterParams* p) {
+    Consts<float> K;
     K.thr = p->dist_eps * p->sigma_val;  // kernel.cu:333 (float * float)
     K.sigma = p->sigma_val;
     K.gamma = p->gamma_val;
@@ -1961,7 +1418,7 @@ static int raster_forward(const float* face_vertices, const float* textures, flo
     rc = ensure_smem_attrs();
     if (rc) return rc;
     const int B = p->batch_size, F = p->num_faces;
-    Consts K = make_consts(p);
+    Consts<float> K = make_consts(p);
     if (!K.aa && soft_colors == nullptr) soft_colors = images;
     K.vec_store = (K.aa && (K.S % 8) == 0 && (((uintptr_t)images | (uintptr_t)soft_colors | (uintptr_t)aggrs_info) & 15) == 0) ? 1 : 0;
     const WorkspaceLayout L = ws_layout(B, F, K.S);
@@ -2083,7 +1540,7 @@ extern "C" int umr_raster_visibility(const float* face_vertices, float* aggrs_in
     rc = ensure_smem_attrs();
     if (rc) return rc;
     const int B = p->batch_size, F = p->num_faces;
-    Consts K = make_consts(p);
+    Consts<float> K = make_consts(p);
     K.vec_store = (K.aa && (K.S % 8) == 0 && ((uintptr_t)aggrs_info & 15) == 0) ? 1 : 0;
     const WorkspaceLayout L = ws_layout(B, F, K.S);
     char* ws = (char*)workspace;
@@ -2138,7 +1595,7 @@ static int raster_backward(const float* face_vertices, const float* textures, co
     int rc = ensure_smem_attrs();
     if (rc) return rc;
     const int B = p->batch_size, F = p->num_faces;
-    const Consts K = make_consts(p);
+    const Consts<float> K = make_consts(p);
     const WorkspaceLayout L = ws_layout(B, F, K.S);
     char* ws = (char*)workspace;
     float* rec = (float*)(ws + L.rec_off);
@@ -2278,7 +1735,7 @@ static int raster_backward_det(const float* face_vertices, const float* textures
     if (nc4 && grad_textures) return UMR_ERR_UNSUPPORTED;  // part maps are constants (loss_utils.py:367-381)
     cudaStream_t stream = (cudaStream_t)stream_;
     const int B = p->batch_size, F = p->num_faces;
-    const Consts K = make_consts(p);
+    const Consts<float> K = make_consts(p);
     const WorkspaceLayout L = ws_layout(B, F, K.S);
     char* ws = (char*)workspace;
     float* rec = (float*)(ws + L.rec_off);
@@ -2292,21 +1749,22 @@ static int raster_backward_det(const float* face_vertices, const float* textures
         e = cudaMemsetAsync(grad_textures, 0, (n / K.tex_div) * p->texture_size * 3 * sizeof(float), stream);
         if (e != cudaSuccess) return (int)e;
     }
-    const dim3 grid((unsigned)((F + DET_WARPS - 1) / DET_WARPS), (unsigned)(B / K.tex_div));
+    const dim3 grid((unsigned)((F + NWARP - 1) / NWARP), (unsigned)(B / K.tex_div));
     const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
     if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
 #define UMR_BWD_DET(RGBM, TG, NCH)                                                                                        \
     do {                                                                                                                    \
-        if (gen) k_raster_bwd_det<RGBM, TG, NCH, true><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info,     \
+        if (gen) k_raster_bwd_det<float, RGBM, TG, NCH, true><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors,        \
+                                                                                      aggrs_info, grad_images, grad_faces, \
+                                                                                      grad_textures, K);                   \
+        else k_raster_bwd_det<float, RGBM, TG, NCH><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info,         \
                                                                                grad_images, grad_faces, grad_textures, K); \
-        else k_raster_bwd_det<RGBM, TG, NCH><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images,  \
-                                                                        grad_faces, grad_textures, K);                     \
     } while (0)
-    if (nc4) k_raster_bwd_det<1, false, 4><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images,
-                                                                      grad_faces, grad_textures, K);
-    else if (split && softmax) k_raster_bwd_det<1, true, 3, false, true><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors,
-                                                                                                   aggrs_info, grad_images,
-                                                                                                   grad_faces, grad_textures, K);
+    if (nc4) k_raster_bwd_det<float, 1, false, 4><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images,
+                                                                             grad_faces, grad_textures, K);
+    else if (split && softmax) k_raster_bwd_det<float, 1, true, 3, false, true><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors,
+                                                                                                          aggrs_info, grad_images,
+                                                                                                          grad_faces, grad_textures, K);
     else if (softmax) { if (grad_textures) UMR_BWD_DET(1, true, 3); else UMR_BWD_DET(1, false, 3); }
     else { if (grad_textures) UMR_BWD_DET(0, true, 3); else UMR_BWD_DET(0, false, 3); }  // hard: split == full
 #undef UMR_BWD_DET

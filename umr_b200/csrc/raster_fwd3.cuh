@@ -24,14 +24,14 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
                                                         const float* __restrict__ textures, float* __restrict__ images,
                                                         float* __restrict__ colors_hi, float* __restrict__ aggrs,
                                                         float* __restrict__ p2f_acc, const uint32_t* __restrict__ ubox,
-                                                        Consts K, float eps, float bg0, float bg1, float bg2, PairBuf pb,
+                                                        Consts<float> K, float eps, float bg0, float bg1, float bg2, PairBuf pb,
                                                         int ncb, float bg3 = 0.f,
                                                         uint8_t* __restrict__ vis_mask = nullptr) {  // RGB = 2: optional [B,F] "face is visible" bytes; aggrs may be NULL
     constexpr int NPL = NC + 1;                                      // image planes: colours + alpha
     constexpr bool VIS = RGB == 2;
     const float bgc[4] = {bg0, bg1, bg2, bg3};
     constexpr int WG = 16;                                           // list entries per warp group
-    __shared__ __align__(128) float s_wrec[NWARP * 2 * WG * REC_F];  // 32 KB: warp-private record stages; reused by the store epilogue
+    __shared__ __align__(128) float s_wrec[NWARP * 2 * WG * REC_LEN];  // 32 KB: warp-private record stages; reused by the store epilogue
     float* s_rec = s_wrec;
     __shared__ IdxT s_list[LCAP];
     __shared__ uint8_t s_meet[LCAP];          // bit w: the face's cull rectangle meets warp w's 8x4 pixel block
@@ -152,7 +152,7 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
     const float xp = s_xp[lcol], yp = s_yp[lrow];
     const int ncol = min(TILE, S - tx0), nrow = min(TILE, S - ty0);
     const float4* box = box_all + (size_t)b * F;
-    const float* rec_img = rec_all + (size_t)b * F * REC_F;
+    const float* rec_img = rec_all + (size_t)b * F * REC_LEN;
     const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
     const float ext0 = s_ext[0], ext1 = s_ext[1], ext2 = s_ext[2], ext3 = s_ext[3];
 
@@ -288,7 +288,7 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
         // entries, stages the records of the faces that meet ITS pixel block into a warp-private double buffer
         // (cp.async, 8 lanes x 16 B per record) and aggregates them in ascending face order.  Warps over empty parts of
         // the tile finish early instead of waiting at chunk barriers (30 % of the stall samples of the barrier version).
-        float* wst = s_wrec + warp * (2 * WG * REC_F);
+        float* wst = s_wrec + warp * (2 * WG * REC_LEN);
         const int ngroup = (n + WG - 1) / WG;
         auto issue = [&](int g) -> uint32_t {
             uint32_t m = 0;
@@ -303,7 +303,7 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
                 for (int r = lane >> 3; r < cntm; r += 4) {
                     const int e = s_pos[warp][r];  // list offset of the r-th face this warp needs
                     const int f = s_list[base + e];
-                    cp_async16(wst + ((size_t)(g & 1) * WG + r) * REC_F + (lane & 7) * 4, rec_img + (size_t)f * REC_F + (lane & 7) * 4);
+                    cp_async16(wst + ((size_t)(g & 1) * WG + r) * REC_LEN + (lane & 7) * 4, rec_img + (size_t)f * REC_LEN + (lane & 7) * 4);
                 }
             }
             __syncwarp();  // table reads done before the next issue() rewrites it
@@ -316,7 +316,7 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
             cp_async_wait<1>();  // group g has landed for this lane (g + 1 may still be in flight)
             __syncwarp();        // ... and for the other lanes of the warp
             const int base = g * WG;
-            const float* stage = wst + (size_t)(g & 1) * WG * REC_F;
+            const float* stage = wst + (size_t)(g & 1) * WG * REC_LEN;
             float own_x = 0.f, own_y = 0.f, own_w = 0.f;  // p2f partial sums: lane r owns the r-th staged face
             uint32_t mm = m_cur;
             for (int r = 0; mm; ++r) {
@@ -324,11 +324,11 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
                 mm &= mm - 1u;
                 const int jl = base + e;  // list position
                 const uint32_t meet = s_meet[jl];
-                const float* rc = stage + r * REC_F;
+                const float* rc = stage + r * REC_LEN;
                 const float4 bb = *reinterpret_cast<const float4*>(rc + R_BOX);
                 float a_x = 0.f, a_y = 0.f, a_w = 0.f;
                 bool contrib = false, emit = false;
-                Frag fr;
+                Frag<float> fr;
                 float k0 = 0.f, k1 = 0.f, k2 = 0.f, zsave = 0.f;
                 uint32_t tix = 0, front = 0;
                 if (VIS) {

@@ -32,7 +32,7 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
                                                         const float* __restrict__ textures, float* __restrict__ images,
                                                         float* __restrict__ colors_hi, float* __restrict__ aggrs,
                                                         float* __restrict__ p2f_acc, const uint32_t* __restrict__ ubox,
-                                                        Consts K, float eps, float bg0, float bg1, float bg2, PairBuf pb,
+                                                        Consts<float> K, float eps, float bg0, float bg1, float bg2, PairBuf pb,
                                                         int ncb) {
     extern __shared__ __align__(16) unsigned char smem_dyn[];
     const int F = K.F;
@@ -40,7 +40,7 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
     uint32_t* s_boff = reinterpret_cast<uint32_t*>(smem_dyn);                 // [LC + 1]
     uint32_t* s_meet = s_boff + (LC + 1);                                     // [LC]  bit q: rectangle meets pixel block q
     IdxT* s_list = reinterpret_cast<IdxT*>(s_meet + LC);                      // [LC]
-    __shared__ __align__(128) float s_wrec[NWARP * 2 * WG4 * REC_F];          // 32 KB: warp-private record stages
+    __shared__ __align__(128) float s_wrec[NWARP * 2 * WG4 * REC_LEN];          // 32 KB: warp-private record stages
     __shared__ float s_xp[T4], s_yp[T4], s_ext[4];
     __shared__ int s_warp_cnt[NWARP];
     __shared__ uint32_t s_warp_blk[NWARP];
@@ -141,7 +141,7 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
 
     const int ncol = min(T4, S - tx0), nrow = min(T4, S - ty0);
     const float4* box = box_all + (size_t)b * F;
-    const float* rec_img = rec_all + (size_t)b * F * REC_F;
+    const float* rec_img = rec_all + (size_t)b * F * REC_LEN;
     const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
     const float ext0 = s_ext[0], ext1 = s_ext[1], ext2 = s_ext[2], ext3 = s_ext[3];
     const uint32_t lt = (1u << lane) - 1u;
@@ -194,7 +194,7 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
         return n;
     };
     const bool slow = nc > LC;  // uniform: the bin's list does not fit the shared tile list -> windowed static path below
-    float* wst = s_wrec + warp * (2 * WG4 * REC_F);
+    float* wst = s_wrec + warp * (2 * WG4 * REC_LEN);
     // S = 1: torch 1.1's affine_grid takes linspace(-1, 1, 1) = [-1] (DESIGN.md §2), where 2 / 0 would give -1 + inf * 0 = NaN
     const float gstep = S > 1 ? 2.f / (float)(S - 1) : 0.f;
 
@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
                 for (int r = lane >> 3; r < cntm; r += 4) {
                     const int e = __fns(m, 0, r + 1);  // list offset of the r-th face this block needs
                     const int f = s_list[base + e];
-                    cp_async16(wst + ((size_t)(g & 1) * WG4 + r) * REC_F + (lane & 7) * 4, rec_img + (size_t)f * REC_F + (lane & 7) * 4);
+                    cp_async16(wst + ((size_t)(g & 1) * WG4 + r) * REC_LEN + (lane & 7) * 4, rec_img + (size_t)f * REC_LEN + (lane & 7) * 4);
                 }
             }
             cp_async_commit();
@@ -242,18 +242,18 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
             cp_async_wait<1>();  // group g has landed for this lane (g + 1 may still be in flight)
             __syncwarp();        // ... and for the other lanes of the warp
             const int base = g * WG4;
-            const float* stage = wst + (size_t)(g & 1) * WG4 * REC_F;
+            const float* stage = wst + (size_t)(g & 1) * WG4 * REC_LEN;
             float own_x = 0.f, own_y = 0.f, own_w = 0.f;  // p2f partial sums: lane r owns the r-th staged face
             uint32_t mm = m_cur;
             for (int r = 0; mm; ++r) {
                 const int e = __ffs(mm) - 1;
                 mm &= mm - 1u;
                 const int jl = base + e;  // list position
-                const float* rc = stage + r * REC_F;
+                const float* rc = stage + r * REC_LEN;
                 const float4 bb = *reinterpret_cast<const float4*>(rc + R_BOX);
                 float a_x = 0.f, a_y = 0.f, a_w = 0.f;
                 bool contrib = false, emit = false;
-                Frag fr;
+                Frag<float> fr;
                 float k0 = 0.f, k1 = 0.f, k2 = 0.f, zsave = 0.f;
                 uint32_t tix = 0, front = 0;
                 if (live && !(xp > bb.y || xp < bb.x || yp > bb.w || yp < bb.z)) {

@@ -148,7 +148,7 @@ __global__ void __launch_bounds__(CTA) k_bin_coarse(const float4* __restrict__ b
 // ---------------------------------------------------------------------------------------------
 template <typename IdxT>
 __global__ void __launch_bounds__(CTA) k_visible_faces(const float* __restrict__ rec_all, const IdxT* __restrict__ clist,
-                                                       const int* __restrict__ ccount, uint8_t* __restrict__ vis, Consts K) {
+                                                       const int* __restrict__ ccount, uint8_t* __restrict__ vis, Consts<float> K) {
     __shared__ unsigned long long s_z[CB * CB];   // 32 KB
     __shared__ float s_xp[CB], s_yp[CB];
     __shared__ int s_bg, s_next;
@@ -169,12 +169,12 @@ __global__ void __launch_bounds__(CTA) k_visible_faces(const float* __restrict__
     else if (tid < 2 * CB) s_yp[tid - CB] = pixel_coord(S - 1 - (y0 + tid - CB), S);
     if (tid == 0) { s_bg = 0; s_next = NWARP; }
     __syncthreads();
-    const float* rec_img = rec_all + (size_t)b * F * REC_F;
+    const float* rec_img = rec_all + (size_t)b * F * REC_LEN;
     auto scan_face = [&](int i) {
         const int f = bin_face(cb, i);
-        const float* rc = rec_img + (size_t)f * REC_F;
+        const float* rc = rec_img + (size_t)f * REC_LEN;
         if (lane == 0 && i + NWARP < nc)   // the warp's next face: pull its 128-byte record into L1 while this one is scanned
-            asm volatile("prefetch.global.L1 [%0];" ::"l"(rec_img + (size_t)bin_face(cb, i + NWARP) * REC_F));
+            asm volatile("prefetch.global.L1 [%0];" ::"l"(rec_img + (size_t)bin_face(cb, i + NWARP) * REC_LEN));
         const uint32_t flg = __float_as_uint(__ldg(rc + R_FLG));
         if (!(K.double_side || (flg & 8u))) return;   // back face of a single-sided render never wins (warp-uniform)
         // pixel rectangle to test: bounding box of the vertices widened by 2 pixels (an inside pixel lies in the box; the
@@ -212,7 +212,7 @@ __global__ void __launch_bounds__(CTA) k_visible_faces(const float* __restrict__
             if (!(w0 <= 1 && w0 >= 0 && w1 <= 1 && w1 >= 0 && w2 <= 1 && w2 >= 0)) continue;   // kernel.cu:404
             bool pass = w0 > 0 && w1 > 0 && w2 > 0 && w0 < 1 && w1 < 1 && w2 < 1;
             if (!pass) {  // a barycentric exactly 0 or 1: the reference's outside branch decides (kernel.cu:380-383)
-                Frag fr;
+                Frag<float> fr;
                 pass = fragment(rc, xp, yp, K.thr, K.sigma, fr);
             }
             if (!pass) continue;
@@ -282,7 +282,7 @@ template <int RGB, bool TEXGRAD, int TS, int NC = 3, bool GEOM = true, bool PRE 
 __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const float* __restrict__ rec_all, const float* __restrict__ textures,
                                                         const float* __restrict__ colors_hi,
                                                         const float* __restrict__ aggrs, const float* __restrict__ grad_images,
-                                                        float* __restrict__ grad_faces, float* __restrict__ grad_tex, Consts K,
+                                                        float* __restrict__ grad_faces, float* __restrict__ grad_tex, Consts<float> K,
                                                         PairBuf pb) {
     constexpr int NPL = NC + 1, NV = 2 * NPL + 2;
     __shared__ float s_pix[NV][TS * TS];  // g[NC], g_alpha, C[NC], alpha, ssum, smax (row-major tile pixels)
@@ -329,11 +329,11 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
     const float* tex_img = textures + (size_t)(b / K.tex_div) * K.tex_bs;
     float* gtex_img = TEXGRAD ? grad_tex + (size_t)(b / K.tex_div) * K.tex_bs : nullptr;
     float* gf_img = grad_faces + (size_t)b * F * 9;
-    const float* rec_img = ZGRAD ? rec_all + (size_t)b * F * REC_F : nullptr;
+    const float* rec_img = ZGRAD ? rec_all + (size_t)b * F * REC_LEN : nullptr;
     // the 128-byte face record of a step is pulled into L1 one step ahead: lanes 1-3 take the 32-byte sectors that hold
     // R_INV and R_IZ2
     auto prefetch_face = [&](int f) {
-        if (lane >= 1 && lane < 4) asm volatile("prefetch.global.L1 [%0];" ::"l"(rec_img + (size_t)f * REC_F + 8 * lane));
+        if (lane >= 1 && lane < 4) asm volatile("prefetch.global.L1 [%0];" ::"l"(rec_img + (size_t)f * REC_LEN + 8 * lane));
     };
 
     float acc[9];
@@ -503,7 +503,7 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
                                 const float Cz = Crgb * K.r_gamma * K.r_nf * zp * zp;  // :624
                                 // w_clip_k / z_k^2 (kernel.cu:624-627) exactly as the forward forms them: the w of
                                 // fragment(), clip_bary, times the face record's 1 / z_k^2
-                                const float* q = rec_img + (size_t)f * REC_F;
+                                const float* q = rec_img + (size_t)f * REC_LEN;
                                 const float xp = s_xp[pix % TS], yp = s_yp[pix / TS];
                                 float k0 = __ldg(q + R_INV + 0) * xp + __ldg(q + R_INV + 1) * yp + __ldg(q + R_INV + 2);
                                 float k1 = __ldg(q + R_INV + 3) * xp + __ldg(q + R_INV + 4) * yp + __ldg(q + R_INV + 5);
