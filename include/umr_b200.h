@@ -191,6 +191,33 @@ int umr_raster_backward_split_deterministic(const float* face_vertices, const fl
                                             float* grad_textures, const UmrRasterParams* params, void* workspace,
                                             void* stream);
 
+/* Silhouette render (DESIGN.md §12): the alpha plane of umr_raster_forward and nothing else -- no colour, no p2f, no
+ * aggregation planes.  alpha [B,is,is] is bitwise images[:, 3] of umr_raster_forward with the same params (any
+ * func_id_rgb, any textures: alpha depends on neither).  alpha_hi [B,S,S] receives the full-resolution alpha the backward
+ * reads; it may be NULL when no backward follows (anti_aliasing), and without anti_aliasing it may be alpha itself (NULL
+ * also means alpha).  The pair buffer of params is filled exactly as umr_raster_forward fills it (same pairs, same
+ * blocks), so one sizing serves both calls.  Workspace: umr_raster_workspace_bytes.
+ *
+ * The backward takes the gradient of alpha [B,is,is] and writes grad_faces [B,F,9]: the full backward's vertex gradient
+ * when only the alpha plane of grad_images is non-zero -- bitwise equal in the deterministic variant, the same per-pair
+ * expressions summed with float atomics in the default one.  Pairs outside (near, far) count in alpha and get no gradient,
+ * as in the full render.
+ *
+ * UMR's configuration only (euclidean / prod / surface, 3 colour channels; texture_size only has to be positive): the
+ * generic modes and color_channels = 4 return UMR_ERR_BAD_ARG, as do NULL and misaligned (not 4-byte aligned) buffers.
+ * There is no double-precision variant.  No host synchronisation; the calls can be captured in a CUDA graph. */
+int umr_raster_forward_silhouette(const float* face_vertices, float* alpha, float* alpha_hi, const UmrRasterParams* params,
+                                  void* workspace, void* stream);
+int umr_raster_backward_silhouette(const float* face_vertices, const float* alpha_hi, const float* grad_alpha,
+                                   float* grad_faces, const UmrRasterParams* params, void* workspace, void* stream);
+/* Deterministic twins (as umr_raster_forward_deterministic / umr_raster_backward_deterministic: 16x16 tiles, no pair
+ * buffer, the gather backward): bitwise reproducible.  Workspace: umr_raster_workspace_bytes (no p2f accumulators). */
+int umr_raster_forward_silhouette_deterministic(const float* face_vertices, float* alpha, float* alpha_hi,
+                                                const UmrRasterParams* params, void* workspace, void* stream);
+int umr_raster_backward_silhouette_deterministic(const float* face_vertices, const float* alpha_hi, const float* grad_alpha,
+                                                 float* grad_faces, const UmrRasterParams* params, void* workspace,
+                                                 void* stream);
+
 /* Double precision (DESIGN.md §9).  The arguments, outputs, validation and error codes of umr_raster_forward /
  * umr_raster_backward with every buffer in double: an operation-for-operation twin of the reference kernels' `scalar_t =
  * double` instantiation (every operation one IEEE binary64 rounding; the scalars of UmrRasterParams stay float, as in the

@@ -75,6 +75,16 @@ EXPORTS = {
                                                                ctypes.c_void_p]),
     "umr_raster_backward_split_deterministic": (ctypes.c_int, [c_f32p] * 7 + [ctypes.POINTER(UmrRasterParams), ctypes.c_void_p,
                                                                              ctypes.c_void_p]),
+    # silhouette render: alpha plane only (forward: face_vertices, alpha, alpha_hi; backward: face_vertices, alpha_hi,
+    # grad_alpha, grad_faces)
+    "umr_raster_forward_silhouette": (ctypes.c_int, [c_f32p] * 3 + [ctypes.POINTER(UmrRasterParams), ctypes.c_void_p,
+                                                                   ctypes.c_void_p]),
+    "umr_raster_forward_silhouette_deterministic": (ctypes.c_int, [c_f32p] * 3 + [ctypes.POINTER(UmrRasterParams),
+                                                                                 ctypes.c_void_p, ctypes.c_void_p]),
+    "umr_raster_backward_silhouette": (ctypes.c_int, [c_f32p] * 4 + [ctypes.POINTER(UmrRasterParams), ctypes.c_void_p,
+                                                                    ctypes.c_void_p]),
+    "umr_raster_backward_silhouette_deterministic": (ctypes.c_int, [c_f32p] * 4 + [ctypes.POINTER(UmrRasterParams),
+                                                                                  ctypes.c_void_p, ctypes.c_void_p]),
     # double-precision rasteriser: the arguments of umr_raster_forward / umr_raster_backward with double buffers
     "umr_raster_workspace_bytes_f64": (ctypes.c_size_t, [ctypes.c_int32] * 4),
     "umr_raster_forward_f64": (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.POINTER(UmrRasterParams), ctypes.c_void_p,

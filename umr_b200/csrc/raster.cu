@@ -849,6 +849,7 @@ __global__ void __launch_bounds__(CTA, 3) k_raster_bwd(const float* __restrict__
 // SPLIT (the split backward, softmax only): the vertex gradients keep only the terms driven by the alpha adjoint g3; the texel
 // gradients are formed from the colour adjoints as always.  Skipping the colour terms leaves every other expression as it is,
 // so the vertex gradients equal, bit for bit, those of the same pairs with zero colour adjoints.
+// RGB_SIL (the silhouette backward): the alpha terms alone, from the staged g_alpha and alpha planes (PixPlanes).
 // (Declared with its default arguments in raster_generic.cuh, for the deterministic gather.)
 template <int RGB, bool TEXGRAD, int NC, class Sink, bool SPLIT>
 __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float xp, float yp, const Consts<float>& K,
@@ -856,9 +857,10 @@ __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float
                                              float* __restrict__ gtex_img, float* acc, Sink sink) {
     Frag<float> fr;
     if (!fragment(rc, xp, yp, K.thr, K.sigma, fr)) return false;
-    constexpr int NP = PT * PT, NPL = NC + 1, NV = 2 * NPL + 2;  // planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
-    const float g3 = sp[NC * NP];
-    const float one_m_a = 1 - sp[(2 * NC + 1) * NP];
+    using PP = PixPlanes<RGB, NC>;
+    constexpr int NP = PT * PT, NPL = PP::NPL, NV = PP::NV;  // planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
+    const float g3 = sp[PP::GA * NP];
+    const float one_m_a = 1 - sp[PP::AL * NP];
     float Cxy = (one_m_a == 0.f || g3 == 0.f)
                     ? g3 * one_m_a
                     : (float)((double)g3 * ((double)one_m_a / fmax((double)(1 - fr.D), 1e-6)));
@@ -880,7 +882,7 @@ __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float
                 }
             }
         }
-    } else if (front || K.double_side) {
+    } else if (RGB == 1 && (front || K.double_side)) {
         float g[NC];
         bool any = false;
 #pragma unroll
@@ -941,8 +943,9 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
     __shared__ int s_warp_cnt[NWARP];
     __shared__ float s_ext[4];
     // PT x PT pixel tile (PT = 32 puts 4x the pairs in a chunk).
-    constexpr int NPL = NC + 1, NV = 2 * NPL + 2;
-    __shared__ float s_pix[NV][PT * PT];   // g[NC], g_alpha, C[NC], alpha, ssum, smax of the tile's pixels (row-major)
+    using PP = PixPlanes<RGB, NC>;
+    constexpr int NPL = PP::NPL, NV = PP::NV;
+    __shared__ float s_pix[NV][PT * PT];   // g[NC], g_alpha, C[NC], alpha, ssum, smax of the tile's pixels (row-major; PixPlanes)
     __shared__ float s_xp[PT], s_yp[PT];
     __shared__ unsigned int s_cm[CHUNK], s_rm[CHUNK];  // column / row pass masks of the chunk faces
     __shared__ int s_off[CHUNK + 1];                  // prefix sums of the rectangle sizes
@@ -979,7 +982,7 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
         const size_t np = (size_t)S * S;
         float v[NV];
 #pragma unroll
-        for (int k = 0; k < NV; ++k) v[k] = (k == NV - 2) ? 1.f : 0.f;
+        for (int k = 0; k < NV; ++k) v[k] = (!PP::SIL && k == NV - 2) ? 1.f : 0.f;
         if (px < S && py < S) {
             const size_t p = (size_t)py * S + px;
             if (K.aa) {  // avg_pool2d backward: g / 4
@@ -993,8 +996,10 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
             }
 #pragma unroll
             for (int k = 0; k < NPL; ++k) v[NPL + k] = __ldg(colors_hi + ((size_t)b * NPL + k) * np + p);
-            v[NV - 2] = __ldg(aggrs + ((size_t)b * 2 + 0) * np + p);
-            v[NV - 1] = __ldg(aggrs + ((size_t)b * 2 + 1) * np + p);
+            if (!PP::SIL) {
+                v[NV - 2] = __ldg(aggrs + ((size_t)b * 2 + 0) * np + p);
+                v[NV - 1] = __ldg(aggrs + ((size_t)b * 2 + 1) * np + p);
+            }
         }
 #pragma unroll
         for (int k = 0; k < NV; ++k) s_pix[k][pi] = v[k];
@@ -1351,6 +1356,8 @@ static int ensure_smem_attrs() {
     UMR_SET((k_raster_bwd_pairs_list<0, false>)) UMR_SET((k_raster_bwd_pairs_list<0, true>))
     UMR_SET((k_raster_bwd_pairs_list<1, false>)) UMR_SET((k_raster_bwd_pairs_list<1, true>))
     UMR_SET((k_raster_bwd_pairs<1, true, 3, true>)) UMR_SET((k_raster_bwd_pairs_list<1, true, 3, true>))
+    UMR_SET((k_raster_fwd4<RGB_SIL>)) UMR_SET((k_raster_fwd4<RGB_SIL, uint32_t>))
+    UMR_SET((k_raster_bwd_pairs<RGB_SIL, false>)) UMR_SET((k_raster_bwd_pairs_list<RGB_SIL, false>))
 #undef UMR_SET
     done[dev] = true;
     return 0;
@@ -1792,4 +1799,163 @@ extern "C" int umr_raster_backward_split_deterministic(const float* face_vertice
     if (split_refused(p, grad_faces, grad_textures)) return UMR_ERR_BAD_ARG;
     return raster_backward_det(face_vertices, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, p,
                                workspace, stream_, true);
+}
+
+// =============================================================================================
+// Silhouette render (DESIGN.md §12): the alpha plane and its vertex gradient, UMR's configuration only
+// =============================================================================================
+// Refused before any device work: what check_params refuses, the generic modes and the 4-channel render (UMR_ERR_BAD_ARG).
+static int check_silhouette_params(const UmrRasterParams* p) {
+    int rc = check_params(p);
+    if (rc) return rc;
+    if (is_generic(p) || p->color_channels == 4) return UMR_ERR_BAD_ARG;
+    return UMR_OK;
+}
+static bool misaligned_f32(const void* ptr) { return ((uintptr_t)ptr & (sizeof(float) - 1)) != 0; }
+
+// det: the deterministic twin -- the 16x16-tile forward whatever tile_mode says and no pair buffer (the silhouette forward
+// has no float atomics either way, so its planes are those of the default call)
+static int raster_forward_silhouette(const float* face_vertices, float* alpha, float* alpha_hi, const UmrRasterParams* p,
+                                     void* workspace, void* stream_, bool det) {
+    int rc = check_silhouette_params(p);
+    if (rc) return rc;
+    if (det && (int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;
+    if (!face_vertices || !alpha || !workspace) return UMR_ERR_BAD_ARG;
+    if (misaligned_f32(face_vertices) || misaligned_f32(alpha) || misaligned_f32(alpha_hi) || ((uintptr_t)workspace & 255) != 0)
+        return UMR_ERR_BAD_ARG;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    rc = ensure_smem_attrs();
+    if (rc) return rc;
+    const int B = p->batch_size, F = p->num_faces;
+    const Consts<float> K = make_consts(p);
+    if (!K.aa && alpha_hi == nullptr) alpha_hi = alpha;  // the raster is the image
+    const WorkspaceLayout L = ws_layout(B, F, K.S);
+    char* ws = (char*)workspace;
+    float* rec = (float*)(ws + L.rec_off);
+    float4* box = (float4*)(ws + L.box_off);
+    uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
+    int* ccount = (int*)(ws + L.ccount_off);
+    void* clist = ws + L.clist_off;
+    cudaError_t e = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
+    if (e != cudaSuccess) return (int)e;
+    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr));
+    count_launch();
+    const PairBuf pb = det ? PairBuf{nullptr, nullptr, nullptr, nullptr, nullptr, 0u} : make_pairbuf(p, K.S);
+    if (pb.cap > 0) {
+        e = cudaMemsetAsync(pb.ctrl, 0, 16, stream);
+        if (e != cudaSuccess) return (int)e;
+    }
+    count_launch(2);
+    rc = launch_bin_coarse(box, ubox, clist, ccount, B, F, K.S, L, stream);
+    if (rc) return rc;
+    const int ncb = (K.S + CB - 1) / CB;
+    const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
+    const dim3 grid32((K.S + T4 - 1) / T4, (K.S + T4 - 1) / T4, B);
+    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
+#define UMR_SIL_ARGS(IDX) rec, box, (const IDX*)clist, ccount, /*textures*/ nullptr, alpha, alpha_hi, /*aggrs*/ nullptr, \
+                          /*p2f*/ nullptr, ubox, K, p->eps, 0.f, 0.f, 0.f, pb, ncb
+#define UMR_SIL_FWD(IDX)                                                                                                  \
+    if (det || forward_impl(p->tile_mode) == 3)                                                                           \
+        k_raster_fwd3<RGB_SIL, 3, IDX><<<grid, CTA, 0, stream>>>(UMR_SIL_ARGS(IDX));                                      \
+    else                                                                                                                  \
+        k_raster_fwd4<RGB_SIL, IDX><<<grid32, CTA, fwd4_dyn_smem(F, sizeof(IDX)), stream>>>(UMR_SIL_ARGS(IDX));
+    if (F > NARROW_MAX_FACES) { UMR_SIL_FWD(uint32_t) } else { UMR_SIL_FWD(uint16_t) }
+#undef UMR_SIL_FWD
+#undef UMR_SIL_ARGS
+    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+    return (int)cudaGetLastError();
+}
+
+// det: k_prep, then the face-parallel gather (no pair buffer, no atomics); otherwise the streamed backward over the pairs the
+// forward saved and the recompute backward for the tiles it could not save (or for every tile without a pair buffer)
+static int raster_backward_silhouette(const float* face_vertices, const float* alpha_hi, const float* grad_alpha,
+                                      float* grad_faces, const UmrRasterParams* p, void* workspace, void* stream_, bool det) {
+    int rc = check_silhouette_params(p);
+    if (rc) return rc;
+    if (det && (int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;
+    if (!face_vertices || !alpha_hi || !grad_alpha || !grad_faces || !workspace) return UMR_ERR_BAD_ARG;
+    if (misaligned_f32(face_vertices) || misaligned_f32(alpha_hi) || misaligned_f32(grad_alpha) || misaligned_f32(grad_faces) ||
+        ((uintptr_t)workspace & 255) != 0)
+        return UMR_ERR_BAD_ARG;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    rc = ensure_smem_attrs();
+    if (rc) return rc;
+    const int B = p->batch_size, F = p->num_faces;
+    const Consts<float> K = make_consts(p);
+    const WorkspaceLayout L = ws_layout(B, F, K.S);
+    char* ws = (char*)workspace;
+    float* rec = (float*)(ws + L.rec_off);
+    float4* box = (float4*)(ws + L.box_off);
+    uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
+    // the workspace is scratch (another render may have used it since forward): rebuild the records
+    cudaError_t e = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
+    if (e != cudaSuccess) return (int)e;
+    if (det) {
+        k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr));
+        const dim3 grid((unsigned)((F + NWARP - 1) / NWARP), (unsigned)(B / K.tex_div));
+        if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
+        k_raster_bwd_det<float, RGB_SIL, false><<<grid, CTA, 0, stream>>>(rec, nullptr, alpha_hi, nullptr, grad_alpha, grad_faces,
+                                                                         nullptr, K);
+        if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+        count_launch(2);
+        return (int)cudaGetLastError();
+    }
+    const PairBuf pb = make_pairbuf(p, K.S);
+    // the streamed silhouette backward reads no face record: with a pair buffer only the recompute fallback needs them, so
+    // k_prep returns at once when no tile is unsaved
+    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr),
+                                                         pb.cap > 0 ? pb.ctrl + 1 : nullptr);
+    count_launch();
+    e = cudaMemsetAsync(grad_faces, 0, (size_t)B * F * 9 * sizeof(float), stream);
+    if (e != cudaSuccess) return (int)e;
+    const size_t smem = raster_dyn_smem(F);
+    const dim3 grid_pairs((K.S + PT - 1) / PT, (K.S + PT - 1) / PT, B);
+    const dim3 grid32((K.S + T4 - 1) / T4, (K.S + T4 - 1) / T4, B);
+    const size_t ntiles = (size_t)grid_pairs.x * grid_pairs.y * B;
+    int sms = 0;
+    rc = sm_count(&sms);
+    if (rc) return rc;
+    const size_t list_max = (size_t)3 * sms;  // 3 resident CTAs per SM walk the unsaved-tile list
+    const unsigned list_grid = (unsigned)(ntiles < list_max ? ntiles : list_max);
+    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
+    count_launch();
+    if (pb.cap > 0) {
+        count_launch();
+#define UMR_SIL_BWD2(TS, IDX, G)                                                                                          \
+        k_raster_bwd2<RGB_SIL, false, TS, 3, true, false, IDX><<<G, BWD2_THREADS, 0, stream>>>(                           \
+            nullptr, nullptr, alpha_hi, nullptr, grad_alpha, grad_faces, nullptr, K, pb)
+        const bool wide = F > NARROW_MAX_FACES;
+        if (forward_impl(p->tile_mode) == 4) { if (wide) UMR_SIL_BWD2(32, uint32_t, grid32); else UMR_SIL_BWD2(32, uint16_t, grid32); }
+        else { if (wide) UMR_SIL_BWD2(16, uint32_t, grid_pairs); else UMR_SIL_BWD2(16, uint16_t, grid_pairs); }
+#undef UMR_SIL_BWD2
+        k_raster_bwd_pairs_list<RGB_SIL, false><<<list_grid, CTA, smem, stream>>>(
+            rec, box, nullptr, alpha_hi, nullptr, grad_alpha, grad_faces, nullptr, ubox, K, pb.ctrl + 1, pb.ulist,
+            (int)grid_pairs.x, (int)grid_pairs.y);
+    } else {
+        k_raster_bwd_pairs<RGB_SIL, false><<<grid_pairs, CTA, smem, stream>>>(rec, box, nullptr, alpha_hi, nullptr, grad_alpha,
+                                                                              grad_faces, nullptr, ubox, K);
+    }
+    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+    return (int)cudaGetLastError();
+}
+
+extern "C" int umr_raster_forward_silhouette(const float* face_vertices, float* alpha, float* alpha_hi,
+                                             const UmrRasterParams* p, void* workspace, void* stream_) {
+    return raster_forward_silhouette(face_vertices, alpha, alpha_hi, p, workspace, stream_, false);
+}
+
+extern "C" int umr_raster_forward_silhouette_deterministic(const float* face_vertices, float* alpha, float* alpha_hi,
+                                                           const UmrRasterParams* p, void* workspace, void* stream_) {
+    return raster_forward_silhouette(face_vertices, alpha, alpha_hi, p, workspace, stream_, true);
+}
+
+extern "C" int umr_raster_backward_silhouette(const float* face_vertices, const float* alpha_hi, const float* grad_alpha,
+                                              float* grad_faces, const UmrRasterParams* p, void* workspace, void* stream_) {
+    return raster_backward_silhouette(face_vertices, alpha_hi, grad_alpha, grad_faces, p, workspace, stream_, false);
+}
+
+extern "C" int umr_raster_backward_silhouette_deterministic(const float* face_vertices, const float* alpha_hi,
+                                                            const float* grad_alpha, float* grad_faces,
+                                                            const UmrRasterParams* p, void* workspace, void* stream_) {
+    return raster_backward_silhouette(face_vertices, alpha_hi, grad_alpha, grad_faces, p, workspace, stream_, true);
 }

@@ -16,6 +16,10 @@ constexpr int FWD3_CTAS = 4;
 // (aggrs planes: depth_min, face_index_min) and nothing else: no distance / sigmoid / alpha / colour arithmetic, no image
 // planes.  That is all `MultiTextureLoss` keeps of its hard render (loss_utils.py:327-329: `_, p2f, aggr = hard_renderer(...)`,
 // and p2f is zero in hard mode, kernel.cu:417-431).  Same winner as RGB = 0, bit for bit.
+// RGB = RGB_SIL (3): SILHOUETTE -- the alpha plane alone: images is [B,is,is] (pooled alpha), colors_hi [B,S,S] (the
+// full-resolution alpha for the backward, may be NULL), aggrs / p2f / textures are not touched.  No softmax weight, texel or
+// colour work.  Alpha and the set of saved pairs are those of RGB = 0 / 1, bit for bit, and so is every record field the
+// SPLIT walk reads for the alpha terms (and zn, as the softmax forward writes it); the texel field holds 0.
 // IdxT: face-index width of the coarse lists, the tile list and the pair-block headers (uint16_t: F <= 65535)
 // DET: p2f partials go to the fixed-point accumulators of the deterministic mode (red_p2f_fixed) instead of float REDs
 template <int RGB, int NC = 3, typename IdxT = uint16_t, bool DET = false>  // NC colour channels (3, or 4: the part-map render of SURVEY.md 8f-2); planes = NC + 1 (alpha)
@@ -29,6 +33,7 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
                                                         uint8_t* __restrict__ vis_mask = nullptr) {  // RGB = 2: optional [B,F] "face is visible" bytes; aggrs may be NULL
     constexpr int NPL = NC + 1;                                      // image planes: colours + alpha
     constexpr bool VIS = RGB == 2;
+    constexpr bool SIL = RGB == RGB_SIL;
     const float bgc[4] = {bg0, bg1, bg2, bg3};
     constexpr int WG = 16;                                           // list entries per warp group
     __shared__ __align__(128) float s_wrec[NWARP * 2 * WG * REC_LEN];  // 32 KB: warp-private record stages; reused by the store epilogue
@@ -74,6 +79,21 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
         // ---- untouched tile (most of the image): every pixel holds the initial state.  Same arithmetic as the
         // general path (kernel.cu:335-348, 443-475), evaluated once, stored with 128-bit stores where possible.
         if (tid == 0 && pb.cap > 0) pb.tile_head[tile_id] = TILE_EMPTY;
+        if (SIL) {  // alpha 1 - 1 = 0 everywhere, pooled ((0 + 0) + 0 + 0) * 0.25 = 0
+            const int px = tx0 + (tid & (TILE - 1)), py = ty0 + (tid >> 4);
+            if (px < S && py < S) {
+                const size_t p = (size_t)py * S + px;
+                const float a0 = (float)(1. - (double)1.f);
+                if (colors_hi != nullptr) colors_hi[(size_t)b * np + p] = a0;
+                if (K.aa) {
+                    if ((px & 1) == 0 && (py & 1) == 0 && px + 1 < S && py + 1 < S)
+                        images[(size_t)b * K.IS * K.IS + (size_t)(py >> 1) * K.IS + (px >> 1)] = (((a0 + a0) + a0) + a0) * 0.25f;
+                } else if (images != colors_hi) {
+                    images[(size_t)b * np + p] = a0;
+                }
+            }
+            return;
+        }
         const float ssum0 = expf(eps / K.gamma);
         float full[NC + 3], g0, g1;
         if (RGB != 1) {
@@ -363,10 +383,12 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
                         if (!(zp < K.near_ || zp > K.far_)) {
                             emit = true;  // kernel.cu:592: pairs outside the depth range get no gradient at all
                             front = (__float_as_uint(rc[R_FLG]) & 8u) ? 1u : 0u;
-                            tix = (uint32_t)texel_index(k0, k1, K.R);
+                            tix = SIL ? 0u : (uint32_t)texel_index(k0, k1, K.R);
                             const int f = s_list[jl];
                             zsave = zp;
-                            if (RGB == 0) {
+                            if (SIL) {
+                                zsave = (K.far_ - zp) / (K.far_ - K.near_);  // the softmax forward's zn (below)
+                            } else if (RGB == 0) {
                                 const bool inside = fr.w0 <= 1 && fr.w0 >= 0 && fr.w1 <= 1 && fr.w1 >= 0 &&
                                                     fr.w2 <= 1 && fr.w2 >= 0;
                                 if (zp < zmin && inside && (K.double_side || front)) {
@@ -444,6 +466,26 @@ __global__ void __launch_bounds__(CTA, FWD3_CTAS) k_raster_fwd3(const float* __r
 
     // ---- finalise (kernel.cu:443-475) + fused 2x2 pool + coalesced stores (as round 1) --------------------
     const float alpha = (float)(1. - (double)acc_a);  // kernel.cu:449-451
+    if (SIL) {  // the alpha plane of the epilogue below: same value, same pooling sum
+        float v = alpha;
+        if (K.aa) {
+            const float a01 = __shfl_xor_sync(0xffffffffu, v, 1);
+            const float a10 = __shfl_xor_sync(0xffffffffu, v, 8);
+            const float a11 = __shfl_xor_sync(0xffffffffu, v, 9);
+            v = (((v + a01) + a10) + a11) * 0.25f;  // meaningful on the (even x, even y) lane
+        }
+        if (live) {
+            const size_t p = (size_t)py * S + px;
+            if (colors_hi != nullptr) colors_hi[(size_t)b * np + p] = alpha;
+            if (K.aa) {
+                if ((lane & 1) == 0 && (lane & 8) == 0)
+                    images[(size_t)b * K.IS * K.IS + (size_t)(py >> 1) * K.IS + (px >> 1)] = v;
+            } else if (images != colors_hi) {
+                images[(size_t)b * np + p] = alpha;
+            }
+        }
+        return;
+    }
     if (VIS) {
         // face-visibility bytes (what TexCycle derives from the face-index plane with torch.unique, loss_utils.py:161-166):
         // test before set -- a stale 0 only repeats the store

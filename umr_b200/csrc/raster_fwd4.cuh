@@ -26,6 +26,7 @@ __host__ __device__ inline size_t fwd4_dyn_smem(int F, size_t idx_bytes = 2) {
 }
 
 // IdxT: face-index width of the coarse lists, the tile list and the pair-block headers (uint16_t: F <= 65535)
+// RGB: 0 hard, 1 softmax, RGB_SIL the silhouette (alpha plane only; see k_raster_fwd3)
 template <int RGB, typename IdxT = uint16_t>
 __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict__ rec_all, const float4* __restrict__ box_all,
                                                         const IdxT* __restrict__ clist, const int* __restrict__ ccount,
@@ -47,6 +48,7 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
     __shared__ uint32_t s_segbase;
     __shared__ int s_save, s_next;
 
+    constexpr bool SIL = RGB == RGB_SIL;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.z;
     const int S = K.S;
@@ -83,6 +85,21 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
         // ---- untouched tile: store-only, 128-bit stores where the tile is full and the buffers are aligned
         if (tid == 0 && pb.cap > 0) pb.tile_head[tile_id] = TILE_EMPTY;
         const float alpha = (float)(1. - (double)1.f);
+        if (SIL) {  // alpha 0 everywhere, pooled ((0 + 0) + 0 + 0) * 0.25 = 0
+            for (int pi = tid; pi < T4 * T4; pi += CTA) {
+                const int px = tx0 + (pi & (T4 - 1)), py = ty0 + (pi >> 5);
+                if (px >= S || py >= S) continue;
+                const size_t p = (size_t)py * S + px;
+                if (colors_hi != nullptr) colors_hi[(size_t)b * np + p] = alpha;
+                if (K.aa) {
+                    if ((px & 1) == 0 && (py & 1) == 0)
+                        images[(size_t)b * K.IS * K.IS + (size_t)(py >> 1) * K.IS + (px >> 1)] = (((alpha + alpha) + alpha) + alpha) * 0.25f;
+                } else if (images != colors_hi) {
+                    images[(size_t)b * np + p] = alpha;
+                }
+            }
+            return;
+        }
         const float full[6] = {e0, e1, e2, alpha, eg0, eg1};
         float pooled[4];
 #pragma unroll
@@ -265,10 +282,12 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
                         if (!(zp < K.near_ || zp > K.far_)) {
                             emit = true;  // kernel.cu:592: pairs outside the depth range get no gradient at all
                             front = (__float_as_uint(rc[R_FLG]) & 8u) ? 1u : 0u;
-                            tix = (uint32_t)texel_index(k0, k1, K.R);
+                            tix = SIL ? 0u : (uint32_t)texel_index(k0, k1, K.R);
                             const int f = s_list[jl];
                             zsave = zp;
-                            if (RGB == 0) {
+                            if (SIL) {
+                                zsave = (K.far_ - zp) / (K.far_ - K.near_);  // the softmax forward's zn (below)
+                            } else if (RGB == 0) {
                                 const bool inside = fr.w0 <= 1 && fr.w0 >= 0 && fr.w1 <= 1 && fr.w1 >= 0 &&
                                                     fr.w2 <= 1 && fr.w2 >= 0;
                                 if (zp < zmin && inside && (K.double_side || front)) {
@@ -346,6 +365,26 @@ __global__ void __launch_bounds__(CTA, 4) k_raster_fwd4(const float* __restrict_
         const int px = tx0 + lcol, py = ty0 + lrow;
         const bool live = px < S && py < S;
         const float alpha = (float)(1. - (double)st.acc_a);  // kernel.cu:449-451
+        if (SIL) {  // the alpha plane of the stores below: same value, same pooling sum
+            float v = alpha;
+            if (K.aa) {
+                const float a01 = __shfl_xor_sync(0xffffffffu, v, 1);
+                const float a10 = __shfl_xor_sync(0xffffffffu, v, 8);
+                const float a11 = __shfl_xor_sync(0xffffffffu, v, 9);
+                v = (((v + a01) + a10) + a11) * 0.25f;  // meaningful on the (even x, even y) lane
+            }
+            if (live) {
+                const size_t p = (size_t)py * S + px;
+                if (colors_hi != nullptr) colors_hi[(size_t)b * np + p] = alpha;
+                if (K.aa) {
+                    if ((lane & 1) == 0 && (lane & 8) == 0)
+                        images[(size_t)b * K.IS * K.IS + (size_t)(py >> 1) * K.IS + (px >> 1)] = v;
+                } else if (images != colors_hi) {
+                    images[(size_t)b * np + p] = alpha;
+                }
+            }
+            return;
+        }
         float o0, o1, o2, g0, g1;
         if (RGB == 0) {
             o0 = st.c0; o1 = st.c1; o2 = st.c2;

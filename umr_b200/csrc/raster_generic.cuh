@@ -48,6 +48,22 @@ struct Consts {
 // the float kernels' parameter blocks keep their layout
 static_assert(sizeof(Consts<float>) == 104, "Consts<float> layout");
 
+// RGB mode of the float UMR-configuration kernels that form the alpha plane and nothing else (the silhouette render,
+// DESIGN.md §12): no softmax weight, no texel, no colour, no p2f.  Alpha, the pair records and the alpha terms of the
+// vertex gradients are those of the softmax / hard render.
+constexpr int RGB_SIL = 3;
+
+// Per-pixel planes the float backward stages for a pixel: g[NC], g_alpha, C[NC], alpha, ssum, smax -- or, for a silhouette,
+// g_alpha and alpha only.  NPL: planes of the image gradient and of the full-resolution image; GA / AL: plane of g_alpha /
+// alpha in the staged set.
+template <int RGB, int NC>
+struct PixPlanes {
+    static constexpr bool SIL = RGB == RGB_SIL;
+    static constexpr int NPL = SIL ? 1 : NC + 1;
+    static constexpr int NV = SIL ? 2 : 2 * NPL + 2;
+    static constexpr int GA = SIL ? 0 : NC, AL = SIL ? 1 : 2 * NC + 1;
+};
+
 template <typename T>
 struct Frag {
     T w0, w1, w2;  // unclipped barycentrics
@@ -408,14 +424,17 @@ __device__ __forceinline__ bool bwd_pair_acc(const float* __restrict__ rc, float
 // steps); grad_tex is zero-filled by the caller.  Every output is therefore bitwise reproducible.
 // GEN: the generic modes (distance, alpha and texture mode read at run time), evaluated with bwd_pair_generic; a
 // vertex-texture pair adds to the face's 9 corner colours, which the warp sums the same way.  Otherwise (float only) UMR's
-// configuration, evaluated with bwd_pair_acc -- the recompute backward's arithmetic; SPLIT: see bwd_pair_acc.
+// configuration, evaluated with bwd_pair_acc -- the recompute backward's arithmetic; SPLIT: see bwd_pair_acc.  RGB_SIL: the
+// silhouette backward (colors_hi = the full-resolution alpha plane, grad_images = the alpha gradient; aggrs is not read).
 template <typename T, int RGB, bool TEXGRAD, int NC = 3, bool GEN = false, bool SPLIT = false>
 __global__ void __launch_bounds__(CTA) k_raster_bwd_det(const T* __restrict__ rec_all, const T* __restrict__ textures,
                                                         const T* __restrict__ colors_hi, const T* __restrict__ aggrs,
                                                         const T* __restrict__ grad_images, T* __restrict__ grad_faces,
                                                         T* __restrict__ grad_tex, Consts<T> K) {
     static_assert(std::is_same_v<T, float> || (GEN && NC == 3 && !SPLIT), "double runs the generic modes, 3 channels");
-    constexpr int NPL = NC + 1, NV = 2 * NPL + 2, NP = CTA;  // planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
+    static_assert(RGB != RGB_SIL || (!GEN && !TEXGRAD), "the silhouette backward is UMR's configuration, vertex gradients only");
+    using PP = PixPlanes<RGB, NC>;
+    constexpr int NPL = PP::NPL, NV = PP::NV, NP = CTA;  // planes: g[NC], g_alpha, C[NC], alpha, ssum, smax (PixPlanes)
     __shared__ T s_pix[NV][NP];
     __shared__ __align__(16) T s_rc[NWARP][REC_LEN];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -460,8 +479,10 @@ __global__ void __launch_bounds__(CTA) k_raster_bwd_det(const T* __restrict__ re
                     }
 #pragma unroll
                     for (int k = 0; k < NPL; ++k) sp[(NPL + k) * NP] = __ldg(colors_hi + ((size_t)b * NPL + k) * np + p);
-                    sp[(NV - 2) * NP] = __ldg(aggrs + ((size_t)b * 2 + 0) * np + p);
-                    sp[(NV - 1) * NP] = __ldg(aggrs + ((size_t)b * 2 + 1) * np + p);
+                    if (!PP::SIL) {
+                        sp[(NV - 2) * NP] = __ldg(aggrs + ((size_t)b * 2 + 0) * np + p);
+                        sp[(NV - 1) * NP] = __ldg(aggrs + ((size_t)b * 2 + 1) * np + p);
+                    }
                     if constexpr (GEN) {
                         T gv[9];
 #pragma unroll

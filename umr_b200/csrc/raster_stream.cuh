@@ -277,18 +277,22 @@ constexpr int BWD2_THREADS = 256, BWD2_WARPS = BWD2_THREADS / 32;  // threads of
 // SPLIT = true (the split backward, softmax only): the vertex gradients keep only the terms driven by the alpha adjoint, the
 // texel gradients are formed from the colour adjoints as always -- one walk serves a mask loss on alpha and a texture loss on
 // RGB whose geometry is detached.  Without the colour terms no face record is read (no z-gradient factors).
+// RGB = RGB_SIL (the silhouette backward): the alpha terms of SPLIT alone, from two pixel planes -- colors_hi is the
+// full-resolution alpha plane, grad_images the alpha gradient; aggrs, textures and the face records are not read.
 template <int RGB, bool TEXGRAD, int TS, int NC = 3, bool GEOM = true, bool PRE = false, typename IdxT = uint16_t,
-          bool SPLIT = false>  // NC colour channels; pixel planes: g[NC], g_alpha, C[NC], alpha, ssum, smax
+          bool SPLIT = false>  // NC colour channels; pixel planes: g[NC], g_alpha, C[NC], alpha, ssum, smax (PixPlanes)
 __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const float* __restrict__ rec_all, const float* __restrict__ textures,
                                                         const float* __restrict__ colors_hi,
                                                         const float* __restrict__ aggrs, const float* __restrict__ grad_images,
                                                         float* __restrict__ grad_faces, float* __restrict__ grad_tex, Consts<float> K,
                                                         PairBuf pb) {
-    constexpr int NPL = NC + 1, NV = 2 * NPL + 2;
+    using PP = PixPlanes<RGB, NC>;
+    static_assert(!PP::SIL || (GEOM && !TEXGRAD), "the silhouette backward forms vertex gradients only");
+    constexpr int NPL = PP::NPL, NV = PP::NV;
     __shared__ float s_pix[NV][TS * TS];  // g[NC], g_alpha, C[NC], alpha, ssum, smax (row-major tile pixels)
     __shared__ float s_xp[TS], s_yp[TS];  // pixel centres, built as the forward builds its tables (same bits)
     constexpr int NP = TS * TS;
-    constexpr bool ZGRAD = GEOM && !SPLIT;  // the colour terms of the vertex gradients (they read the face records)
+    constexpr bool ZGRAD = GEOM && !SPLIT && !PP::SIL;  // the colour terms of the vertex gradients (they read the face records)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int b = blockIdx.z;
     const int S = K.S, F = K.F;
@@ -305,7 +309,7 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
         const size_t np = (size_t)S * S;
         float v[NV];
 #pragma unroll
-        for (int k = 0; k < NV; ++k) v[k] = (k == NV - 2) ? 1.f : 0.f;
+        for (int k = 0; k < NV; ++k) v[k] = (!PP::SIL && k == NV - 2) ? 1.f : 0.f;
         if (px < S && py < S) {
             const size_t p = (size_t)py * S + px;
             if (K.aa) {  // avg_pool2d backward: g / 4
@@ -319,8 +323,10 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
             }
 #pragma unroll
             for (int k = 0; k < NPL; ++k) v[NPL + k] = __ldg(colors_hi + ((size_t)b * NPL + k) * np + p);
-            v[NV - 2] = __ldg(aggrs + ((size_t)b * 2 + 0) * np + p);
-            v[NV - 1] = __ldg(aggrs + ((size_t)b * 2 + 1) * np + p);
+            if (!PP::SIL) {
+                v[NV - 2] = __ldg(aggrs + ((size_t)b * 2 + 0) * np + p);
+                v[NV - 1] = __ldg(aggrs + ((size_t)b * 2 + 1) * np + p);
+            }
         }
 #pragma unroll
         for (int k = 0; k < NV; ++k) s_pix[k][pi] = v[k];
@@ -454,8 +460,8 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
                 const float* sp = &s_pix[0][pix];
                 float Cxy = 0.f;
                 if (GEOM) {
-                    const float g3 = sp[NC * NP];  // gradient of alpha
-                    const float one_m_a = 1 - sp[(2 * NC + 1) * NP];
+                    const float g3 = sp[PP::GA * NP];  // gradient of alpha
+                    const float one_m_a = 1 - sp[PP::AL * NP];
                     // g3 * ((1 - alpha) / max(1 - D, 1e-6)) (kernel.cu:584), in fp32 (the reference promotes to double;
                     // gradients are compared at 1e-4, see DESIGN.md "backward arithmetic")
                     Cxy = (one_m_a == 0.f || g3 == 0.f) ? g3 * one_m_a : g3 * __fdividef(one_m_a, fmaxf(1 - D, 1e-6f));
@@ -470,7 +476,7 @@ __global__ void __launch_bounds__(BWD2_THREADS, BWD2_CTAS) k_raster_bwd2(const f
                             red_add_texel<NC>(gt, g_);
                         }
                     }
-                } else if (front || K.double_side) {
+                } else if (RGB == 1 && (front || K.double_side)) {
                     float g[NC];
                     bool any = false;
 #pragma unroll

@@ -259,8 +259,9 @@ class MultiMaskLoss(nn.Module):
         H = self.num_hypo_cams
         # vertices / faces are NOT repeated per hypothesis (the reference materialises repeat(1, 8, ...) copies,
         # loss_utils.py:260-261): the vertex kernel broadcasts each mesh over its H cameras (SURVEY.md §8f-1)
-        rgba, _, _ = self.renderer.forward(vs, fs, cams_all_hypo.view(-1, 7))
-        mask_all_hypo = rgba[:, 3, :, :]
+        # only the alpha plane is used (loss_utils.py:262-263): the silhouette render skips the colour work, with the
+        # same values and gradients
+        mask_all_hypo = self.renderer.render_silhouettes(vs, fs, cams_all_hypo.view(-1, 7))
         per_render = neg_iou_loss(mask_all_hypo, tile_hypotheses(masks_gt, H), avg=False)
         return expected_over_hypotheses(per_render, cam_probs), mask_all_hypo
 

@@ -132,6 +132,19 @@ class SoftRenderer(torch.nn.Module):
         rgba, p2f, aggrs = self.forward(vertices.detach(), faces, cams.detach(), textures)
         return torch.cat((rgba[:, :3], alpha), dim=1), p2f, aggrs
 
+    def render_silhouettes(self, vertices, faces, cams):
+        """The alpha plane [B*H,is,is] of `forward(vertices, faces, cams)` (cameras broadcast as there), e.g. for a mask
+        loss.  In the fused configuration: one vertex kernel without lighting and the silhouette raster, whose forward
+        and backward skip every colour, texel and p2f term (alpha depends on neither light nor texture).  Elsewhere
+        (float64, CPU, other raster modes or cameras) `forward(...)[0][:, 3]`."""
+        r = self.renderer
+        if self._fusable(vertices) and r.rasterizer.supports_silhouettes():
+            tr = r.transform.transformer
+            fv, _ = project_faces(vertices, cams, faces, offset_z=self.offset_z, eye_z=float(tr._eye[2]),
+                                  viewing_scale=tr.viewing_scale, flip_y=True, light=None)
+            return r.rasterizer.rasterize_silhouettes(fv)
+        return self.forward(vertices, faces, cams)[0][:, 3]
+
     def visibility(self, vertices, faces, cams):
         """(p2f_info, aggrs_info) of this renderer WITHOUT the image: what `MultiTextureLoss` keeps of its hard render
         (loss_utils.py:327-329, `_, p2f_info, aggr_info = self.hard_renderer(...)`).  For the hard renderer on CUDA this

@@ -401,6 +401,106 @@ def soft_rasterize_split(face_vertices, textures, image_size=256, background_col
                                             aggr_func_rgb, aggr_func_alpha, texture_type, anti_aliasing)
 
 
+class SoftRasterizeSilhouetteFunction(torch.autograd.Function):
+    """forward(face_vertices[B,F,3,3|9], ...) -> alpha [B,is,is]: the alpha plane of SoftRasterizeFunction (euclidean
+    distance, prod alpha), bit for bit, without the colour, p2f and aggregation work (umr_raster_forward_silhouette).  Its
+    gradient is the full render's vertex gradient when only the alpha plane has an adjoint: bitwise in the deterministic
+    mode, the same per-pair terms summed with float atomics otherwise.  float32 only (float64 raises; SoftRenderer's
+    `render_silhouettes` renders such meshes in full).  Saves only the full-resolution alpha (and the pair buffer)."""
+
+    @staticmethod
+    def forward(ctx, face_vertices, image_size=256, near=1, far=100, fill_back=True, eps=1e-3, sigma_val=1e-5,
+                dist_eps=1e-4, gamma_val=1e-4, anti_aliasing=False):
+        if not face_vertices.is_cuda:
+            raise TypeError("Rasterize module supports only cuda Tensors")  # soft_rasterize.py:117-118
+        if face_vertices.dtype == torch.float64:
+            raise ValueError("the silhouette raster is float32 only: render float64 meshes in full (SoftRenderer.render_silhouettes)")
+        mode = KernelMode(False)
+        dev = face_vertices.device
+        B, F = face_vertices.shape[:2]
+        fv = face_vertices.detach().reshape(B, F, 9).contiguous().float()
+        S = int(image_size) * (2 if anti_aliasing else 1)
+        # no texture: one texel per face, and the colour mode does not touch alpha
+        params = make_params(B, F, 1, image_size, anti_aliasing, (0, 0, 0), near, far, fill_back, eps, sigma_val,
+                             "euclidean", dist_eps, gamma_val, "softmax", "prod", "surface")
+        params.tile_mode = FORWARD_TILE
+        params.color_channels = 3
+        need_bwd = face_vertices.requires_grad
+        _attach_events(params, "fwd")
+        with torch.cuda.device(dev):
+            alpha = torch.empty(B, image_size, image_size, device=dev, dtype=torch.float32)
+            if anti_aliasing:
+                alpha_hi = torch.empty(B, S, S, device=dev, dtype=torch.float32) if need_bwd else None
+            else:
+                alpha_hi = alpha
+            ws = torch.empty(_lib.load().umr_raster_workspace_bytes(B, F, int(image_size), params.anti_aliasing), device=dev,
+                             dtype=torch.uint8)
+            pairs = None
+            pair_key = (S, F, FORWARD_TILE)   # the full render's key: both forwards save the same pairs
+            if need_bwd and not mode.det and PAIR_CAND_PER_PIXEL > 0:
+                capturing = torch.cuda.is_current_stream_capturing()
+                if PAIR_ADAPTIVE and not capturing:
+                    _pair_poll()
+                need = _pair_need.get(pair_key) if (PAIR_ADAPTIVE and PAIR_CAND_PER_PIXEL >= 1.0) else None
+                pairs = torch.empty(pair_buffer_bytes(B, image_size, anti_aliasing, blocks_per_image=need, device=dev), device=dev,
+                                    dtype=torch.uint8)
+                params.pair_buffer, params.pair_buffer_bytes = pairs.data_ptr(), pairs.numel()
+            mode.call("umr_raster_forward_silhouette", True, _ptr(fv), _ptr(alpha), _ptr(alpha_hi), ctypes.byref(params),
+                      _ptr(ws), _stream_ptr(dev))
+        if pairs is not None:
+            _pair_record(pair_key, B, pairs)
+        params.ev_kernel_start = params.ev_kernel_stop = None
+        ctx.params = params
+        ctx.in_shape = tuple(face_vertices.shape)
+        ctx.has_pairs = pairs is not None
+        ctx.mode = mode
+        if need_bwd:
+            if pairs is not None:
+                ctx.save_for_backward(fv, alpha_hi, pairs)
+            else:
+                ctx.save_for_backward(fv, alpha_hi)
+        return alpha
+
+    @staticmethod
+    def backward(ctx, grad_alpha):
+        mode = ctx.mode
+        if ctx.has_pairs:
+            fv, alpha_hi, pairs = ctx.saved_tensors
+            assert ctx.params.pair_buffer == pairs.data_ptr()
+        else:
+            fv, alpha_hi = ctx.saved_tensors
+        dev = fv.device
+        B, F = fv.shape[:2]
+        g = grad_alpha.contiguous().float()
+        _attach_events(ctx.params, "bwd")
+        with torch.cuda.device(dev):
+            grad_faces = torch.empty_like(fv)
+            ws = torch.empty(_lib.load().umr_raster_workspace_bytes(B, F, ctx.params.image_size, ctx.params.anti_aliasing),
+                             device=dev, dtype=torch.uint8)
+            mode.call("umr_raster_backward_silhouette", True, _ptr(fv), _ptr(alpha_hi), _ptr(g), _ptr(grad_faces),
+                      ctypes.byref(ctx.params), _ptr(ws), _stream_ptr(dev))
+        ctx.params.ev_kernel_start = ctx.params.ev_kernel_stop = None
+        return (grad_faces.view(ctx.in_shape),) + (None,) * 9
+
+
+def soft_rasterize_silhouettes(face_vertices, image_size=256, near=1, far=100, fill_back=True, eps=1e-3, sigma_val=1e-5,
+                               dist_eps=1e-4, gamma_val=1e-4, anti_aliasing=False):
+    """The alpha plane [B,is,is] of `soft_rasterize(face_vertices, ...)` with euclidean distance and prod alpha (any colour
+    mode and texture give the same alpha), rendered and differentiated without colour (SoftRasterizeSilhouetteFunction)."""
+    return SoftRasterizeSilhouetteFunction.apply(face_vertices, image_size, near, far, fill_back, eps, sigma_val, dist_eps,
+                                                 gamma_val, anti_aliasing)
+
+
+def raster_calls_wrapped():
+    """True while something other than SoftRasterizeFunction's own `apply` is installed on it (a wrapper that captures
+    or traces raster calls).  Such a wrapper expects to see every render of the package, so the renderers take the full
+    render, through it, in place of a silhouette render while it is installed."""
+    return SoftRasterizeFunction.apply != _PLAIN_APPLY
+
+
+_PLAIN_APPLY = SoftRasterizeFunction.apply
+
+
 def visibility(face_vertices, image_size=256, near=1, far=100, fill_back=True, eps=1e-3, sigma_val=1e-5,
                dist_eps=1e-4, gamma_val=1e-4, anti_aliasing=False, want_faces=False):
     """The hard z-buffer's winner per raster pixel and nothing else: returns aggrs_info [B,2,S,S] = (depth_min,

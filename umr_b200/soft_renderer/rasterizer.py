@@ -2,7 +2,7 @@
 and error messages); the 2x supersampling + `avg_pool2d` of rasterizer.py:43,52-53 is fused into the kernels."""
 import torch.nn as nn
 
-from ..raster import soft_rasterize, soft_rasterize_split, visibility
+from ..raster import raster_calls_wrapped, soft_rasterize, soft_rasterize_silhouettes, soft_rasterize_split, visibility
 from ._args import bind
 
 # (name, default) in the reference's positional order
@@ -44,6 +44,19 @@ class SoftRasterizer(nn.Module):
     def supports_split(self):
         """The split backward exists for UMR's configuration (euclidean / prod / surface), softmax or hard colours."""
         return self.dist_func == "euclidean" and self.aggr_func_alpha == "prod" and self.texture_type == "surface"
+
+    def rasterize_silhouettes(self, face_vertices):
+        """The alpha plane [B,is,is] of `rasterize` (whatever the textures and colour mode), rendered without colour
+        (raster.soft_rasterize_silhouettes); see supports_silhouettes."""
+        return soft_rasterize_silhouettes(face_vertices, self.image_size, self.near, self.far, self.fill_back, self.eps,
+                                          self.sigma_val, self.dist_eps, self.gamma_val, self.anti_aliasing)
+
+    def supports_silhouettes(self):
+        """The silhouette kernels exist for UMR's configuration (euclidean distance, prod alpha, surface textures).  While a
+        wrapper is installed on SoftRasterizeFunction.apply (raster.raster_calls_wrapped) callers render in full, through
+        it."""
+        return (self.dist_func == "euclidean" and self.aggr_func_alpha == "prod" and self.texture_type == "surface"
+                and not raster_calls_wrapped())
 
     def supports_visibility(self):
         """The visibility-only kernel exists for UMR's configuration of the hard renderer (nnutils/smr.py:52-58)."""
