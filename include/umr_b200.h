@@ -635,6 +635,32 @@ int umr_corr_chamfer_backward_f64(const double* vertices, int64_t vertices_batch
                                   double* grad_vertices, double* grad_cams, int32_t B, int32_t NS, int32_t V,
                                   const int32_t* vert_rowptr, const int32_t* vert_selection, void* workspace, void* stream);
 
+/* part_matching_loss head (nnutils/loss_utils.py, everything after the part render; DESIGN.md §13), square H x H maps.
+ * maps: HOST array of 4 device pointers to the part maps P_1..P_4, each [B,H,W] dense per image with map_bstrides[k]
+ * elements between images (e.g. channels of a [B,4|5,H,W] render, or [B,1,H,W] tensors).  c0 [B,H,W] (c0_bstride): channel
+ * 0 of proj.  part_segs [B,5,H,W] dense per image (segs_bstride).  weights [5] device.  kld: 0 = mse, 1 = kld.
+ * terms [B,2] per image: [0] = sum over the 4 parts and x, y of (C - C^Q)^2 (soft centroids of softmax(proj) and
+ * softmax(part_segs) + 1e-3), [1] = mse: sum_c w_c sum_hw (proj_c / max(max_hw proj_c, 1e-5) - Q_c / max(max_hw Q_c, 1e-5))^2,
+ * kld: sum_{c,hw} xlogy(R, R) - R log_softmax(proj) with R = softmax(part_segs).  The caller applies avg / cam_probs / the
+ * final scaling.  `workspace` (umr_part_head_workspace_bytes) is filled by the forward and read by the backward, which
+ * takes the forward's arguments and writes grad_maps [B,4,H,W] (contiguous, fully written) from grad_terms [B,2].  The
+ * max's gradient goes to torch.max's index (NaN first, then the lowest flat index); a clamped max passes none.
+ * Reductions store per-CTA partials summed in ascending order (no atomics): bitwise reproducible in every mode, so there
+ * is no _deterministic form.  `dtype` (UMR_DTYPE_FLOAT32 / UMR_DTYPE_FLOAT64, as umr_voxelize takes it) is the element
+ * type of every buffer; float64 runs double kernels with each operation rounded once.  NULL, non-positive sizes, kld not
+ * 0/1, another dtype, negative strides or buffers not aligned to their element size return UMR_ERR_BAD_ARG (the workspace
+ * query returns 0 for them); B > 65535 or H * H > INT32_MAX UMR_ERR_TOO_LARGE.  Forward: 4 launches (mse) or 2 (kld);
+ * backward: 1.  No host synchronisation (CUDA-graph capturable). */
+size_t umr_part_head_workspace_bytes(int32_t B, int32_t H, int32_t dtype);
+/* = B * (S * 40 * (ceil(H*H / 2048) + 1) + 4 * (8 + 10 * ceil(H*H / 2048))), S = 4 (UMR_DTYPE_FLOAT32) or 8 (UMR_DTYPE_FLOAT64) */
+int umr_part_head_forward(const void* const* maps, const int64_t* map_bstrides, const void* c0, int64_t c0_bstride,
+                          const void* part_segs, int64_t segs_bstride, const void* weights, void* terms, int32_t B, int32_t H,
+                          int32_t kld, int32_t dtype, void* workspace, void* stream);
+int umr_part_head_backward(const void* const* maps, const int64_t* map_bstrides, const void* c0, int64_t c0_bstride,
+                           const void* part_segs, int64_t segs_bstride, const void* weights, const void* workspace,
+                           const void* grad_terms, void* grad_maps, int32_t B, int32_t H, int32_t kld, int32_t dtype,
+                           void* stream);
+
 #ifdef __cplusplus
 }
 #endif

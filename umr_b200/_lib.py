@@ -222,6 +222,14 @@ EXPORTS = {
                                                      ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_int32),
                                                      ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_double)] +
                                       [ctypes.c_void_p] * 6 + [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 4),
+    # part_matching_loss head: maps / map_bstrides are host arrays of 4; `dtype` as umr_voxelize takes it
+    "umr_part_head_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 3),
+    "umr_part_head_forward": (ctypes.c_int, [ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_int64), ctypes.c_void_p,
+                                             ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p] +
+                              [ctypes.c_int32] * 4 + [ctypes.c_void_p] * 2),
+    "umr_part_head_backward": (ctypes.c_int, [ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_int64), ctypes.c_void_p,
+                                              ctypes.c_int64, ctypes.c_void_p, ctypes.c_int64] + [ctypes.c_void_p] * 4 +
+                               [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
 }
 
 _lock = threading.Lock()

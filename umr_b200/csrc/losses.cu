@@ -322,3 +322,34 @@ extern "C" int umr_bilinear_sample_backward_deterministic(const float* image, co
     return sample_backward_gather(image, flow, grad_out, grad_flow, grad_image, B, C, H, W, N, cell_rowptr, cell_samples,
                                   stream_);
 }
+
+// part_matching_loss head (include/umr_b200.h, DESIGN.md §13): one entry point per operation for both precisions (the
+// double instantiations live in losses_f64.cu).  Slot reductions only, so there is no _deterministic form.
+extern "C" size_t umr_part_head_workspace_bytes(int32_t B, int32_t H, int32_t dtype) {
+    if (dtype == UMR_DTYPE_FLOAT32) return part_head_workspace_bytes<float>(B, H);
+    if (dtype == UMR_DTYPE_FLOAT64) return part_head_workspace_bytes<double>(B, H);
+    return 0;
+}
+extern "C" int umr_part_head_forward(const void* const* maps, const int64_t* map_bstrides, const void* c0, int64_t c0_bstride,
+                                     const void* part_segs, int64_t segs_bstride, const void* weights, void* terms, int32_t B,
+                                     int32_t H, int32_t kld, int32_t dtype, void* workspace, void* stream_) {
+    if (dtype == UMR_DTYPE_FLOAT64)
+        return part_head_forward_f64(maps, map_bstrides, c0, c0_bstride, part_segs, segs_bstride, weights, terms, B, H, kld,
+                                     workspace, stream_);
+    if (dtype != UMR_DTYPE_FLOAT32) return UMR_ERR_BAD_ARG;
+    return part_head_forward(reinterpret_cast<const float* const*>(maps), map_bstrides, (const float*)c0, c0_bstride,
+                             (const float*)part_segs, segs_bstride, (const float*)weights, (float*)terms, B, H, kld, workspace,
+                             stream_);
+}
+extern "C" int umr_part_head_backward(const void* const* maps, const int64_t* map_bstrides, const void* c0, int64_t c0_bstride,
+                                      const void* part_segs, int64_t segs_bstride, const void* weights, const void* workspace,
+                                      const void* grad_terms, void* grad_maps, int32_t B, int32_t H, int32_t kld, int32_t dtype,
+                                      void* stream_) {
+    if (dtype == UMR_DTYPE_FLOAT64)
+        return part_head_backward_f64(maps, map_bstrides, c0, c0_bstride, part_segs, segs_bstride, weights, workspace,
+                                      grad_terms, grad_maps, B, H, kld, stream_);
+    if (dtype != UMR_DTYPE_FLOAT32) return UMR_ERR_BAD_ARG;
+    return part_head_backward(reinterpret_cast<const float* const*>(maps), map_bstrides, (const float*)c0, c0_bstride,
+                              (const float*)part_segs, segs_bstride, (const float*)weights, workspace, (const float*)grad_terms,
+                              (float*)grad_maps, B, H, kld, stream_);
+}

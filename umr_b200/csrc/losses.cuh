@@ -572,6 +572,320 @@ __global__ void __launch_bounds__(256) k_losshead_bwd(const T* __restrict__ rgba
 }
 
 // ---------------------------------------------------------------------------------------------
+// part_matching_loss head (nnutils/loss_utils.py, everything after the part render; DESIGN.md §13).  Per image b, with
+// proj = (c0, P_1..P_4) and Q the five part_segs channels, S = softmax_c(proj), R = softmax_c(Q), x/y the float32
+// coordinate maps of `_coordinate_maps`:
+//   terms[b][0] = sum_{c=1..4, d} (C_cd - CQ_cd)^2,  C_c = (sum m x, sum m y) / sum m,  m = S_c + 1e-3 (CQ likewise from R)
+//   terms[b][1] = mse: sum_c w_c sum_p (proj_c / mp_c - Q_c / mq_c)^2,  mp_c = clamp_min(max_p proj_c, 1e-5) (mq_c of Q)
+//                 kld: sum_{c,p} xlogy(R, R) - R log_softmax_c(proj)
+// Forward: a per-CTA partial pass (centroid sums of S and R, the KL sum, max and arg-max of all ten channels) into
+// workspace slots, a per-image finalize that sums the slots in ascending order, and for mse a second partial pass (the
+// terms and, per channel, sum_p d_c proj_c for the max's adjoint) with its finalize.  Backward: one elementwise pass from
+// per-image adjoints of the two terms.  No atomics: every output is bitwise reproducible.
+// ---------------------------------------------------------------------------------------------
+constexpr int PH_THREADS = 256;
+constexpr int PH_PER_CTA = PH_THREADS * 8;  // pixels per CTA
+constexpr int PH_SUMS = 25;                 // (Z, X, Y) of S_1..S_4, then of R_1..R_4, then the KL sum
+constexpr int PH_MAX = 10;                  // max of proj_0..4, then of Q_0..4
+constexpr int PH_MSE = 5;                   // E, then G_1..G_4 = sum_p d_c proj_c
+constexpr int PH_SLOT = PH_SUMS + PH_MAX + PH_MSE;
+// per-image stats: Z_1..4 [0,4), C [4,12), CQ [12,20), mp [20,25), mq [25,30), raw max of proj [30,35), G [35,40)
+constexpr int PH_STATS = 40;
+constexpr int PH_IDX = 8;                   // per-image int32: arg-max of proj_0..4 (3 unused)
+
+template <typename T>
+struct PartHeadIn {
+    const T* map[4];
+    int64_t map_bs[4];
+    const T* c0;
+    int64_t c0_bs;
+    const T* q;
+    int64_t q_bs;
+};
+
+__device__ __forceinline__ float ph_exp(float v) { return expf(v); }
+__device__ __forceinline__ double ph_exp(double v) { return exp(v); }
+__device__ __forceinline__ float ph_log(float v) { return logf(v); }
+__device__ __forceinline__ double ph_log(double v) { return log(v); }
+
+// `_coordinate_maps`: k / n * 2 - 1 evaluated in double and rounded to float32 (widened again for T = double)
+template <typename T>
+__device__ __forceinline__ T ph_coord(int k, int n) { return (T)(float)((double)k / (double)n * 2.0 - 1.0); }
+
+// torch.max's choice: NaN wins, then the larger value, then the lower flat index (a total order, so any reduction tree
+// picks the same element)
+template <typename T>
+__device__ __forceinline__ bool ph_beats(T a, int ia, T b, int ib) {
+    const bool na = a != a, nb = b != b;
+    if (na || nb) return na && (!nb || ia < ib);
+    return a > b || (a == b && ia < ib);
+}
+
+template <typename T>
+__device__ __forceinline__ void ph_load(const PartHeadIn<T>& in, int b, int64_t HW, int p, T v[5], T q[5]) {
+    v[0] = __ldg(in.c0 + (size_t)b * in.c0_bs + p);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) v[k + 1] = __ldg(in.map[k] + (size_t)b * in.map_bs[k] + p);
+    const T* qb = in.q + (size_t)b * in.q_bs;
+#pragma unroll
+    for (int c = 0; c < 5; ++c) q[c] = __ldg(qb + (size_t)c * HW + p);
+}
+
+// s[c] = softmax over the five channels; returns log of the sum of exp(v - max), with `mx` the max
+template <typename T>
+__device__ __forceinline__ void ph_softmax(const T v[5], T s[5], T& mx, T& sum) {
+    mx = v[0];
+#pragma unroll
+    for (int c = 1; c < 5; ++c) mx = v[c] > mx ? v[c] : mx;
+    sum = 0;
+#pragma unroll
+    for (int c = 0; c < 5; ++c) { s[c] = ph_exp(v[c] - mx); sum += s[c]; }
+#pragma unroll
+    for (int c = 0; c < 5; ++c) s[c] = s[c] / sum;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(PH_THREADS) k_part_head_partial(const PartHeadIn<T> in, T* __restrict__ slots,
+                                                                  int32_t* __restrict__ slot_idx, int H, int kld) {
+    const int b = blockIdx.y;
+    const int64_t HW = (int64_t)H * H;
+    const int begin = blockIdx.x * PH_PER_CTA;
+    const int end = (int)min(HW, (int64_t)begin + PH_PER_CTA);
+    T acc[PH_SUMS];
+#pragma unroll
+    for (int k = 0; k < PH_SUMS; ++k) acc[k] = 0;
+    T mv[PH_MAX];
+    int mi[PH_MAX];
+#pragma unroll
+    for (int c = 0; c < PH_MAX; ++c) { mv[c] = -(T)INFINITY; mi[c] = INT_MAX; }
+    for (int p = begin + threadIdx.x; p < end; p += PH_THREADS) {
+        const int i = p / H, j = p - i * H;
+        const T x = ph_coord<T>(j, H), y = ph_coord<T>(i, H);
+        T v[5], q[5], s[5], r[5], mx, sum, qmx, qsum;
+        ph_load(in, b, HW, p, v, q);
+#pragma unroll
+        for (int c = 0; c < 5; ++c) {
+            if (ph_beats(v[c], p, mv[c], mi[c])) { mv[c] = v[c]; mi[c] = p; }
+            if (ph_beats(q[c], p, mv[5 + c], mi[5 + c])) { mv[5 + c] = q[c]; mi[5 + c] = p; }
+        }
+        ph_softmax(v, s, mx, sum);
+        ph_softmax(q, r, qmx, qsum);
+#pragma unroll
+        for (int c = 1; c < 5; ++c) {
+            const T m = s[c] + T(1e-3), mr = r[c] + T(1e-3);
+            acc[3 * (c - 1) + 0] += m;
+            acc[3 * (c - 1) + 1] += m * x;
+            acc[3 * (c - 1) + 2] += m * y;
+            acc[12 + 3 * (c - 1) + 0] += mr;
+            acc[12 + 3 * (c - 1) + 1] += mr * x;
+            acc[12 + 3 * (c - 1) + 2] += mr * y;
+        }
+        if (kld) {
+            const T lse = mx + ph_log(sum);
+#pragma unroll
+            for (int c = 0; c < 5; ++c) acc[24] += (r[c] == T(0) ? T(0) : r[c] * ph_log(r[c])) - r[c] * (v[c] - lse);  // xlogy(R, R) - R logS
+        }
+    }
+    __shared__ T s_sum[PH_THREADS / 32][PH_SUMS];
+    __shared__ T s_mv[PH_THREADS / 32][PH_MAX];
+    __shared__ int s_mi[PH_THREADS / 32][PH_MAX];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < PH_SUMS; ++k) {
+        const T t = warp_sum(acc[k]);
+        if (lane == 0) s_sum[warp][k] = t;
+    }
+#pragma unroll
+    for (int c = 0; c < PH_MAX; ++c) {
+        T a = mv[c];
+        int ia = mi[c];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const T ob = __shfl_xor_sync(0xffffffffu, a, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, ia, o);
+            if (ph_beats(ob, oi, a, ia)) { a = ob; ia = oi; }
+        }
+        if (lane == 0) { s_mv[warp][c] = a; s_mi[warp][c] = ia; }
+    }
+    __syncthreads();
+    const size_t slot = (size_t)b * gridDim.x + blockIdx.x;
+    const int t = threadIdx.x;
+    if (t < PH_SUMS) {
+        T tot = 0;
+        for (int w = 0; w < PH_THREADS / 32; ++w) tot += s_sum[w][t];
+        slots[slot * PH_SLOT + t] = tot;
+    } else if (t >= 32 && t < 32 + PH_MAX) {
+        const int c = t - 32;
+        T a = s_mv[0][c];
+        int ia = s_mi[0][c];
+        for (int w = 1; w < PH_THREADS / 32; ++w)
+            if (ph_beats(s_mv[w][c], s_mi[w][c], a, ia)) { a = s_mv[w][c]; ia = s_mi[w][c]; }
+        slots[slot * PH_SLOT + PH_SUMS + c] = a;
+        slot_idx[slot * PH_MAX + c] = ia;
+    }
+}
+
+// one CTA per image: the slots summed / reduced in ascending CTA order, then the centroids, lmeqv and the clamped maxima
+template <typename T>
+__global__ void __launch_bounds__(64) k_part_head_finalize(const T* __restrict__ slots, const int32_t* __restrict__ slot_idx,
+                                                           T* __restrict__ stats, int32_t* __restrict__ idx,
+                                                           T* __restrict__ terms, int nslot, int kld) {
+    const int b = blockIdx.x, t = threadIdx.x;
+    __shared__ T tot[PH_SUMS];
+    const T* sl = slots + (size_t)b * nslot * PH_SLOT;
+    T* st = stats + (size_t)b * PH_STATS;
+    if (t < PH_SUMS) {
+        T a = 0;
+        for (int k = 0; k < nslot; ++k) a += sl[(size_t)k * PH_SLOT + t];
+        tot[t] = a;
+    } else if (t >= 32 && t < 32 + PH_MAX) {
+        const int c = t - 32;
+        const int32_t* si = slot_idx + (size_t)b * nslot * PH_MAX;
+        T a = sl[PH_SUMS + c];
+        int ia = si[c];
+        for (int k = 1; k < nslot; ++k) {
+            const T o = sl[(size_t)k * PH_SLOT + PH_SUMS + c];
+            const int oi = si[(size_t)k * PH_MAX + c];
+            if (ph_beats(o, oi, a, ia)) { a = o; ia = oi; }
+        }
+        const T clamped = a < T(1e-5) ? T(1e-5) : a;   // clamp_min keeps a NaN
+        if (c < 5) {
+            st[20 + c] = clamped;
+            st[30 + c] = a;
+            idx[(size_t)b * PH_IDX + c] = ia;
+        } else {
+            st[25 + c - 5] = clamped;
+        }
+    }
+    __syncthreads();
+    if (t == 0) {
+        T L = 0;
+        for (int c = 0; c < 4; ++c) {
+            const T z = tot[3 * c], zq = tot[12 + 3 * c];
+            st[c] = z;
+            for (int d = 0; d < 2; ++d) {
+                const T cc = tot[3 * c + 1 + d] / z, cq = tot[12 + 3 * c + 1 + d] / zq;
+                st[4 + 2 * c + d] = cc;
+                st[12 + 2 * c + d] = cq;
+                L += (cc - cq) * (cc - cq);
+            }
+        }
+        terms[2 * b] = L;
+        if (kld) terms[2 * b + 1] = tot[24];
+    }
+}
+
+// mse: E and G_1..G_4 partials once the maxima are known
+template <typename T>
+__global__ void __launch_bounds__(PH_THREADS) k_part_head_mse(const PartHeadIn<T> in, const T* __restrict__ w,
+                                                              const T* __restrict__ stats, T* __restrict__ slots, int H) {
+    const int b = blockIdx.y;
+    const int64_t HW = (int64_t)H * H;
+    const int begin = blockIdx.x * PH_PER_CTA;
+    const int end = (int)min(HW, (int64_t)begin + PH_PER_CTA);
+    const T* st = stats + (size_t)b * PH_STATS;
+    T mp[5], mq[5], wc[5], acc[PH_MSE];
+#pragma unroll
+    for (int c = 0; c < 5; ++c) { mp[c] = st[20 + c]; mq[c] = st[25 + c]; wc[c] = __ldg(w + c); acc[c] = 0; }
+    for (int p = begin + threadIdx.x; p < end; p += PH_THREADS) {
+        T v[5], q[5];
+        ph_load(in, b, HW, p, v, q);
+#pragma unroll
+        for (int c = 0; c < 5; ++c) {
+            const T d = v[c] / mp[c] - q[c] / mq[c];
+            acc[0] += (d * d) * wc[c];
+            if (c > 0) acc[c] += d * v[c];
+        }
+    }
+    __shared__ T s[PH_THREADS / 32][PH_MSE];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < PH_MSE; ++k) {
+        const T t = warp_sum(acc[k]);
+        if (lane == 0) s[warp][k] = t;
+    }
+    __syncthreads();
+    if (threadIdx.x < PH_MSE) {
+        T tot = 0;
+        for (int w2 = 0; w2 < PH_THREADS / 32; ++w2) tot += s[w2][threadIdx.x];
+        slots[((size_t)b * gridDim.x + blockIdx.x) * PH_SLOT + PH_SUMS + PH_MAX + threadIdx.x] = tot;
+    }
+}
+template <typename T>
+__global__ void __launch_bounds__(32) k_part_head_mse_finalize(const T* __restrict__ slots, T* __restrict__ stats,
+                                                               T* __restrict__ terms, int nslot) {
+    const int b = blockIdx.x, t = threadIdx.x;
+    if (t >= PH_MSE) return;
+    const T* sl = slots + (size_t)b * nslot * PH_SLOT + PH_SUMS + PH_MAX + t;
+    T a = 0;
+    for (int k = 0; k < nslot; ++k) a += sl[(size_t)k * PH_SLOT];
+    if (t == 0) terms[2 * b + 1] = a;
+    else stats[(size_t)b * PH_STATS + 35 + t] = a;
+}
+
+// grad_maps [B,4,HW] from the per-image adjoints grad_terms [B,2]
+template <typename T>
+__global__ void __launch_bounds__(256) k_part_head_bwd(const PartHeadIn<T> in, const T* __restrict__ w,
+                                                       const T* __restrict__ stats, const int32_t* __restrict__ idx,
+                                                       const T* __restrict__ gterms, T* __restrict__ gmaps, int H, int kld) {
+    const int b = blockIdx.y;
+    const int64_t HW = (int64_t)H * H;
+    const T* st = stats + (size_t)b * PH_STATS;
+    const T aL = __ldg(gterms + 2 * b), aE = __ldg(gterms + 2 * b + 1);
+    T cx[4], cy[4], kx[4], ky[4], kd[4], km[4], wc[4], mp[4];
+    int im[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        const T z = st[c];
+        cx[c] = st[4 + 2 * c];
+        cy[c] = st[5 + 2 * c];
+        kx[c] = aL * (T(2) * (cx[c] - st[12 + 2 * c])) / z;   // d terms[0] / d m_c = aL * 2 (C - CQ) . (xy - C) / Z_c
+        ky[c] = aL * (T(2) * (cy[c] - st[13 + 2 * c])) / z;
+        mp[c] = st[21 + c];
+        wc[c] = __ldg(w + 1 + c);
+        kd[c] = aE * T(2) * wc[c] / mp[c];
+        km[c] = st[31 + c] >= T(1e-5) ? aE * (T(-2) * wc[c] * st[36 + c] / (mp[c] * mp[c])) : T(0);  // clamped: none
+        im[c] = idx[(size_t)b * PH_IDX + 1 + c];
+    }
+    T mq[4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) mq[c] = st[26 + c];
+    T* gb = gmaps + (size_t)b * 4 * HW;
+    for (int64_t pp = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pp < HW; pp += (int64_t)gridDim.x * blockDim.x) {
+        const int p = (int)pp;
+        const int i = p / H, j = p - i * H;
+        const T x = ph_coord<T>(j, H), y = ph_coord<T>(i, H);
+        T v[5], q[5], s[5], mx, sum;
+        ph_load(in, b, HW, p, v, q);
+        ph_softmax(v, s, mx, sum);
+        T gs[4], dot = 0;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            gs[c] = kx[c] * (x - cx[c]) + ky[c] * (y - cy[c]);
+            dot += s[c + 1] * gs[c];
+        }
+        T r[5], rsum = 0;
+        if (kld) {
+            T qmx, qsum;
+            ph_softmax(q, r, qmx, qsum);
+#pragma unroll
+            for (int c = 0; c < 5; ++c) rsum += r[c];
+        }
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            T g = s[c + 1] * (gs[c] - dot);
+            if (kld) {
+                g += aE * (s[c + 1] * rsum - r[c + 1]);
+            } else {
+                g += kd[c] * (v[c + 1] / mp[c] - q[c + 1] / mq[c]);
+                if (p == im[c]) g += km[c];
+            }
+            gb[(size_t)c * HW + p] = g;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Host launchers shared by the deterministic float32 entry points (losses.cu) and the float64 ones (losses_f64.cu).
 // Each validates as both entry points do; where their checks differ, the entry points check and call the launcher.
 // ---------------------------------------------------------------------------------------------
@@ -802,5 +1116,87 @@ static int loss_head_backward(const T* rgba, const T* gt, const T* mask_gt, cons
                                                                       T(1) / (T(3) * (T)HW), w_iou, w_tex);
     return (int)cudaGetLastError();
 }
+
+// part_matching_loss head.  Workspace: stats [B][PH_STATS] T | slots [B][nslot][PH_SLOT] T | idx [B][PH_IDX] int32 |
+// slot indices [B][nslot][PH_MAX] int32.  The forward fills it; the backward reads stats and idx.
+static inline bool ph_too_large(int32_t B, int32_t H) { return B > 65535 || (int64_t)H * H > INT_MAX; }
+static inline int64_t ph_slots(int32_t H) { return ((int64_t)H * H + PH_PER_CTA - 1) / PH_PER_CTA; }
+template <typename T>
+static size_t part_head_workspace_bytes(int32_t B, int32_t H) {
+    if (B <= 0 || H <= 0 || ph_too_large(B, H)) return 0;
+    const int64_t ns = ph_slots(H);
+    return (size_t)B * ((size_t)(ns + 1) * PH_STATS * sizeof(T) + (size_t)(PH_IDX + ns * PH_MAX) * sizeof(int32_t));
+}
+template <typename T>
+static bool ph_misaligned(const void* p) { return ((uintptr_t)p & (sizeof(T) - 1)) != 0; }
+// validates the arguments the forward and backward share and fills `in`
+template <typename T>
+static int part_head_check(const T* const* maps, const int64_t* map_bstrides, const T* c0, int64_t c0_bstride,
+                           const T* part_segs, int64_t segs_bstride, const T* weights, const void* workspace, int32_t B,
+                           int32_t H, int32_t kld, PartHeadIn<T>& in) {
+    if (!maps || !map_bstrides || !c0 || !part_segs || !weights || !workspace || B <= 0 || H <= 0 || (kld != 0 && kld != 1) ||
+        c0_bstride < 0 || segs_bstride < 0 || ph_misaligned<T>(c0) || ph_misaligned<T>(part_segs) ||
+        ph_misaligned<T>(weights) || ph_misaligned<T>(workspace))
+        return UMR_ERR_BAD_ARG;
+    for (int k = 0; k < 4; ++k) {
+        if (!maps[k] || map_bstrides[k] < 0 || ph_misaligned<T>(maps[k])) return UMR_ERR_BAD_ARG;
+        in.map[k] = maps[k];
+        in.map_bs[k] = map_bstrides[k];
+    }
+    if (ph_too_large(B, H)) return UMR_ERR_TOO_LARGE;
+    in.c0 = c0;
+    in.c0_bs = c0_bstride;
+    in.q = part_segs;
+    in.q_bs = segs_bstride;
+    return UMR_OK;
+}
+template <typename T>
+static int part_head_forward(const T* const* maps, const int64_t* map_bstrides, const T* c0, int64_t c0_bstride,
+                             const T* part_segs, int64_t segs_bstride, const T* weights, T* terms, int32_t B, int32_t H,
+                             int32_t kld, void* workspace, void* stream_) {
+    PartHeadIn<T> in;
+    if (!terms || ph_misaligned<T>(terms)) return UMR_ERR_BAD_ARG;
+    const int rc = part_head_check(maps, map_bstrides, c0, c0_bstride, part_segs, segs_bstride, weights, workspace, B, H, kld,
+                                   in);
+    if (rc != UMR_OK) return rc;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const int ns = (int)ph_slots(H);
+    T* stats = (T*)workspace;
+    T* slots = stats + (size_t)B * PH_STATS;
+    int32_t* idx = (int32_t*)(slots + (size_t)B * ns * PH_SLOT);
+    int32_t* slot_idx = idx + (size_t)B * PH_IDX;
+    count_launch(kld ? 2 : 4);
+    k_part_head_partial<T><<<dim3(ns, B), PH_THREADS, 0, st>>>(in, slots, slot_idx, H, kld);
+    k_part_head_finalize<T><<<B, 64, 0, st>>>(slots, slot_idx, stats, idx, terms, ns, kld);
+    if (!kld) {
+        k_part_head_mse<T><<<dim3(ns, B), PH_THREADS, 0, st>>>(in, weights, stats, slots, H);
+        k_part_head_mse_finalize<T><<<B, 32, 0, st>>>(slots, stats, terms, ns);
+    }
+    return (int)cudaGetLastError();
+}
+template <typename T>
+static int part_head_backward(const T* const* maps, const int64_t* map_bstrides, const T* c0, int64_t c0_bstride,
+                              const T* part_segs, int64_t segs_bstride, const T* weights, const void* workspace,
+                              const T* grad_terms, T* grad_maps, int32_t B, int32_t H, int32_t kld, void* stream_) {
+    PartHeadIn<T> in;
+    if (!grad_terms || !grad_maps || ph_misaligned<T>(grad_terms) || ph_misaligned<T>(grad_maps)) return UMR_ERR_BAD_ARG;
+    const int rc = part_head_check(maps, map_bstrides, c0, c0_bstride, part_segs, segs_bstride, weights, workspace, B, H, kld,
+                                   in);
+    if (rc != UMR_OK) return rc;
+    const int64_t HW = (int64_t)H * H;
+    const T* stats = (const T*)workspace;
+    const int32_t* idx = (const int32_t*)(stats + (size_t)B * PH_STATS + (size_t)B * ph_slots(H) * PH_SLOT);
+    const unsigned gx = (unsigned)std::min<int64_t>((HW + 255) / 256, 1024);
+    count_launch();
+    k_part_head_bwd<T><<<dim3(gx, B), 256, 0, (cudaStream_t)stream_>>>(in, weights, stats, idx, grad_terms, grad_maps, H, kld);
+    return (int)cudaGetLastError();
+}
+// losses_f64.cu: the double instantiations, reached through the dtype argument of the entry points in losses.cu
+int part_head_forward_f64(const void* const* maps, const int64_t* map_bstrides, const void* c0, int64_t c0_bstride,
+                          const void* part_segs, int64_t segs_bstride, const void* weights, void* terms, int32_t B, int32_t H,
+                          int32_t kld, void* workspace, void* stream_);
+int part_head_backward_f64(const void* const* maps, const int64_t* map_bstrides, const void* c0, int64_t c0_bstride,
+                           const void* part_segs, int64_t segs_bstride, const void* weights, const void* workspace,
+                           const void* grad_terms, void* grad_maps, int32_t B, int32_t H, int32_t kld, void* stream_);
 
 }  // namespace umr

@@ -125,3 +125,19 @@ extern "C" int umr_texcycle_backward_f64(const double* flow, const double* prob,
     if (B > 65535 || (int64_t)B * F > INT_MAX) return UMR_ERR_TOO_LARGE;
     return texcycle_backward(flow, prob, visible, grad_loss, grad_flow, B, F, T2, stream_);
 }
+
+// the double half of umr_part_head_forward / _backward (losses.cu), instantiated in this -fmad=false unit
+int umr::part_head_forward_f64(const void* const* maps, const int64_t* map_bstrides, const void* c0, int64_t c0_bstride,
+                               const void* part_segs, int64_t segs_bstride, const void* weights, void* terms, int32_t B,
+                               int32_t H, int32_t kld, void* workspace, void* stream_) {
+    return part_head_forward(reinterpret_cast<const double* const*>(maps), map_bstrides, (const double*)c0, c0_bstride,
+                             (const double*)part_segs, segs_bstride, (const double*)weights, (double*)terms, B, H, kld,
+                             workspace, stream_);
+}
+int umr::part_head_backward_f64(const void* const* maps, const int64_t* map_bstrides, const void* c0, int64_t c0_bstride,
+                                const void* part_segs, int64_t segs_bstride, const void* weights, const void* workspace,
+                                const void* grad_terms, void* grad_maps, int32_t B, int32_t H, int32_t kld, void* stream_) {
+    return part_head_backward(reinterpret_cast<const double* const*>(maps), map_bstrides, (const double*)c0, c0_bstride,
+                              (const double*)part_segs, segs_bstride, (const double*)weights, workspace,
+                              (const double*)grad_terms, (double*)grad_maps, B, H, kld, stream_);
+}

@@ -475,31 +475,66 @@ class part_matching_loss(nn.Module):
             for stex in (self.stex1, self.stex2, self.stex3, self.stex4):
                 p, _, _ = self.renderer(verts, faces, cams, stex[:bs])
                 projs.append(torch.mean(p[:, 0:3, :, :], dim=1).unsqueeze(1))
-        proj = torch.cat([self.proj[:bs].detach()] + projs, dim=1)
-        centers_proj = batch_get_centers(nn.Softmax(dim=1)(proj)[:, 1:, :, :])
-        centers_parts = batch_get_centers(nn.Softmax(dim=1)(part_segs)[:, 1:, :, :])
+        return self.head(projs, part_segs, cam_probs, avg), projs
+
+    def head(self, projs, part_segs, cam_probs=None, avg=True):
+        """The loss from the four part maps `projs` ([B,1,H,W] each): the part-head kernels when every input is on the GPU,
+        the maps are square, `part_segs` is data and B <= 65535 (DESIGN.md §13), else the torch composition."""
+        c0 = self.proj[:projs[0].size(0)].detach()
+        kld = self.loss_type in "kld"
+        if not part_head_on_device(projs, c0, part_segs):
+            return part_head_torch(projs, c0, part_segs, self.weights, kld, cam_probs, avg)
+        bs, hw = part_segs.size(0), part_segs.size(2) * part_segs.size(3)
+        terms = ops.part_matching_head(projs, c0, part_segs, self.weights, kld)
         if avg:
-            loss_lmeqv = torch.nn.functional.mse_loss(centers_proj, centers_parts)
+            loss_lmeqv = terms[:, 0].sum() / (bs * 8)
         else:
-            loss_lmeqv = torch.nn.functional.mse_loss(centers_proj, centers_parts, reduction="none")
-            loss_lmeqv = torch.sum(loss_lmeqv, dim=(1, 2)) / (loss_lmeqv.size(1) * loss_lmeqv.size(2))
-            loss_lmeqv = (loss_lmeqv.view(cam_probs.size()) * cam_probs).sum(dim=1).mean()
-        if self.loss_type in "kld":
-            loss_eqv = self.kl(torch.nn.functional.log_softmax(proj, dim=1),
-                               torch.nn.functional.softmax(part_segs, dim=1))
+            loss_lmeqv = ((terms[:, 0] / 8).view(cam_probs.size()) * cam_probs).sum(dim=1).mean()
+        if kld:
+            loss_eqv = terms[:, 1].sum() / bs
+        elif avg:
+            loss_eqv = terms[:, 1].sum() / (bs * 5 * hw)
         else:
-            max_proj, _ = torch.max(proj.view(bs, 5, -1), dim=2)
-            max_proj = max_proj.clamp_min(1e-5)
-            proj_norm = proj / max_proj.view(bs, 5, 1, 1)
-            max_part, _ = torch.max(part_segs.view(bs, 5, -1), dim=2)
-            max_part = max_part.clamp_min(1e-5)
-            part_norm = part_segs / max_part.view(bs, 5, 1, 1)
-            if avg:
-                loss_eqv = torch.mean(nn.MSELoss(reduction="none")(proj_norm, part_norm) * self.weights)
-            else:
-                _, cs, iis, _ = part_norm.size()
-                loss_eqv = nn.MSELoss(reduction="none")(proj_norm, part_norm) * self.weights
-                loss_eqv = torch.sum(loss_eqv, dim=(1, 2, 3)) / (cs * iis * iis)
-                loss_eqv = (loss_eqv.view(cam_probs.size()) * cam_probs).sum(dim=1).mean()
-        total_loss = loss_eqv + loss_lmeqv
-        return total_loss / 4.0, projs
+            loss_eqv = ((terms[:, 1] / (5 * hw)).view(cam_probs.size()) * cam_probs).sum(dim=1).mean()
+        return (loss_eqv + loss_lmeqv) / 4.0
+
+
+def part_head_on_device(projs, c0, part_segs):
+    """Whether part_matching_loss's head runs on the part-head kernels: every input on the GPU, square maps, a
+    `part_segs` that needs no gradient (the kernels differentiate the part maps only) and B <= 65535."""
+    return (all(t.is_cuda for t in projs) and c0.is_cuda and part_segs.is_cuda and not part_segs.requires_grad
+            and part_segs.dim() == 4 and part_segs.size(2) == part_segs.size(3) and part_segs.size(0) <= 65535)
+
+
+def part_head_torch(projs, c0, part_segs, weights, kld, cam_probs=None, avg=True):
+    """part_matching_loss's head as torch ops (loss_utils.py:401-440, scops_utils.py:37-54): the path of CPU tensors,
+    non-square maps and a differentiable `part_segs`, and the reference the part-head kernels are tested against."""
+    bs = part_segs.size(0)
+    proj = torch.cat([c0] + list(projs), dim=1)
+    centers_proj = batch_get_centers(nn.Softmax(dim=1)(proj)[:, 1:, :, :])
+    centers_parts = batch_get_centers(nn.Softmax(dim=1)(part_segs)[:, 1:, :, :])
+    if avg:
+        loss_lmeqv = torch.nn.functional.mse_loss(centers_proj, centers_parts)
+    else:
+        loss_lmeqv = torch.nn.functional.mse_loss(centers_proj, centers_parts, reduction="none")
+        loss_lmeqv = torch.sum(loss_lmeqv, dim=(1, 2)) / (loss_lmeqv.size(1) * loss_lmeqv.size(2))
+        loss_lmeqv = (loss_lmeqv.view(cam_probs.size()) * cam_probs).sum(dim=1).mean()
+    if kld:
+        loss_eqv = torch.nn.functional.kl_div(torch.nn.functional.log_softmax(proj, dim=1),
+                                              torch.nn.functional.softmax(part_segs, dim=1), reduction="batchmean")
+    else:
+        max_proj, _ = torch.max(proj.view(bs, 5, -1), dim=2)
+        max_proj = max_proj.clamp_min(1e-5)
+        proj_norm = proj / max_proj.view(bs, 5, 1, 1)
+        max_part, _ = torch.max(part_segs.view(bs, 5, -1), dim=2)
+        max_part = max_part.clamp_min(1e-5)
+        part_norm = part_segs / max_part.view(bs, 5, 1, 1)
+        if avg:
+            loss_eqv = torch.mean(nn.MSELoss(reduction="none")(proj_norm, part_norm) * weights)
+        else:
+            _, cs, iis, _ = part_norm.size()
+            loss_eqv = nn.MSELoss(reduction="none")(proj_norm, part_norm) * weights
+            loss_eqv = torch.sum(loss_eqv, dim=(1, 2, 3)) / (cs * iis * iis)
+            loss_eqv = (loss_eqv.view(cam_probs.size()) * cam_probs).sum(dim=1).mean()
+    total_loss = loss_eqv + loss_lmeqv
+    return total_loss / 4.0

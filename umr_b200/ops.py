@@ -594,7 +594,82 @@ def corr_chamfer(verts, cams, selection, targets, part_ends, weights, vert_table
     return CorrChamferFunction.apply(verts, cams, selection, *targets, part_ends, weights, *vert_table)
 
 
-_VOXEL_DTYPES = {torch.float32: 0, torch.float64: 1}  # UMR_DTYPE_FLOAT32 / UMR_DTYPE_FLOAT64
+_DTYPE_IDS = {torch.float32: 0, torch.float64: 1}  # UMR_DTYPE_FLOAT32 / UMR_DTYPE_FLOAT64
+
+
+# -------------------------------------------------------------------------------------------------
+# part_matching_loss head (nnutils/loss_utils.py part_matching_loss after its render)
+# -------------------------------------------------------------------------------------------------
+def _planes(t, inner, dtype):
+    """(tensor, batch stride) of `t` [B, ...] read in place when each image is dense, in `dtype` and aligned to its element
+    size (the library refuses a misaligned pointer), else a contiguous copy."""
+    v, bs = _batch_view(t.detach(), inner, dtype)
+    if v.data_ptr() % v.element_size():
+        v, bs = v.contiguous().clone(), inner
+    return v, bs
+
+
+class PartMatchingHeadFunction(torch.autograd.Function):
+    """The head of part_matching_loss (DESIGN.md §13).  Part maps P_1..P_4 (each [B,H,H] dense per image: [B,1,H,H]
+    tensors or channels of a render, read in place), c0 [B,H,H] (channel 0 of proj), part_segs [B,5,H,H], weights (5
+    values), kld -> per-image terms [B,2]: (sum of the 8 squared centroid differences, the weighted squared-difference sum
+    of the max-normalised maps, or for kld the KL sum).  Gradients reach the four maps; c0, part_segs and weights are
+    data.  Forward: 4 launches (mse) or 2 (kld); backward: 1."""
+
+    @staticmethod
+    def forward(ctx, p1, p2, p3, p4, c0, part_segs, weights, kld):
+        maps = (p1, p2, p3, p4)
+        _need_cuda(*maps, c0, part_segs, weights)
+        B, C, H, W = part_segs.shape
+        if C != 5 or H != W:
+            raise ValueError("part_matching_head: part_segs must be [B,5,H,H], got %s" % (tuple(part_segs.shape),))
+        for t in maps + (c0,):
+            if t.shape[0] != B or t[0].numel() != H * W:
+                raise ValueError("part_matching_head: part maps and c0 must hold [B,%d,%d] values, got %s"
+                                 % (H, W, tuple(t.shape)))
+        if weights.numel() != 5:
+            raise ValueError("part_matching_head: 5 weights expected, got %d" % weights.numel())
+        m = KernelMode(_is_f64(*maps, c0, part_segs, weights))
+        planes = [_planes(t, H * W, m.dtype) for t in maps]
+        cz, cbs = _planes(c0, H * W, m.dtype)
+        q, qbs = _planes(part_segs, 5 * H * W, m.dtype)
+        w = _as(weights.reshape(-1), m)
+        kld = 1 if kld else 0
+        with torch.cuda.device(q.device):
+            terms = torch.empty(B, 2, device=q.device, dtype=m.dtype)
+            lib, dt = _lib.load(), _DTYPE_IDS[m.dtype]
+            ws = torch.empty(lib.umr_part_head_workspace_bytes(B, H, dt), device=q.device, dtype=torch.uint8)
+            mp = (ctypes.c_void_p * 4)(*[v.data_ptr() for v, _ in planes])
+            mb = (ctypes.c_int64 * 4)(*[bs for _, bs in planes])
+            _lib.check(lib.umr_part_head_forward(mp, mb, _ptr(cz), cbs, _ptr(q), qbs, _ptr(w), _ptr(terms), B, H, kld, dt,
+                                                 _ptr(ws), _stream_ptr(q.device)), "umr_part_head_forward")
+        ctx.inputs = (planes, cz, cbs, q, qbs, w, ws, kld, [(t.shape, t.dtype) for t in maps])
+        ctx.mode = m
+        return terms
+
+    @staticmethod
+    def backward(ctx, grad_terms):
+        m = ctx.mode
+        planes, cz, cbs, q, qbs, w, ws, kld, metas = ctx.inputs
+        B, _, H, W = q.shape
+        g = grad_terms.contiguous().to(m.dtype)
+        with torch.cuda.device(q.device):
+            gm = torch.empty(B, 4, H, W, device=q.device, dtype=m.dtype)
+            mp = (ctypes.c_void_p * 4)(*[v.data_ptr() for v, _ in planes])
+            mb = (ctypes.c_int64 * 4)(*[bs for _, bs in planes])
+            _lib.check(_lib.load().umr_part_head_backward(mp, mb, _ptr(cz), cbs, _ptr(q), qbs, _ptr(w), _ptr(ws), _ptr(g),
+                                                          _ptr(gm), B, H, kld, _DTYPE_IDS[m.dtype], _stream_ptr(q.device)),
+                       "umr_part_head_backward")
+        grads = tuple(gm[:, k].reshape(shape).to(dtype) if ctx.needs_input_grad[k] else None
+                      for k, (shape, dtype) in enumerate(metas))
+        return grads + (None,) * 4
+
+
+def part_matching_head(maps, c0, part_segs, weights, kld):
+    """-> terms [B,2] of the part_matching_loss head; see PartMatchingHeadFunction."""
+    return PartMatchingHeadFunction.apply(*maps, c0, part_segs, weights, bool(kld))
+
+
 _voxel_status = {}  # device -> the status word of the last voxelize call on that device
 
 
@@ -607,14 +682,14 @@ def voxelize(faces, size, normalize=False):
     if size < 1:
         raise ValueError("voxelize: size must be >= 1, got %d" % size)
     _need_cuda(faces)
-    if faces.dtype not in _VOXEL_DTYPES:
+    if faces.dtype not in _DTYPE_IDS:
         raise TypeError("voxelize: faces must be float32 or float64, got %s" % faces.dtype)
     if faces.dim() != 4 or faces.shape[2:] != (3, 3):
         raise ValueError("voxelize: faces must be [B, F, 3, 3], got %s" % (tuple(faces.shape),))
     lib = _lib.load()
     f = faces.detach().contiguous()
     B, F_ = f.shape[0], f.shape[1]
-    dtype, scale = _VOXEL_DTYPES[f.dtype], 1.0 if normalize else float(size)
+    dtype, scale = _DTYPE_IDS[f.dtype], 1.0 if normalize else float(size)
     nbytes = lib.umr_voxelize_workspace_bytes(B, size)
     if nbytes == 0:  # sizes the library refuses: it checks them before the buffers, so let it say which
         _lib.check(lib.umr_voxelize(_ptr(f), dtype, None, B, F_, size, scale, None, None), "umr_voxelize")
