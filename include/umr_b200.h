@@ -18,6 +18,8 @@
  *   umr_corr_chamfer_forward / _backward replace nnutils/loss_utils.py:218-248 (`CorrLossChamfer.forward`).
  *   umr_nmr_forward / umr_nmr_backward_textures replace the render of `neural_renderer.Renderer` (driven by
  *       nnutils/nmr_pytorch.py; the upstream package is not vendored, its contract is DESIGN.md §7).
+ *   umr_nmr_backward_faces adds NMR's approximate geometry gradient for the functional `neural_renderer.rasterize*`
+ *       (DESIGN.md §14).
  *
  * Conventions: plain device pointers + sizes, no torch types.  Every buffer is CALLER-allocated
  * (torch owns all memory); the library keeps no global mutable state and is re-entrant across host
@@ -447,6 +449,32 @@ int umr_nmr_forward(const float* vertices, const int32_t* faces, const float* te
 int umr_nmr_backward_textures(const float* vertices, const int32_t* faces, const int32_t* face_index,
                               const float* grad_rgb, float* grad_textures, const UmrNmrParams* params, void* workspace,
                               void* stream);
+/* Geometry gradient of the functional rasteriser (neural_renderer.rasterize*, DESIGN.md §14): NMR's approximate edge
+ * gradient (Kato et al., CVPR 2018, §3) for rgb and alpha plus the analytic depth gradient, in raster pixel units at
+ * S = is * (anti_aliasing ? 2 : 1).  Arguments are the forward's (vertices, faces, params, face_index; textures when
+ * grad_rgb is given) and the output adjoints grad_rgb [B,3,is,is], grad_alpha / grad_depth [B,is,is], each NULL when
+ * that output has none.  grad_face_vertices [B,F,3,3] (the gradient of face f's three vertices, in its own corner order)
+ * is fully written.
+ *   - Edge term, for every face that is front-facing under the forward's test and has finite coordinates: for each edge
+ *     (a, b, o) = (e, e+1, e+2) mod 3, axis 0 (columns d0, moving y) and axis 1 (rows d0, moving x), and each integer
+ *     d0 the edge spans inside the image: the line crosses the edge at vc; pixel `in` = floor / ceil(vc) on the inner
+ *     side, `out` = in + dir.  When `in` is this face's, every pixel from `out` to the border is compared with `in`;
+ *     every pixel of this face from `in` to the face's other edge is compared with `out`.  diff = sum over the given
+ *     channels (alpha, then rgb) of (I_p - I_ref) * g_p; a term with diff > 0 adds -diff / dist to the moving coordinate
+ *     of a and of b, dist the vertex displacement that moves the edge onto p (in NDC, moved away from 0 by eps).
+ *   - Depth term: at every pixel this face wins, d zp / d (x, y, z) of its three vertices, zp = 1 / sum w_l / z_l.
+ * Gradients are summed per face by one warp in a fixed order (no atomics): bitwise reproducible in every mode.
+ * workspace: umr_nmr_backward_faces_workspace_bytes(B, F, is, aa) bytes, 256-byte aligned.  Refusals as
+ * umr_nmr_forward; also UMR_ERR_BAD_ARG for NULL grad_face_vertices, grad_rgb without textures, a misaligned
+ * grad_face_vertices or eps negative or not finite, and UMR_ERR_UNSUPPORTED for fill_back or a non-zero directional
+ * light (the functional rasteriser renders one copy per face with light 1).  2 launches, 3 with grad_rgb. */
+size_t umr_nmr_backward_faces_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t image_size,
+                                              int32_t anti_aliasing);
+/* = align256(128 B F) + align256(16 B F) + align256(12 B S^2); 0 for the sizes the call refuses */
+int umr_nmr_backward_faces(const float* vertices, const int32_t* faces, const int32_t* face_index, const float* textures,
+                           const float* grad_rgb, const float* grad_alpha, const float* grad_depth,
+                           float* grad_face_vertices, const UmrNmrParams* params, float eps, void* workspace,
+                           void* stream);
 
 /* Mesh voxelisation: SoftRas `functional.voxelization` (functional/voxelization.py:41-58, kernels
  * cuda/voxelization_cuda_kernel.cu).  faces [B,F,3,3] (float32 or float64 as `dtype` says, contiguous; coordinates are

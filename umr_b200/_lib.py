@@ -138,6 +138,11 @@ EXPORTS = {
     "umr_nmr_forward": (ctypes.c_int, [c_f32p] * 8 + [ctypes.POINTER(UmrNmrParams), ctypes.c_void_p, ctypes.c_void_p]),
     "umr_nmr_backward_textures": (ctypes.c_int, [c_f32p] * 5 + [ctypes.POINTER(UmrNmrParams), ctypes.c_void_p,
                                                                 ctypes.c_void_p]),
+    # geometry gradient of the functional rasteriser: vertices, faces, face_index, textures, grad_rgb, grad_alpha,
+    # grad_depth, grad_face_vertices, params, eps, workspace, stream
+    "umr_nmr_backward_faces_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 4),
+    "umr_nmr_backward_faces": (ctypes.c_int, [c_f32p] * 8 + [ctypes.POINTER(UmrNmrParams), ctypes.c_float, ctypes.c_void_p,
+                                                             ctypes.c_void_p]),
     "umr_voxelize_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 2),
     "umr_voxelize": (ctypes.c_int, [c_f32p, ctypes.c_int32, c_f32p] + [ctypes.c_int32] * 3 + [ctypes.c_double, ctypes.c_void_p,
                                                                                            ctypes.c_void_p]),

@@ -11,6 +11,8 @@
 //   k_nmr_shade    thread = 4 output pixels: texture cube, light, background, vertical flip and the 2x2 pool fused,
 //                  128-bit stores.  The winner's barycentrics are recomputed with the z-buffer's exact op sequence.
 //   k_nmr_bwd_tex  thread = output pixel: the texture adjoint of k_nmr_shade, red.global into [B/G, F, T^3, 3].
+//   k_nmr_shade_raster / k_nmr_grad_faces  the functional rasteriser's geometry gradient (DESIGN.md §14): the raster-
+//                  resolution colour plane, then one warp per face for NMR's edge term and the depth term.
 //
 // Compiled with -fmad=false (umr_b200/build.py): every product and sum rounds once, in the contract's order.
 #include <cuda_runtime.h>
@@ -271,20 +273,9 @@ __global__ void __launch_bounds__(CTA) k_nmr_zbuf(const float* __restrict__ rec,
 // ---------------------------------------------------------------------------------------------
 // shading: texture, light, background, flip, pool
 // ---------------------------------------------------------------------------------------------
-// one raster pixel
-__device__ __forceinline__ void shade_px(const float* __restrict__ rec, const int32_t* __restrict__ face_index,
-                                         const float* __restrict__ rdepth, const float* __restrict__ textures,
-                                         const Consts& K, int b, int xi, int yi, float rgb[3], float& a, float& d) {
-    const size_t o = ((size_t)b * K.S + yi) * K.S + xi;
-    const int fi = __ldg(face_index + o);
-    d = __ldg(rdepth + o);
-    if (fi < 0) {
-        a = 0.f;
-        rgb[0] = K.bg[0]; rgb[1] = K.bg[1]; rgb[2] = K.bg[2];
-        return;
-    }
-    a = 1.f;
-    if (textures == nullptr) return;
+// colour of raster pixel (xi, yi) won by face copy fi >= 0
+__device__ __forceinline__ void shade_color(const float* __restrict__ rec, const float* __restrict__ textures,
+                                            const Consts& K, int b, int fi, int xi, int yi, float rgb[3]) {
     const float* rc = rec + ((size_t)b * K.Fc + fi) * REC;
     float w[3], zp;
     bary(rc, xi, yi, w, zp);
@@ -301,6 +292,23 @@ __device__ __forceinline__ void shade_px(const float* __restrict__ rec, const in
         s2 = s2 + wt * (__ldg(t + 2) * l2);
     });
     rgb[0] = s0; rgb[1] = s1; rgb[2] = s2;
+}
+
+// one raster pixel
+__device__ __forceinline__ void shade_px(const float* __restrict__ rec, const int32_t* __restrict__ face_index,
+                                         const float* __restrict__ rdepth, const float* __restrict__ textures,
+                                         const Consts& K, int b, int xi, int yi, float rgb[3], float& a, float& d) {
+    const size_t o = ((size_t)b * K.S + yi) * K.S + xi;
+    const int fi = __ldg(face_index + o);
+    d = __ldg(rdepth + o);
+    if (fi < 0) {
+        a = 0.f;
+        rgb[0] = K.bg[0]; rgb[1] = K.bg[1]; rgb[2] = K.bg[2];
+        return;
+    }
+    a = 1.f;
+    if (textures == nullptr) return;
+    shade_color(rec, textures, K, b, fi, xi, yi, rgb);
 }
 
 // V output pixels per thread (4: 128-bit stores).  rgb [B,3,is,is], alpha / depth [B,is,is]; any may be NULL.
@@ -468,6 +476,258 @@ __global__ void __launch_bounds__(DET_WARPS * 32) k_nmr_bwd_tex_det(const float*
 }
 
 // ---------------------------------------------------------------------------------------------
+// geometry gradient (DESIGN.md §14): NMR's approximate edge gradient plus the analytic depth gradient
+// ---------------------------------------------------------------------------------------------
+// raster-resolution colour plane [B,S,S,3] (background where no face wins), k_nmr_shade's op sequence per pixel
+__global__ void __launch_bounds__(256) k_nmr_shade_raster(const float* __restrict__ rec, const int32_t* __restrict__ face_index,
+                                                          const float* __restrict__ textures, float* __restrict__ color,
+                                                          Consts K) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t plane = (size_t)K.S * K.S;
+    if (t >= (size_t)K.B * plane) return;
+    const int b = (int)(t / plane), yi = (int)((t % plane) / K.S), xi = (int)(t % K.S);
+    const int fi = __ldg(face_index + t);
+    float c[3] = {K.bg[0], K.bg[1], K.bg[2]};
+    if (fi >= 0) shade_color(rec, textures, K, b, fi, xi, yi, c);
+    float* o = color + t * 3;
+    o[0] = c[0]; o[1] = c[1]; o[2] = c[2];
+}
+
+// The output-resolution adjoint planes read at raster pixel (xi, yi): flip, then the 2x2 pool's 1/4.
+struct GradPlanes {
+    const float* rgb;    // [B,3,is,is] or NULL
+    const float* alpha;  // [B,is,is] or NULL
+    const float* depth;  // [B,is,is] or NULL
+    const float* color;  // raster colour plane [B,S,S,3] (with rgb)
+    const int32_t* fidx; // [B,S,S]
+};
+
+__device__ __forceinline__ size_t out_index(const Consts& K, int b, int xi, int yi) {
+    const int r = K.aa ? (K.S - 1 - yi) >> 1 : K.S - 1 - yi;
+    const int c = K.aa ? xi >> 1 : xi;
+    return ((size_t)b * K.IS + r) * K.IS + c;
+}
+
+__device__ __forceinline__ float out_grad(const Consts& K, const float* g, size_t o) {
+    const float v = __ldg(g + o);
+    return K.aa ? v / 4.f : v;
+}
+
+// the channels the edge term compares: alpha, then rgb
+struct Px {
+    float a, c[3];
+};
+
+__device__ __forceinline__ Px px_value(const GradPlanes& G, const Consts& K, int b, int xi, int yi) {
+    const size_t o = ((size_t)b * K.S + yi) * K.S + xi;
+    Px v;
+    v.a = __ldg(G.fidx + o) >= 0 ? 1.f : 0.f;
+    if (G.rgb) {
+        v.c[0] = __ldg(G.color + o * 3); v.c[1] = __ldg(G.color + o * 3 + 1); v.c[2] = __ldg(G.color + o * 3 + 2);
+    } else {
+        v.c[0] = v.c[1] = v.c[2] = 0.f;
+    }
+    return v;
+}
+
+// diff = sum over the requested channels of (I_p - I_ref) * g_p, alpha first, then r, g, b
+__device__ __forceinline__ float edge_diff(const GradPlanes& G, const Consts& K, int b, int xi, int yi, const Px& ref) {
+    const Px p = px_value(G, K, b, xi, yi);
+    const size_t o = out_index(K, b, xi, yi);
+    const size_t plane = (size_t)K.IS * K.IS;
+    float diff = 0.f;
+    if (G.alpha) diff = diff + (p.a - ref.a) * out_grad(K, G.alpha, o);
+    if (G.rgb) {
+        const size_t oc = o + (size_t)b * 2 * plane;  // [B,3,is,is]: b * 3 * plane + ch * plane + pixel
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) diff = diff + (p.c[ch] - ref.c[ch]) * out_grad(K, G.rgb, oc + ch * plane);
+    }
+    return diff;
+}
+
+// One edge term at walk pixel d1 of line d0, skipped unless diff > 0: -diff / dist to the line's vertex a (ga) and b (gb),
+// dist moved away from zero by eps.
+__device__ __forceinline__ void edge_term(float& ga, float& gb, float diff, int d1, float vc, float ua, float ub, float d0f,
+                                          float Sf, float eps) {
+    if (!(diff > 0.f)) return;
+    const float dd = (float)d1 - vc;
+    if (ub != d0f) {
+        float dist = ((((ub - ua) / (ub - d0f)) * dd) * 2.f) / Sf;
+        dist = dist > 0.f ? dist + eps : dist - eps;
+        ga = ga - diff / dist;
+    }
+    if (ua != d0f) {
+        float dist = ((((ub - ua) / (d0f - ua)) * dd) * 2.f) / Sf;
+        dist = dist > 0.f ? dist + eps : dist - eps;
+        gb = gb - diff / dist;
+    }
+}
+
+__device__ __forceinline__ float sel3(const float a[3], int k) { return k == 0 ? a[0] : (k == 1 ? a[1] : a[2]); }
+
+// Line (e, axis, d0) of face f: the growing walk (only when the 'in' pixel is this face's) and the shrinking walk.
+// Returns the line's sums for the moving coordinate of vertex a = e (ga) and b = e + 1 (gb).
+__device__ __forceinline__ void edge_line(float& ga, float& gb, const GradPlanes& G, const Consts& K, int b, int f, const float px[3],
+                          const float py[3], int e, int axis, int d0, float eps) {
+    const int S = K.S;
+    const float Sf = (float)S, d0f = (float)d0;
+    const int ka = e, kb = e == 2 ? 0 : e + 1, ko = e == 0 ? 2 : e - 1;
+    const float ua = sel3(axis == 0 ? px : py, ka), ub = sel3(axis == 0 ? px : py, kb), uo = sel3(axis == 0 ? px : py, ko);
+    const float va = sel3(axis == 0 ? py : px, ka), vb = sel3(axis == 0 ? py : px, kb), vo = sel3(axis == 0 ? py : px, ko);
+    const int dir = axis == 0 ? (ua < ub ? -1 : 1) : (ua < ub ? 1 : -1);
+    const float vc = ((vb - va) / (ub - ua)) * (d0f - ua) + va;
+    const float fin = dir > 0 ? floorf(vc) : ceilf(vc);
+    if (!(fin >= 0.f && fin <= Sf - 1.f)) return;  // NaN included
+    const int in = (int)fin, out = in + dir;
+    if (out < 0 || out >= S) return;
+    // raster pixel of walk position d1: axis 0 walks a column (x = d0), axis 1 a row (y = d0)
+    const int step = axis == 0 ? S : 1;
+    const int base = axis == 0 ? d0 : d0 * S;
+    const size_t img = (size_t)b * S * S;
+    auto xy = [&](int d1, int& xi, int& yi) {
+        if (axis == 0) { xi = d0; yi = d1; } else { xi = d1; yi = d0; }
+    };
+    int xi, yi;
+    xy(in, xi, yi);
+    const Px I_in = px_value(G, K, b, xi, yi);
+    const bool in_is_f = __ldg(G.fidx + img + base + in * step) == f;
+    xy(out, xi, yi);
+    const Px I_out = px_value(G, K, b, xi, yi);
+    // growing: from 'out' to the border in direction dir, every pixel compared with I_in
+    if (in_is_f) {
+        const int p0 = dir > 0 ? out : 0, p1 = dir > 0 ? S - 1 : out;
+        for (int p = p0; p <= p1; ++p) {
+            xy(p, xi, yi);
+            edge_term(ga, gb, edge_diff(G, K, b, xi, yi, I_in), p, vc, ua, ub, d0f, Sf, eps);
+        }
+    }
+    // shrinking: from 'in' to where the line u = d0 meets the other edge (rounded outward), this face's pixels only
+    float x;
+    if ((d0f - ua) * (d0f - uo) < 0.f) x = ((vo - va) / (uo - ua)) * (d0f - ua) + va;
+    else x = ((vb - vo) / (ub - uo)) * (d0f - uo) + vo;
+    float lf = dir > 0 ? ceilf(x) : floorf(x);
+    lf = lf != lf ? fin : fminf(fmaxf(lf, -1.f), Sf);  // NaN: the 'in' pixel alone; clamped before the conversion
+    const int lim = (int)lf;
+    const int p0 = max(min(in, lim), 0), p1 = min(max(in, lim), S - 1);
+    for (int p = p0; p <= p1; ++p) {
+        if (__ldg(G.fidx + img + base + p * step) != f) continue;
+        xy(p, xi, yi);
+        edge_term(ga, gb, edge_diff(G, K, b, xi, yi, I_out), p, vc, ua, ub, d0f, Sf, eps);
+    }
+}
+
+// d0 range of (e, axis): [max(ceil(min u), 0), min(floor(max u), S-1)], empty when u_a == u_b
+__device__ __forceinline__ void line_range(const float px[3], const float py[3], int e, int axis, int S, int& lo, int& n) {
+    const float* U = axis == 0 ? px : py;
+    const float ua = U[e], ub = U[(e + 1) % 3];
+    lo = 0;
+    n = 0;
+    if (ua == ub) return;
+    const float l = fmaxf(ceilf(fminf(ua, ub)), 0.f), h = fminf(floorf(fmaxf(ua, ub)), (float)(S - 1));
+    if (l <= h) { lo = (int)l; n = (int)h - lo + 1; }
+}
+
+// One warp per (image, face), the only writer of that face's 9 gradient values.  Lane l takes lines l, l + 32, ... of
+// the face's (edge, axis, d0) lines in that order, then the depth pixels of its pixel box (rows ascending, 32-pixel
+// row segments); the 9 lane sums are reduced by a fixed xor-shuffle tree.  No atomics: bitwise reproducible.
+__global__ void __launch_bounds__(256) k_nmr_grad_faces(const float* __restrict__ rec, const int4* __restrict__ box,
+                                                        GradPlanes G, float* __restrict__ grad, float eps, Consts K) {
+    const int lane = threadIdx.x & 31;
+    const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (gw >= (long long)K.B * K.F) return;  // whole warps
+    const int b = (int)(gw / K.F), f = (int)(gw - (long long)b * K.F);
+    const float* rc = rec + ((size_t)b * K.Fc + f) * REC;
+    const int S = K.S;
+    const float Sf = (float)S;
+    float acc[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) acc[k] = 0.f;
+
+    if (G.rgb || G.alpha) {
+        float x[3], y[3];
+        bool finite = true;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            x[k] = __ldg(rc + R_X + 2 * k);
+            y[k] = __ldg(rc + R_X + 2 * k + 1);
+            finite = finite && isfinite(x[k]) && isfinite(y[k]) && isfinite(__ldg(rc + R_Z + k));
+        }
+        const bool back = (y[2] - y[0]) * (x[1] - x[0]) < (y[1] - y[0]) * (x[2] - x[0]);
+        if (finite && !back) {
+            float px[3], py[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                px[k] = 0.5f * ((x[k] * Sf + Sf) - 1.f);
+                py[k] = 0.5f * ((y[k] * Sf + Sf) - 1.f);
+            }
+            int lo[6], n[6], total = 0;
+#pragma unroll
+            for (int s = 0; s < 6; ++s) {
+                line_range(px, py, s >> 1, s & 1, S, lo[s], n[s]);
+                total += n[s];
+            }
+            for (int li = lane; li < total; li += 32) {
+                int s = 0, d0 = 0, r = li;
+                bool found = false;
+#pragma unroll
+                for (int q = 0; q < 6; ++q) {
+                    if (found) continue;
+                    if (r < n[q]) { found = true; s = q; d0 = lo[q] + r; } else { r -= n[q]; }
+                }
+                const int e = s >> 1, axis = s & 1;
+                float ga = 0.f, gb = 0.f;
+                edge_line(ga, gb, G, K, b, f, px, py, e, axis, d0, eps);
+                // the line moves y (axis 0) or x (axis 1) of vertices e and e + 1
+                const int ia = e * 3 + (axis == 0 ? 1 : 0), ib = (e == 2 ? 0 : e + 1) * 3 + (axis == 0 ? 1 : 0);
+#pragma unroll
+                for (int k = 0; k < 9; ++k) {
+                    if (k == ia) acc[k] = acc[k] + ga;
+                    if (k == ib) acc[k] = acc[k] + gb;
+                }
+            }
+        }
+    }
+
+    if (G.depth) {
+        const int4 bb = __ldg(box + (size_t)b * K.Fc + f);
+        const float z0 = __ldg(rc + R_Z), z1 = __ldg(rc + R_Z + 1), z2 = __ldg(rc + R_Z + 2);
+        const float half = 0.5f * Sf;
+        for (int yi = bb.z; yi <= bb.w; ++yi) {
+            for (int xs = bb.x; xs <= bb.y; xs += 32) {
+                const int xi = xs + lane;
+                if (xi > bb.y || __ldg(G.fidx + ((size_t)b * S + yi) * S + xi) != f) continue;
+                const float g = out_grad(K, G.depth, out_index(K, b, xi, yi));
+                if (g == 0.f) continue;
+                float w[3], zp;
+                bary(rc, xi, yi, w, zp);
+                const float a = (zp * zp) * g;
+                const float sx = (__ldg(rc + R_INV + 0) / z0 + __ldg(rc + R_INV + 3) / z1) + __ldg(rc + R_INV + 6) / z2;
+                const float sy = (__ldg(rc + R_INV + 1) / z0 + __ldg(rc + R_INV + 4) / z1) + __ldg(rc + R_INV + 7) / z2;
+                const float zk[3] = {z0, z1, z2};
+#pragma unroll
+                for (int k = 0; k < 3; ++k) {
+                    const float t = a * w[k];
+                    acc[3 * k] = acc[3 * k] + (t * sx) * half;
+                    acc[3 * k + 1] = acc[3 * k + 1] + (t * sy) * half;
+                    acc[3 * k + 2] = acc[3 * k + 2] + t / (zk[k] * zk[k]);
+                }
+            }
+        }
+    }
+
+#pragma unroll
+    for (int k = 0; k < 9; ++k) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) acc[k] = acc[k] + __shfl_xor_sync(0xffffffffu, acc[k], off);
+    }
+    if (lane == 0) {
+        float* o = grad + ((size_t)b * K.F + f) * 9;
+#pragma unroll
+        for (int k = 0; k < 9; ++k) o[k] = acc[k];
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
 static int check(const UmrNmrParams* p, bool need_tex) {
@@ -601,6 +861,48 @@ extern "C" int umr_nmr_backward_textures_deterministic(const float* vertices, co
     const long long nwarp = (long long)(K.B / K.tex_div) * K.F;
     k_nmr_bwd_tex_det<<<(unsigned)((nwarp + DET_WARPS - 1) / DET_WARPS), DET_WARPS * 32, 0, stream>>>(rec, box, face_index,
                                                                                                       grad_rgb, grad_textures, K);
+    umr::count_launch();
+    return (int)cudaGetLastError();
+}
+
+// Geometry gradient (include/umr_b200.h, DESIGN.md §14).  Workspace: the forward's record and box arrays, then the
+// raster colour plane [B,S,S,3].
+extern "C" size_t umr_nmr_backward_faces_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t image_size,
+                                                         int32_t anti_aliasing) {
+    if (batch_size <= 0 || num_faces <= 0 || image_size <= 0 || batch_size > 65535 || num_faces > (1 << 30)) return 0;
+    const long long S = (long long)image_size * (anti_aliasing ? 2 : 1);
+    if (S > 16384) return 0;
+    return rec_bytes(batch_size, num_faces) + box_bytes(batch_size, num_faces) +
+           align256((size_t)batch_size * (size_t)(S * S) * 3 * sizeof(float));
+}
+
+extern "C" int umr_nmr_backward_faces(const float* vertices, const int32_t* faces, const int32_t* face_index,
+                                      const float* textures, const float* grad_rgb, const float* grad_alpha,
+                                      const float* grad_depth, float* grad_face_vertices, const UmrNmrParams* p, float eps,
+                                      void* workspace, void* stream_) {
+    int rc = check(p, textures != nullptr);
+    if (rc) return rc;
+    if (!vertices || !faces || !face_index || !grad_face_vertices || !workspace) return UMR_ERR_BAD_ARG;
+    if (grad_rgb && !textures) return UMR_ERR_BAD_ARG;
+    if (((uintptr_t)workspace & 255) != 0 || ((uintptr_t)grad_face_vertices & 3) != 0) return UMR_ERR_BAD_ARG;
+    if (!(eps >= 0.f && eps < INFINITY)) return UMR_ERR_BAD_ARG;
+    // the functional rasteriser's configuration: one copy per face, light exactly 1 (no geometry-dependent shading)
+    if (p->fill_back || p->light_intensity_directional != 0.f) return UMR_ERR_UNSUPPORTED;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const Consts K = make_consts(p);
+    char* ws = (char*)workspace;
+    float* rec = (float*)ws;
+    int4* box = (int4*)(ws + rec_bytes(K.B, K.Fc));
+    float* color = (float*)(ws + rec_bytes(K.B, K.Fc) + box_bytes(K.B, K.Fc));
+    launch_prep(vertices, faces, rec, box, K, stream);
+    if (grad_rgb) {
+        const size_t n = (size_t)K.B * K.S * K.S;
+        k_nmr_shade_raster<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(rec, face_index, textures, color, K);
+        umr::count_launch();
+    }
+    GradPlanes G{grad_rgb, grad_alpha, grad_depth, color, face_index};
+    const long long nthr = (long long)K.B * K.F * 32;
+    k_nmr_grad_faces<<<(unsigned)((nthr + 255) / 256), 256, 0, stream>>>(rec, box, G, grad_face_vertices, eps, K);
     umr::count_launch();
     return (int)cudaGetLastError();
 }

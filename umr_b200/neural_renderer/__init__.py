@@ -27,7 +27,16 @@ anti-aliasing, else is.
 6. Texture gradient: light * w_pn * grad_rgb at the 8 texels of every covered raster pixel (back copies on the
    transposed texel), through the adjoint of the pool and the flip.
 Equivalence of this contract to the upstream package is not verified (its source is not available offline).
+
+The functional rasterisers (`rasterize_rgbad`, `rasterize`, `rasterize_silhouettes`, `rasterize_depth`,
+`vertices_to_faces`; rasterize.py) take face coordinates already in NDC and give them NMR's approximate geometry
+gradient (DESIGN.md §14).  `Renderer` keeps its texture-only gradient.
 """
+from .rasterize import (DEFAULT_ANTI_ALIASING, DEFAULT_BACKGROUND_COLOR, DEFAULT_EPS, DEFAULT_FAR, DEFAULT_IMAGE_SIZE,
+                        DEFAULT_NEAR, rasterize, rasterize_depth, rasterize_rgbad, rasterize_silhouettes,
+                        vertices_to_faces)
 from .renderer import Renderer
 
-__all__ = ["Renderer"]
+__all__ = ["Renderer", "rasterize_rgbad", "rasterize", "rasterize_silhouettes", "rasterize_depth", "vertices_to_faces",
+           "DEFAULT_IMAGE_SIZE", "DEFAULT_ANTI_ALIASING", "DEFAULT_NEAR", "DEFAULT_FAR", "DEFAULT_EPS",
+           "DEFAULT_BACKGROUND_COLOR"]
