@@ -44,10 +44,12 @@ inline double max(float a, double b) { return (double)a > b ? (double)a : b; }
 inline double max(double a, float b) { return a > (double)b ? a : (double)b; }
 inline double min(float a, double b) { return (double)a < b ? (double)a : b; }
 inline double min(double a, float b) { return a < (double)b ? a : (double)b; }
-inline float max(float a, float b) { return a > b ? a : b; }
-inline float min(float a, float b) { return a < b ? a : b; }
-inline double max(double a, double b) { return a > b ? a : b; }
-inline double min(double a, double b) { return a < b ? a : b; }
+// CUDA's max / min(float, float) and (double, double) are fmaxf / fminf and fmax / fmin (crt/math_functions.hpp): a NaN
+// operand is dropped, so kernel.cu:32-38 tests the box of a face's finite coordinates
+inline float max(float a, float b) { return std::fmax(a, b); }
+inline float min(float a, float b) { return std::fmin(a, b); }
+inline double max(double a, double b) { return std::fmax(a, b); }
+inline double min(double a, double b) { return std::fmin(a, b); }
 
 template <class T>
 inline T atomicAdd(T* p, T v) {

@@ -32,8 +32,9 @@ namespace {
 // mixed-precision select helpers: CUDA's max/min(float,double) return double (kernel.cu:56-57,143,259,584)
 template <class S> inline double dmax(S a, double b) { return (double)a > b ? (double)a : b; }
 template <class S> inline double dmin(S a, double b) { return (double)a < b ? (double)a : b; }
-template <class S> inline S smax(S a, S b) { return a > b ? a : b; }
-template <class S> inline S smin(S a, S b) { return a < b ? a : b; }
+// CUDA's max / min(S, S) at kernel.cu:32-38: fmax / fmin, which drop a NaN operand (the box of the finite coordinates)
+template <class S> inline S smax(S a, S b) { return std::fmax(a, b); }
+template <class S> inline S smin(S a, S b) { return std::fmin(a, b); }
 
 struct Params {
     int B, F, IS, T2, R;

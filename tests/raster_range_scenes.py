@@ -8,12 +8,22 @@ Box arithmetic (k_prep_f64 / k_prep, DESIGN.md §3):
   float32  the same in float32 (one IEEE operation each; the raster code is built with -fmad=false).
 The forward lists a face for a 16x16 tile when its box meets the tile's pixel-centre extents; k_raster_fwd_f64 tests
 faces in windows of WINDOW = 1024 and consumes its 2048-entry list before the last window only when more than 1024
-listed faces are waiting."""
+listed faces are waiting.
+
+The default float32 path (raster_stream.cuh, raster_fwd3.cuh, raster_fwd4.cuh, test_raster_fast_range_gpu.py): k_bin_coarse
+lists, per 64x64-pixel coarse bin (CB), the faces whose box meets the bin's pixel-centre extents, in ascending order;
+k_raster_fwd3 walks its bin's list in windows of LCAP = 512 entries, keeps the entries whose box meets its 16x16 tile (one
+tile-list segment per window) and reserves, per segment with a pair, popc(meet) pair blocks per listed face plus 2 header
+words, where meet holds the 8x4-pixel warp blocks whose columns and rows the box reaches (fwd3_blocks restates it).  A
+block holds the survivors of one face in one warp block: at most 32 records.  k_raster_fwd4 holds FWD4_CAP = 1536
+tile-list entries; a longer coarse list takes its windowed path.  The recompute fallback lists faces in windows of
+FACE_WINDOW = 65536."""
 import math
 
 import numpy as np
 
 TILE, WINDOW, LIST_CAP = 16, 1024, 2048
+CB, LCAP, FWD4_CAP, FACE_WINDOW = 64, 512, 1536, 65536
 # soft edges of the range scenes: r = 0.0096 (about a third of a pixel at S = 66)
 KW = dict(sigma_val=1e-5, dist_eps=1e-4, gamma_val=1e-3)
 
@@ -47,19 +57,21 @@ def pixel_centre(i, S, dtype):
 
 
 def boxes(fv, dtype, r=None):
-    """[..., 4] = xlo, xhi, ylo, yhi of every face, as k_prep(_f64) stores them (NaN propagates as the kernels' min/max do
-    for the NaN scenes here: a NaN vertex gives a NaN box)."""
+    """[..., 4] = xlo, xhi, ylo, yhi of every face, as k_prep(_f64) stores them: fmin / fmax drop a NaN coordinate, so a
+    face with a NaN vertex has the box of its finite coordinates (NaN only where all three are)."""
     fv = np.asarray(fv, dtype)
     r = cull_radius(dtype) if r is None else r
     x, y = fv[..., 0::3], fv[..., 1::3]
     with np.errstate(invalid="ignore"):
-        return np.stack([x.min(-1) - r, x.max(-1) + r, y.min(-1) - r, y.max(-1) + r], -1).astype(dtype)
+        return np.stack([np.fmin.reduce(x, -1) - r, np.fmax.reduce(x, -1) + r, np.fmin.reduce(y, -1) - r,
+                         np.fmax.reduce(y, -1) + r], -1).astype(dtype)
 
 
-def tile_hits(box, S, tx, ty, dtype):
-    """Faces whose box meets tile (tx, ty) (ty counts image rows from the top), as the forward's tile test decides."""
-    x0, x1 = pixel_centre(tx * TILE, S, dtype), pixel_centre(min(tx * TILE + TILE - 1, S - 1), S, dtype)
-    top, bot = pixel_centre(S - 1 - ty * TILE, S, dtype), pixel_centre(S - 1 - min(ty * TILE + TILE - 1, S - 1), S, dtype)
+def tile_hits(box, S, tx, ty, dtype, side=TILE):
+    """Faces whose box meets tile (tx, ty) of `side` pixels (ty counts image rows from the top), as the forward's tile
+    test (and, for side = CB, the coarse binning) decides."""
+    x0, x1 = pixel_centre(tx * side, S, dtype), pixel_centre(min(tx * side + side - 1, S - 1), S, dtype)
+    top, bot = pixel_centre(S - 1 - ty * side, S, dtype), pixel_centre(S - 1 - min(ty * side + side - 1, S - 1), S, dtype)
     return ~((x0 > box[..., 1]) | (x1 < box[..., 0]) | (bot > box[..., 3]) | (top < box[..., 2]))
 
 
@@ -79,6 +91,75 @@ def consumes(counts):
         out.append(n)
         n = 0
     return out
+
+
+def fwd3_segments(box, S, tx=0, ty=0, dtype=np.float32):
+    """k_raster_fwd3's tile-list segments of 16x16 tile (tx, ty): per LCAP window of its coarse bin's list, (listed
+    faces, pair blocks).  A face's blocks are popc(cm) * popc(rm): the 8-column halves and 4-row bands of the tile
+    holding a live pixel centre inside the face's box."""
+    cl = np.flatnonzero(tile_hits(box, S, tx * TILE // CB, ty * TILE // CB, dtype, CB))
+    ncol, nrow = min(TILE, S - tx * TILE), min(TILE, S - ty * TILE)
+    xs = pixel_centre(tx * TILE + np.arange(ncol), S, dtype)
+    ys = pixel_centre(S - 1 - (ty * TILE + np.arange(nrow)), S, dtype)
+    out = []
+    for w0 in range(0, len(cl), LCAP):
+        f = cl[w0:w0 + LCAP]
+        b = box[f[tile_hits(box[f], S, tx, ty, dtype)]]
+        with np.errstate(invalid="ignore"):
+            col = ~((xs[None] > b[:, 1:2]) | (xs[None] < b[:, 0:1]))
+            row = ~((ys[None] > b[:, 3:4]) | (ys[None] < b[:, 2:3]))
+        nc = col[:, :8].any(1).astype(int) + col[:, 8:].any(1)
+        nr = sum(row[:, 4 * k:4 * k + 4].any(1).astype(int) for k in range(4))
+        out.append((len(b), int((nc * nr).sum())))
+    return out
+
+
+def fwd3_blocks_wanted(fv, S, dtype=np.float32):
+    """The pair buffer's block cursor after a k_raster_fwd3 forward with room for every tile: per segment holding a
+    block, its blocks plus 2 header words."""
+    nt = (S + TILE - 1) // TILE
+    total = 0
+    for img in np.asarray(fv, dtype):
+        box = boxes(img, dtype)
+        for ty in range(nt):
+            for tx in range(nt):
+                total += sum(nb + 2 for _, nb in fwd3_segments(box, S, tx, ty, dtype) if nb > 0)
+    return total
+
+
+def survivors(fv, S, near=1.0, far=100.0, sigma_val=KW["sigma_val"], dist_eps=KW["dist_eps"]):
+    """[F, S, S] (image rows from the top): the (face, pixel) pairs the euclidean-distance forward keeps -- inside the
+    box, inside the triangle or nearer its edges than sqrt(thr), depth in (near, far) -- evaluated in double, with a
+    check that no pixel lies within 1e-6 (relative) of a decision."""
+    thr = float(np.float32(math.log(1.0 / dist_eps - 1.0)) * np.float32(sigma_val))
+    c = pixel_centre(np.arange(S), S, np.float64)
+    xp, yp = np.meshgrid(c, c[::-1])
+    out = []
+    for f in np.asarray(fv, np.float64):
+        v = f.reshape(3, 3)
+        box = boxes(f[None], np.float32)[0].astype(np.float64)
+        inbox = (xp >= box[0]) & (xp <= box[1]) & (yp >= box[2]) & (yp <= box[3])
+        d2 = np.full(xp.shape, np.inf)
+        for a, b in ((0, 1), (1, 2), (2, 0)):
+            e = v[b, :2] - v[a, :2]
+            t = np.clip(((xp - v[a, 0]) * e[0] + (yp - v[a, 1]) * e[1]) / (e @ e), 0, 1)
+            d2 = np.minimum(d2, (xp - v[a, 0] - t * e[0]) ** 2 + (yp - v[a, 1] - t * e[1]) ** 2)
+        det = (v[1, 0] - v[0, 0]) * (v[2, 1] - v[0, 1]) - (v[2, 0] - v[0, 0]) * (v[1, 1] - v[0, 1])
+        side = [((v[b, 0] - v[a, 0]) * (yp - v[a, 1]) - (v[b, 1] - v[a, 1]) * (xp - v[a, 0])) * np.sign(det)
+                for a, b in ((0, 1), (1, 2), (2, 0))]
+        inside = np.minimum(np.minimum(side[0], side[1]), side[2]) >= 0
+        assert not (inbox & ~inside & (np.abs(d2 - thr) < 1e-6 * thr)).any(), "a pixel on the distance cut-off"
+        z = v[:, 2]
+        assert near < z.min() and z.max() < far, "the depth test would decide pairs"
+        out.append(inbox & (inside | (d2 < thr)))
+    return np.array(out)
+
+
+def tile_records(fv, S, side=TILE):
+    """Saved records per tile of `side` pixels for one image's faces (survivors summed over faces and tile pixels)."""
+    s = survivors(fv, S).sum(0)
+    nt = (S + side - 1) // side
+    return np.array([[int(s[ty * side:(ty + 1) * side, tx * side:(tx + 1) * side].sum()) for tx in range(nt)] for ty in range(nt)])
 
 
 def texel_index(c0, c1, R):
@@ -142,14 +223,20 @@ CROWDS = {"1024+1": [1024, 1], "1+1024+1": [1, 1024, 1], "1024+1024+5": [1024, 1
 
 
 def crowd_all(S, dtype=np.float64, seed=0, F=65535):
-    """F faces, every one on tile (0, 0): 64 consumes of 2048 faces (the last of 2047)."""
+    """F faces, every one on tile (0, 0): for F = 65535, 64 consumes of 2048 faces (the last of 2047)."""
     fv, tex, _ = crowd([WINDOW] * (F // WINDOW) + [F % WINDOW], S, dtype, seed, T2=1)
     return fv, tex
 
 
-def edge_targets(S):
-    """Pixel indices where the edge scene puts box edges: raster ends and the 15 | 16 tile boundary."""
-    return sorted({i for i in (0, 15, 16, S - 1) if 0 <= i < S})
+# tile-list lengths on one tile for the default path: either side of the LCAP segment and of k_raster_fwd4's FWD4_CAP
+# list, and every face of a narrow mesh
+LIST_LENGTHS = [LCAP - 1, LCAP, LCAP + 1, FWD4_CAP - 1, FWD4_CAP, FWD4_CAP + 1, 65535]
+
+
+def edge_targets(S, fast=False):
+    """Pixel indices where the edge scene puts box edges: raster ends and the 15 | 16 tile boundary; fast adds the
+    31 | 32 boundary of k_raster_fwd4's tiles and the 63 | 64 boundary of the coarse bins."""
+    return sorted({i for i in (0, 15, 16, S - 1) + ((31, 32, CB - 1, CB) if fast else ()) if 0 <= i < S})
 
 
 def edge_vertices(c, r, side, dtype):
@@ -176,9 +263,9 @@ def edge_vertices(c, r, side, dtype):
 EDGE_DEPTH = 1.5
 
 
-def edges(S, dtype=np.float64, seed=0, T2=4):
+def edges(S, dtype=np.float64, seed=0, T2=4, fast=False):
     """Faces whose cull-box edge lies on a pixel centre, or at the nearest value either side of it (edge_vertices), for
-    each of the four box sides at every edge_targets(S) index.  Each face has an edge 3 pixels long on its box side,
+    each of the four box sides at every edge_targets(S, fast) index.  Each face has an edge 3 pixels long on its box side,
     centred on a row (column) in the middle of the raster, and its third vertex EDGE_DEPTH = 1.5 away from that edge into
     the raster.  A pixel centre a box radius r outside the edge then has barycentric r / 1.5 against the third vertex,
     well inside the barycentric distance cut-off r^2 (edge_pixels_alive): the box tests alone decide it.  Returns fv,
@@ -190,7 +277,7 @@ def edges(S, dtype=np.float64, seed=0, T2=4):
     faces, meta = [], []
     for side in range(4):   # xlo, xhi, ylo, yhi
         sign = -1 if side % 2 == 0 else 1
-        for i in edge_targets(S):
+        for i in edge_targets(S, fast):
             c = pixel_centre(i, S, dtype)
             for v in edge_vertices(c, r, sign, dtype):
                 d = int(np.sign(dtype(v + sign * r) - c))
@@ -227,6 +314,37 @@ def big(dtype=np.float64, seed=0, T2=9, nan=False):
     fv = np.array(faces, np.float64)[None].astype(dtype)
     tex = rng.uniform(0, 1, size=(1, fv.shape[1], T2, 3)).astype(dtype)
     return fv, tex
+
+
+def records(S, extra, dtype=np.float32, seed=0, T2=4):
+    """The covering face, then `extra` faces of one pixel each in tile (0, 0) (crowd's faces): tile (0, 0) saves
+    min(16, S)^2 + extra records (tile_records), for S >= 16 32 x 8 in the covering face's eight full 32-record blocks
+    and one more block of one record per extra face."""
+    fv, _, hit = crowd([extra], S, np.float64, seed)
+    fv = np.concatenate([np.array(COVER, np.float64)[None, None], fv if extra else fv[:, :0]], 1)
+    tex = np.random.default_rng(seed).uniform(0, 1, size=(1, fv.shape[1], T2, 3))
+    return fv.astype(dtype), tex.astype(dtype)
+
+
+def window_crossing(dtype=np.float32, seed=0, extra=4):
+    """F = FACE_WINDOW + extra faces, on screen only at indices ON = 0, FACE_WINDOW - 1, FACE_WINDOW, F - 1 (returned),
+    every other far off it: the recompute fallback's second face window holds the last two."""
+    F = FACE_WINDOW + extra
+    on = np.array([0, FACE_WINDOW - 1, FACE_WINDOW, F - 1])
+    fv = np.tile(OFF, (F, 1))
+    fv[on] = [[-0.6 + 0.3 * j, -0.5, 3.0 + j, 0.7, -0.4 + 0.2 * j, 4.0 + j, -0.1 * j, 0.8, 5.0 - j * 0.3] for j in range(len(on))]
+    tex = np.full((1, F, 4, 3), 0.5)
+    tex[0, on] = np.random.default_rng(seed).uniform(0, 1, size=(len(on), 4, 3))
+    return fv[None].astype(dtype), tex.astype(dtype), on
+
+
+def many_images(B=65535, seed=7, dtype=np.float64):
+    """B renders of the covering face and one small face moved sideways per render; textures [B, 2, 1, 3]."""
+    rng = np.random.default_rng(seed)
+    fv = np.repeat(np.array([[COVER, [-0.6, -0.5, 2.0, 0.7, -0.4, 2.5, -0.1, 0.8, 3.0]]]), B, 0)
+    fv[:, 1, [0, 3, 6]] += rng.uniform(-0.8, 0.8, size=(B, 1))
+    tex = rng.uniform(0, 1, size=(B, 2, 1, 3))
+    return fv.astype(dtype), tex.astype(dtype)
 
 
 def textured(T2, dtype=np.float64, seed=0):

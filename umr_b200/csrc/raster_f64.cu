@@ -62,10 +62,6 @@ inline Layout ws_layout(int B, int F) {
     return L;
 }
 
-// the reference's max / min chains are comparisons (kernel.cu:32-38); a NaN operand propagates as they do there
-__device__ __forceinline__ double sel_max(double a, double b) { return a > b ? a : b; }
-__device__ __forceinline__ double sel_min(double a, double b) { return a < b ? a : b; }
-
 // kernel.cu:222-282 and the per-face parts of :32-44
 __global__ void __launch_bounds__(256) k_prep_f64(const double* __restrict__ fv, double* __restrict__ rec,
                                                   double* __restrict__ box, int F, double r) {
@@ -92,8 +88,11 @@ __global__ void __launch_bounds__(256) k_prep_f64(const double* __restrict__ fv,
     o[R_SYM + 3] = x1 * x1 + y1 * y1 + 1;
     o[R_SYM + 4] = x1 * x2 + y1 * y2 + 1;
     o[R_SYM + 5] = x2 * x2 + y2 * y2 + 1;
-    const double xlo = sel_min(sel_min(x0, x1), x2) - r, xhi = sel_max(sel_max(x0, x1), x2) + r;
-    const double ylo = sel_min(sel_min(y0, y1), y2) - r, yhi = sel_max(sel_max(y0, y1), y2) + r;
+    // the reference's max / min (kernel.cu:32-38) are CUDA's double overloads, fmax / fmin: a NaN coordinate is dropped,
+    // so a face with one keeps the box of its finite coordinates.  Finite inputs: the same bits as comparisons (the +-r
+    // after them removes the sign of a zero)
+    const double xlo = fmin(fmin(x0, x1), x2) - r, xhi = fmax(fmax(x0, x1), x2) + r;
+    const double ylo = fmin(fmin(y0, y1), y2) - r, yhi = fmax(fmax(y0, y1), y2) + r;
     o[R_BOX + 0] = xlo; o[R_BOX + 1] = xhi; o[R_BOX + 2] = ylo; o[R_BOX + 3] = yhi;
     int flags = 0;  // first obtuse corner only, :273-281
     if ((x1 - x0) * (x2 - x0) + (y1 - y0) * (y2 - y0) < 0) flags = 1;

@@ -193,8 +193,8 @@ __device__ __forceinline__ bool fragment(const T* __restrict__ rc, T xp, T yp, T
     return true;
 }
 
-// NaN-aware note: for float, fmaxf/fminf return the non-NaN operand whereas the reference's comparisons
-// propagate differently; float inputs with NaN coordinates are outside the supported domain.
+// Cull boxes (k_prep, k_prep_f64) take the box of a face's finite coordinates, as the reference's max / min do on the
+// device (CUDA's fmaxf / fmax drop a NaN operand): a face with a NaN vertex turns the pixels of that box NaN.
 
 // Modes UMR does not exercise (SURVEY.md §8f-3): hard / barycentric distance, hard / sum alpha, per-vertex textures.  The
 // generic kernels read the mode ids from Consts at run time; the float UMR configuration (euclidean, prod, surface) has its
