@@ -140,7 +140,8 @@ int umr_raster_forward(const float* face_vertices, const float* textures, float*
  * struct and workspace as umr_raster_forward (UMR's configuration: euclidean / prod / surface).
  * visible_faces [B,F] u8 (optional): 1 where the face wins at least one pixel (a background pixel marks face F-1, as the
  * reference's negative index does) -- the set TexCycle extracts from the plane with torch.unique (loss_utils.py:161-166); hand it to umr_texcycle_forward(face_ids = NULL, visible = ...).  aggrs_info
- * may then be NULL: no plane is written at all. */
+ * may then be NULL: no plane is written at all.  The bytes follow the plane's depth order exactly: depths -0 and +0 are
+ * equal (the lower face index wins), and faces whose box reaches far off the raster are tested like any other. */
 int umr_raster_visibility(const float* face_vertices, float* aggrs_info, uint8_t* visible_faces,
                           const UmrRasterParams* params, void* workspace, void* stream);
 

@@ -35,6 +35,14 @@ RTOL64, ATOL64, GRTOL64 = 1e-11, 1e-13, 1e-11
 # only those scenes (LOOSE) hold float32 vertex gradients to 5e-5 of the tensor's largest with a relative
 # tolerance of 2e-3 and p2f to 2e-6 absolute; the crowd and edge scenes keep test_raster_modes_gpu's gates.
 GRAD_FACE_FLOOR = 1e-2
+# A float32 texel gradient is a sum of one term per (pixel, face) pair that samples the texel, added by the kernels in
+# the order their atomics land and by oracle B in pixel order.  Each addition rounds by at most half an ulp of the
+# partial sum, and every partial sum is at most sum |term|, so the two results differ by a random walk of such
+# roundings: about 2^-24 x sum |term| where the terms cancel.  Where they cancel, that exceeds the float32 floor below
+# (1e-6 of the tensor's largest gradient), and the comparison would depend on the atomics' order: the float32 paths'
+# texel gradients also get a per-texel floor of TEX_SUM_ULPS x 2^-24 x sum |term| (oracle B's texel gradient with
+# absolute adjoints, "grad_tex_abs": every texel weight is >= 0).  A term dropped or added twice is larger than that.
+TEX_SUM_ULPS = 8.0
 DET_STRICT = dict(grad_faces_atol=1e-6, grad_faces_rtol=1e-4, p2f_atol=1e-6)
 DET_LOOSE = dict(grad_faces_atol=5e-5, grad_faces_rtol=2e-3, p2f_atol=2e-6)
 GUARD = 256                                     # bytes of each band
@@ -73,14 +81,15 @@ def oracle_eps(gamma):
 # guarded buffers
 # ---------------------------------------------------------------------------------------------------------------------
 class Banded(object):
-    """A device buffer [guard | body | guard]; the body is a copy of `array` or, for an output, the fill payload."""
+    """A device buffer [guard | body | guard]; the body is a copy of `array` or, for an output, the fill payload.
+    skew: the body starts `skew` elements past a 256-byte boundary (the leading band grows by as much)."""
 
-    def __init__(self, dtype, shape=None, array=None):
+    def __init__(self, dtype, shape=None, array=None, skew=0):
         self.dtype = dtype
         it, fill, guard = BITS[dtype]
         self.shape = tuple(array.shape if array is not None else shape)
         self.n = int(np.prod(self.shape))
-        self.g = GUARD // np.dtype(dtype).itemsize
+        self.g = GUARD // np.dtype(dtype).itemsize + skew
         self.raw = torch.full((self.n + 2 * self.g,), guard, dtype=it, device=DEV)
         self.body = self.raw[self.g:self.g + self.n]
         if array is not None:
@@ -88,7 +97,7 @@ class Banded(object):
             self.body.copy_(torch.from_numpy(src.view(np.int64 if dtype == np.float64 else np.int32)))
         else:
             self.body.fill_(fill)
-        assert self.ptr().value % 256 == 0
+        assert self.ptr().value % 256 == skew * np.dtype(dtype).itemsize
 
     def ptr(self):
         return ctypes.c_void_p(self.body.data_ptr())
@@ -106,6 +115,30 @@ class Banded(object):
 
     def numpy(self):
         return self.tensor().cpu().numpy()
+
+
+class BandedBytes(object):
+    """A uint8 output [guard | body | guard] whose body starts filled with a non-zero byte: an output the call must
+    clear before it marks anything."""
+    FILL, GUARD_BYTE = 0x5A, 0xA5
+
+    def __init__(self, shape):
+        self.shape = tuple(shape)
+        self.n = int(np.prod(self.shape))
+        self.raw = torch.full((self.n + 2 * GUARD,), self.GUARD_BYTE, dtype=torch.uint8, device=DEV)
+        self.body = self.raw[GUARD:GUARD + self.n]
+        self.body.fill_(self.FILL)
+        assert self.ptr().value % 256 == 0
+
+    def ptr(self):
+        return ctypes.c_void_p(self.body.data_ptr())
+
+    def check(self, what):
+        assert bool((self.raw[:GUARD] == self.GUARD_BYTE).all()) and bool((self.raw[GUARD + self.n:] == self.GUARD_BYTE).all()), \
+            "%s: a guard band was written" % what
+
+    def numpy(self):
+        return self.body.view(self.shape).cpu().numpy()
 
 
 class Workspace(object):
@@ -274,6 +307,9 @@ def oracle(path, fv, tex, isz, aa, g, kw, dt=None, alpha_only=False):
         ghi = softras.avg_pool2_backward(np.asarray(g, dt)) if aa else np.asarray(g, dt)
         gf, gt = softras.backward(fwd, ghi, cfg, impl="B")
         out["grad_faces"], out["grad_tex"] = gf, gt.reshape(G, B // G, *tex.shape[1:]).sum(1)
+        if dt == np.float32:
+            gta = softras.backward(fwd, np.abs(ghi), cfg, impl="B")[1]
+            out["grad_tex_abs"] = np.abs(gta).reshape(G, B // G, *tex.shape[1:]).sum(1)
         if alpha_only:
             ga = np.zeros_like(ghi)
             ga[:, 3] = ghi[:, 3]
@@ -317,6 +353,8 @@ def compare(path, got, ref, rgb, what, rtol=1e-4, loose=False, face_floor_shared
         else:
             rel = det["grad_faces_atol"] if name == "grad_faces" else 1e-6
             atol = rel * float(np.nanmax(np.abs(b), initial=0.0)) + 1e-7 if name.startswith("grad") else det["p2f_atol"] if name == "p2f" else 1e-6
+            if name == "grad_tex" and ref.get("grad_tex_abs") is not None:   # rounding of a cancelling sum (TEX_SUM_ULPS)
+                atol = np.fmax(atol, TEX_SUM_ULPS * 2.0 ** -24 * np.asarray(ref["grad_tex_abs"], np.float64))
             worst[name] = _ratio(got[name], b, max(rtol, det["grad_faces_rtol"]) if name == "grad_faces" else rtol, atol)
     msg = "%s %s: worst error/bound %s" % (path, what, ", ".join("%s %.3g" % kv for kv in worst.items()))
     assert all(v <= 1.0 for v in worst.values()), msg

@@ -409,3 +409,212 @@ def edge_pixels_alive(fv, side, i, S, dtype):
     o = o[(o >= lo) & (o <= hi)].astype(np.float64)
     xp, yp = (np.full_like(o, c), o) if side < 2 else (o, np.full_like(o, c))
     return int(barycentric_alive(fv, xp, yp).sum())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# scenes of the visibility range tests (test_raster_visibility_range_gpu.py / _cpu.py): umr_raster_visibility's hard
+# z-buffer, its planes (k_raster_fwd3<2>) and its visible-face bytes (k_visible_faces, which scans a face's pixel box
+# per 64 x 64 bin: the tight vertex box + 2 pixels, or the whole cull box for a thin face, R_FLG bit 4).  Every scene
+# returns face_vertices [B, F, 9] and a dict of its claims for the CPU checks.
+# ---------------------------------------------------------------------------------------------------------------------
+INT32_MIN, INT32_MAX = -2 ** 31, 2 ** 31 - 1
+FAR_FACTORS = [0.5, 1.0, 2.0, 1e3]
+WIDE_DRAWN = 5e7
+FAR_BEHIND = [-0.3, -0.25, 2.0, 0.35, -0.2, 2.5, 0.05, 0.4, 2.0]   # a small nearer face in the middle of every far render
+
+
+def bin_index(v, S, side):
+    """k_visible_faces' pixel index of box coordinate v before the bin offset: floor (side -1) or ceil (+1) of
+    (v S + S - 1) / 2 in float32, -2 / +2 pixels, as int64 (no saturation)."""
+    e = ((np.float32(v) * np.float32(S) + np.float32(S - 1)) * np.float32(0.5)).astype(np.float32)
+    return int(np.floor(e)) - 2 if side < 0 else int(np.ceil(e)) + 2
+
+
+def crosses_int32(v, S, side):
+    """Whether the unclamped index of box coordinate v leaves the int32 range at some bin of an S-pixel raster (the
+    conversion saturates, or the margin or the bin offset x0 <= S - 1 wraps)."""
+    i = bin_index(v, S, side)
+    return i - (S - 1) < INT32_MIN if side < 0 else i > INT32_MAX
+
+
+def far_faces(S, factors=FAR_FACTORS, z=5.0):
+    """Faces covering the raster whose box reaches X = factor * 2^32 / S off it.
+    thin: a sliver from a vertex X away on one side (axis x or y, side -1 low or +1 high) to an edge 1.5 off the other
+          side; its smallest angle is about 1 / X, so it takes the whole-cull-box scan.  It covers the band between
+          -0.5 and 0.5 across the raster.
+    wide: a right triangle with its right angle on a corner (+-1.5, +-1.5) of the raster's surround and legs X long
+          along x and y (the box reaches X off one x side and one y side; a triangle this wide reaching off one side
+          only would be thin).  It covers the whole raster.
+    One face per render, behind FAR_BEHIND and in front of an off-screen face (face F - 1 = 2 is then marked only by
+    a background pixel).  Returns fv [B, 3, 9] and meta: (kind, axis, side, factor, X) per render.
+    Which of them the z-buffer draws (oracle B): every thin one; the wide ones while X < WIDE_DRAWN (between 3.4e7 and
+    6.7e7).  Past it the X^2 terms of the float32 barycentric inverse swamp the pixel terms and no pixel centre tests
+    inside.  At S = 2048 the wide faces of factors 1/2 and 1 are not thin either (X^6, the product k_prep's bit-4 test
+    forms, stays finite): they take the tight vertex box."""
+    renders, meta = [], []
+    for fac in factors:
+        X = float(np.float32(fac * 2.0 ** 32 / S))
+        for axis in (0, 1):
+            for side in (-1, 1):
+                v = [[side * X, -0.5], [-side * 1.5, -0.5], [-side * 1.5, 0.5 + 1e-3]]
+                v = [p[::-1] if axis else p for p in v]
+                renders.append([sum(([x, y, z] for x, y in v), []), FAR_BEHIND, list(OFF)])
+                meta.append(("thin", axis, side, fac, X))
+        for cx in (-1.5, 1.5):
+            for cy in (-1.5, 1.5):
+                v = [[cx, cy], [-np.sign(cx) * X, cy], [cx, -np.sign(cy) * X]]
+                renders.append([sum(([x, y, z] for x, y in v), []), FAR_BEHIND, list(OFF)])
+                meta.append(("wide", "x%+d y%+d" % (-np.sign(cx), -np.sign(cy)), 0, fac, X))
+    return np.array(renders, np.float32), meta
+
+
+def huge_faces(z=5.0):
+    """Vertices at 1e15 and 1e20 and at +-inf, in far_faces' layout: the thin faces at 1e15 and 1e20 are drawn; the
+    wide ones are not (at 1e15 as far_faces' past WIDE_DRAWN; at 1e20 x y overflows float32 and the barycentric inverse
+    is not finite), nor is a face with an infinite vertex."""
+    renders, meta = [], []
+    for X in (1e15, 1e20):
+        for kind, v in (("wide", [[-1.5, -1.5], [X, -1.5], [-1.5, X]]), ("thin", [[-X, -0.5], [1.5, -0.5], [1.5, 0.5]])):
+            renders.append([sum(([x, y, z] for x, y in v), []), FAR_BEHIND, list(OFF)])
+            meta.append((kind, X))
+    for v in ([[-np.inf, -0.5], [1.5, -0.5], [1.5, 0.5]], [[-1.5, -1.5], [np.inf, -1.5], [-1.5, np.inf]],
+              [[-np.inf, -1.5], [np.inf, -1.5], [0.0, 1.5]]):
+        renders.append([sum(([x, y, z] for x, y in v), []), FAR_BEHIND, list(OFF)])
+        meta.append(("inf", np.inf))
+    return np.array(renders, np.float32), meta
+
+
+THIN_CUT = np.float32(1e-6)
+
+
+def thin_flag(f):
+    """k_prep's bit 4 (raster.cu), restated in float32 for one face [9]: the sine of the smallest angle below ~1e-3."""
+    x0, y0, _, x1, y1, _, x2, y2, _ = np.asarray(f, np.float32)
+    l01 = (x1 - x0) * (x1 - x0) + (y1 - y0) * (y1 - y0)
+    l02 = (x2 - x0) * (x2 - x0) + (y2 - y0) * (y2 - y0)
+    l12 = (x2 - x1) * (x2 - x1) + (y2 - y1) * (y2 - y1)
+    lmin = np.fmin(np.fmin(l01, l02), l12)
+    with np.errstate(all="ignore"):
+        prod2 = (l01 * l02 * l12) / np.fmax(lmin, np.float32(1e-30))
+        draw = x2 * (y0 - y1) + x0 * (y1 - y2) + x1 * (y2 - y0)
+        return not bool(draw * draw >= THIN_CUT * prod2)
+
+
+def _sliver(S, row, x_lo, x_hi, z, place=lambda f: f):
+    """A right-angled sliver along pixel row `row` from x_lo to x_hi whose far corner's height crosses the bit-4 cut:
+    (thin, not thin), the two adjacent float32 heights of that corner either side of the cut (a height of about
+    1e-3 of its length).  Its base lies 1 % of that height below the row's centres, so it covers the row from about
+    1 % of its length past its sharp end to its right-angled end."""
+    xa, xb = np.float32(x_lo), np.float32(x_hi)
+    yc = float(pixel_centre(S - 1 - row, S, np.float32))
+    y0 = np.float32(yc - 1e-5 * (float(xb) - float(xa)))
+    face = lambda y2: place(np.array([xa, y0, z, xb, y0, z, xb, y2, z], np.float32).reshape(3, 3)).reshape(9)   # noqa: E731
+    lo, hi = np.float32(y0 + 1e-5 * (xb - xa)), np.float32(y0 + 0.01 * (xb - xa))   # thin at lo, not thin at hi
+    assert thin_flag(face(lo)) and not thin_flag(face(hi))
+    while np.nextafter(lo, hi) != hi:
+        mid = np.float32((np.float64(lo) + np.float64(hi)) / 2)
+        if mid == lo or mid == hi:
+            mid = np.nextafter(lo, hi)
+        lo, hi = (mid, hi) if thin_flag(face(mid)) else (lo, mid)
+    return face(lo), face(hi)
+
+
+def thin_switch(S):
+    """Sliver pairs either side of k_prep's bit-4 cut, each sliver on a row of its own: along rows S/4 and S/4 + 2,
+    mirrored in x along rows 3S/4 and 3S/4 + 2, and the four transposed (columns, behind the rows).  Each spans most of
+    the raster (S >= 8).  Returns fv [1, 8, 9], the expected bit 4 per face."""
+    px = 2.0 / S
+    lo, hi = float(pixel_centre(1, S, np.float64)) - 0.25 * px, float(pixel_centre(S - 2, S, np.float64)) + 0.25 * px
+    mirror = lambda f: f * np.float32([-1, 1, 1])           # noqa: E731
+    transpose = lambda f: f[:, [1, 0, 2]]                     # noqa: E731
+    faces, thin = [], []
+    for k, (row, place) in enumerate(((S // 4, lambda f: f), ((3 * S) // 4, mirror), (S // 4, transpose),
+                                      ((3 * S) // 4, lambda f: transpose(mirror(f))))):
+        for t in range(2):   # the thin sliver on one row, the other on the row after next
+            faces.append(_sliver(S, row + 2 * t, lo, hi, 2.0 + k, place)[t])
+            thin.append(t == 0)
+    return np.array(faces, np.float32)[None], np.array(thin)
+
+
+def depth_order(S, seed=0):
+    """Depth ties and near-ties, one render each:
+    repeat   one face four times, between other faces: the lowest index wins everywhere;
+    ulp      two overlapping constant-depth faces one float ulp apart, in both index orders;
+    edge     two faces sharing an edge along a pixel-centre column (a barycentric exactly 0 there: fragment() decides)
+             at the same depth, and a third sharing an edge along a pixel-centre row;
+    centres  a face whose vertices are pixel centres, over one whose vertices are too."""
+    rng = np.random.default_rng(seed)
+    c = lambda i: float(pixel_centre(i, S, np.float32))   # noqa: E731
+    rnd = rng.uniform(-0.9, 0.9, size=(2, 9)) * np.array([1, 1, 0] * 3) + np.array([0, 0, 3.0] * 3)
+    tri = [-0.6, -0.5, 2.0, 0.7, -0.4, 2.5, -0.1, 0.8, 3.0]
+    z = np.float32(2.0)
+    zn = float(np.nextafter(z, np.float32(0)))
+    flat = lambda zz: [-0.8, -0.7, zz, 0.75, -0.6, zz, 0.1, 0.85, zz]   # noqa: E731
+    e = lambda k: c((k * S) // 8)   # noqa: E731
+    m, a, b = c(S // 2), c(S // 4), c((3 * S) // 4)
+    renders = {
+        "repeat": [rnd[0], tri, tri, rnd[1], tri, tri],
+        "ulp": [flat(2.0), flat(zn), OFF, OFF, OFF, OFF],
+        "ulp reversed": [flat(zn), flat(2.0), OFF, OFF, OFF, OFF],
+        # a diamond split along the column of e(2) (faces 0, 1) and one split along the row of e(6) (faces 2, 3)
+        "edge": [[e(2), e(1), 2.0, e(2), e(3), 2.0, e(1), e(2), 2.0], [e(2), e(3), 2.0, e(2), e(1), 2.0, e(3), e(2), 2.0],
+                 [e(5), e(6), 2.0, e(7), e(6), 2.0, e(6), e(7), 2.0], [e(7), e(6), 2.0, e(5), e(6), 2.0, e(6), e(5), 2.0],
+                 OFF, OFF],
+        "centres": [[a, a, 2.0, b, a, 2.0, m, b, 2.0], [c(1), c(1), 3.0, c(S - 2), c(1), 3.0, c(1), c(S - 2), 3.0],
+                    OFF, OFF, OFF, OFF],
+    }
+    return np.array(list(renders.values()), np.float32), list(renders)
+
+
+def zero_depths():
+    """For near = 0: a face with a vertex at depth +0 and the same face with that vertex at -0 (every pixel of either
+    has depth exactly +0 or -0: the clipped barycentric of that vertex is at least 1e-5), in both index orders, then an
+    off-screen face.  The strict '<' of the z-buffer treats +0 and -0 as one depth: the lower index wins."""
+    base = [-0.7, -0.6, 0.0, 0.8, -0.5, 2.0, 0.0, 0.75, 3.0]
+    pos, neg = list(base), list(base)
+    neg[2] = -0.0
+    return np.array([[pos, neg, OFF], [neg, pos, OFF]], np.float32)
+
+
+def negative_depths():
+    """For near = -5, far = 5: faces at negative depths over faces at positive depths and one cut by near."""
+    faces = [[-0.8, -0.7, 2.0, 0.75, -0.6, 2.5, 0.1, 0.85, 3.0],
+             [-0.5, -0.4, -1.0, 0.6, -0.3, -1.5, 0.0, 0.6, -2.0],
+             [-0.2, -0.9, -3.0, 0.9, 0.1, -0.5, -0.6, 0.5, -1.2],
+             [-0.9, 0.2, -8.0, 0.2, 0.3, -2.0, -0.4, 0.9, -6.0],
+             OFF]
+    return np.array([faces], np.float32)
+
+
+def depth_cut():
+    """For far = 1e9: a constant-depth face at 1e7 (the z-buffer's initial depth_min) over one at the float below it,
+    and the same pair the other way round in index."""
+    z0, z1 = 1e7, float(np.nextafter(np.float32(1e7), np.float32(0)))
+    a = [-0.8, -0.7, z0, 0.75, -0.6, z0, 0.1, 0.85, z0]
+    b = [-0.6, -0.8, z1, 0.85, -0.5, z1, -0.1, 0.7, z1]
+    return np.array([[a, b, OFF], [b, a, OFF]], np.float32)
+
+
+def front_back(seed=0, F=12):
+    """fill_back = False: front faces (even indices) and back faces (odd) interleaved and overlapping, the back faces
+    nearer."""
+    rng = np.random.default_rng(seed)
+    faces = []
+    for i in range(F):
+        cx, cy = rng.uniform(-0.5, 0.5, size=2)
+        r = rng.uniform(0.2, 0.5)
+        v = [[cx - r, cy - r], [cx + r, cy - 0.5 * r], [cx, cy + r]]
+        if i % 2 == 0:   # even faces front (k_prep's bit 3), odd ones back
+            v = [v[0], v[2], v[1]]
+        z = 2.0 + (0.0 if i % 2 else 1.0) + 0.01 * i
+        faces.append(sum(([x, y, z] for x, y in v), []))
+    fv = np.array(faces, np.float32)[None]
+    return fv
+
+
+def small(F, seed=0):
+    """F = 1 or 2 faces (face 0 is then the background's marker too, or face 1)."""
+    rng = np.random.default_rng(seed)
+    base = np.array([[-0.6, -0.5, 2.0, 0.7, -0.4, 2.5, -0.1, 0.8, 3.0], [-0.9, -0.2, 2.2, 0.3, -0.9, 2.2, 0.5, 0.6, 4.0]])
+    fv = base[:F] + rng.uniform(-0.05, 0.05, size=(F, 9)) * np.array([1, 1, 0] * 3)
+    return fv[None].astype(np.float32)

@@ -101,7 +101,7 @@ def run_scene(fv, tex, isz, aa, what, feature, loose=False, on=None, wide=True, 
     for rgb in rgbs:
         k = dict(dict(aggr_func_rgb=rgb, eps=oracle_eps(KW["gamma_val"])), **(kw or {}))
         ref = oracle("det", fv[:, on], tex[:, on], isz, aa, g, k, alpha_only=True)
-        ref_split = dict(grad_faces=ref["grad_faces_alpha"], grad_tex=ref["grad_tex"])
+        ref_split = dict(grad_faces=ref["grad_faces_alpha"], grad_tex=ref["grad_tex"], grad_tex_abs=ref["grad_tex_abs"])
         ref_sil = dict(images=ref["images"][:, 3], colors=ref["colors"][:, 3] if aa else None, grad_faces=ref["grad_faces_alpha"])
         for P in ((0, PAD) if wide and F <= 65535 else (0,)):
             if P:

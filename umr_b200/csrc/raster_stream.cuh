@@ -187,11 +187,16 @@ __global__ void __launch_bounds__(CTA) k_visible_faces(const float* __restrict__
             xlo = fminf(fminf(ax, bx), cx); xhi = fmaxf(fmaxf(ax, bx), cx);
             ylo = fminf(fminf(ay, by), cy); yhi = fmaxf(fmaxf(ay, by), cy);
         }
-        // pixel_coord(i) = (2 i + 1 - S) / S  <=>  i = (x S + S - 1) / 2;  rows run top-down: y index j = S - 1 - row
-        int c0 = (int)floorf((xlo * (float)S + (float)(S - 1)) * 0.5f) - 2 - x0;
-        int c1 = (int)ceilf((xhi * (float)S + (float)(S - 1)) * 0.5f) + 2 - x0;
-        const int j0 = (int)floorf((ylo * (float)S + (float)(S - 1)) * 0.5f) - 2;
-        const int j1 = (int)ceilf((yhi * (float)S + (float)(S - 1)) * 0.5f) + 2;
+        // pixel_coord(i) = (2 i + 1 - S) / S  <=>  i = (x S + S - 1) / 2;  rows run top-down: y index j = S - 1 - row.
+        // The index is clamped to [-4, S + 4] in float before the conversion: a box reaching past about 2^32 / S would
+        // saturate it, and the +-2 margin and the bin offset would then wrap, leaving a covering face untested.  Inside
+        // the clamp the indices are unchanged; outside it the raster edge decides as before.
+        const float ilo = -4.f, ihi = (float)(S + 4);
+        auto pix = [&](float v) { return fminf(fmaxf((v * (float)S + (float)(S - 1)) * 0.5f, ilo), ihi); };
+        int c0 = (int)floorf(pix(xlo)) - 2 - x0;
+        int c1 = (int)ceilf(pix(xhi)) + 2 - x0;
+        const int j0 = (int)floorf(pix(ylo)) - 2;
+        const int j1 = (int)ceilf(pix(yhi)) + 2;
         int r0 = (S - 1 - j1) - y0, r1 = (S - 1 - j0) - y0;
         if (!(xlo == xlo && xhi == xhi && ylo == ylo && yhi == yhi)) { c0 = 0; c1 = CB; r0 = 0; r1 = CB; }  // NaN face: whole bin
         c0 = max(c0, 0); c1 = min(c1, ncol - 1); r0 = max(r0, 0); r1 = min(r1, nrow - 1);
@@ -220,8 +225,9 @@ __global__ void __launch_bounds__(CTA) k_visible_faces(const float* __restrict__
             clip_bary(k0, k1, k2);
             const float zp = depth_of(rc, k0, k1, k2);
             if (zp < K.near_ || zp > K.far_ || !(zp < 10000000.f)) continue;   // depth range (:399), initial depth_min (:341)
-            // zp > 0 here (near_ >= 0 is assumed by the packed ordering; negative depths are ordered by the sign fix below)
-            uint32_t zb = __float_as_uint(zp);
+            // -0 and +0 are one depth to the strict '<' of the plane (the lower face index wins the tie): pack both as +0.
+            // Negative depths (near_ < 0) are ordered by the sign fix below.
+            uint32_t zb = __float_as_uint(zp == 0.f ? 0.f : zp);
             zb = (zb & 0x80000000u) ? ~zb : (zb | 0x80000000u);   // total order of floats as unsigned integers
             atomicMin(&s_z[row * CB + col], ((unsigned long long)zb << 32) | (unsigned long long)(uint32_t)f);
         }
