@@ -20,6 +20,7 @@
  *       nnutils/nmr_pytorch.py; the upstream package is not vendored, its contract is DESIGN.md §7).
  *   umr_nmr_backward_faces adds NMR's approximate geometry gradient for the functional `neural_renderer.rasterize*`
  *       (DESIGN.md §14).
+ *   umr_nmr_lighting_forward / _backward compute `neural_renderer.lighting` and its gradients (DESIGN.md §15).
  *
  * Conventions: plain device pointers + sizes, no torch types.  Every buffer is CALLER-allocated
  * (torch owns all memory); the library keeps no global mutable state and is re-entrant across host
@@ -476,6 +477,44 @@ int umr_nmr_backward_faces(const float* vertices, const int32_t* faces, const in
                            const float* grad_rgb, const float* grad_alpha, const float* grad_depth,
                            float* grad_face_vertices, const UmrNmrParams* params, float eps, void* workspace,
                            void* stream);
+
+/* neural_renderer.lighting (DESIGN.md §15): lit_textures[b,f] = textures[b,f] * light[b,f] with the light of DESIGN.md
+ * §7 step 2, light = Ia*ca + Id*(cd*relu(n.d)), n = normalize(cross(v0 - v1, v2 - v1), eps=1e-5), a term whose
+ * intensity is 0 not added.  Every buffer holds `dtype` elements (UMR_DTYPE_FLOAT32 / UMR_DTYPE_FLOAT64, as umr_voxelize
+ * takes it; double computes in double, float in float with the intensities rounded to float):
+ *   faces [B,F,3,3], textures / lit_textures [B,F,T,T,T,3] (n3 = 3 T^3 elements per face),
+ *   color_ambient / color_directional / direction: 3 elements, or [B,3] when the matching *_bstride is 3 (0: one
+ *   vector for every image). */
+typedef struct UmrNmrLightParams {
+    int32_t batch_size, num_faces, texture_res; /* B, F, T (>= 1) */
+    int32_t dtype;
+    double intensity_ambient, intensity_directional;
+    int32_t color_ambient_bstride, color_directional_bstride, direction_bstride; /* 0 or 3 */
+    int32_t reserved;                                                            /* 0 */
+} UmrNmrLightParams;
+
+size_t umr_sizeof_nmr_light_params(void);
+/* One launch; lit_textures is fully written (it may not alias textures).  UMR_ERR_BAD_ARG for a NULL buffer, a buffer
+ * not aligned to its element size, B, F or T < 1, a stride other than 0 / 3, another dtype or reserved != 0;
+ * UMR_ERR_TOO_LARGE when B*F*3*T^3 >= 2^31. */
+int umr_nmr_lighting_forward(const void* faces, const void* textures, const void* color_ambient,
+                             const void* color_directional, const void* direction, void* lit_textures,
+                             const UmrNmrLightParams* params, void* stream);
+/* Bytes of 256-byte aligned device scratch umr_nmr_lighting_backward needs when grad_light is given:
+ * align256(9 * B * F * sizeof(dtype)); 0 for the sizes and dtypes it refuses. */
+size_t umr_nmr_lighting_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t dtype);
+/* Gradients of lit_textures' adjoint grad_lit [B,F,T,T,T,3], each output NULL to skip and fully written otherwise:
+ *   grad_textures [B,F,T,T,T,3] = light * grad_lit;
+ *   grad_faces [B,F,3,3], through relu, normalize and cross (exactly 0 when Id == 0);
+ *   grad_light [B,9]: per image, the gradients of ca, cd and direction (as if each were [B,3]), summed over the faces in
+ *   ascending order (a second launch; needs the workspace).
+ * One warp per (image, face) is the only writer of that face's outputs, and nothing uses atomics: bitwise reproducible.
+ * Refusals as umr_nmr_lighting_forward; also UMR_ERR_BAD_ARG for a NULL grad_lit, no output at all, or grad_light
+ * without a 256-byte aligned workspace.  1 launch, 2 with grad_light. */
+int umr_nmr_lighting_backward(const void* faces, const void* textures, const void* color_ambient,
+                              const void* color_directional, const void* direction, const void* grad_lit,
+                              void* grad_faces, void* grad_textures, void* grad_light, const UmrNmrLightParams* params,
+                              void* workspace, void* stream);
 
 /* Mesh voxelisation: SoftRas `functional.voxelization` (functional/voxelization.py:41-58, kernels
  * cuda/voxelization_cuda_kernel.cu).  faces [B,F,3,3] (float32 or float64 as `dtype` says, contiguous; coordinates are

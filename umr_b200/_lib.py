@@ -48,6 +48,14 @@ class UmrNmrParams(ctypes.Structure):
                 ("light_direction", ctypes.c_float * 3), ("background_color", ctypes.c_float * 3)]
 
 
+class UmrNmrLightParams(ctypes.Structure):
+    _fields_ = [("batch_size", ctypes.c_int32), ("num_faces", ctypes.c_int32), ("texture_res", ctypes.c_int32),
+                ("dtype", ctypes.c_int32), ("intensity_ambient", ctypes.c_double),
+                ("intensity_directional", ctypes.c_double), ("color_ambient_bstride", ctypes.c_int32),
+                ("color_directional_bstride", ctypes.c_int32), ("direction_bstride", ctypes.c_int32),
+                ("reserved", ctypes.c_int32)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "umr_error_string": (ctypes.c_char_p, [ctypes.c_int]),
@@ -143,6 +151,13 @@ EXPORTS = {
     "umr_nmr_backward_faces_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 4),
     "umr_nmr_backward_faces": (ctypes.c_int, [c_f32p] * 8 + [ctypes.POINTER(UmrNmrParams), ctypes.c_float, ctypes.c_void_p,
                                                              ctypes.c_void_p]),
+    # neural_renderer.lighting: faces, textures, color_ambient, color_directional, direction, lit_textures (forward);
+    # ..., grad_lit, grad_faces, grad_textures, grad_light, params, workspace, stream (backward)
+    "umr_sizeof_nmr_light_params": (ctypes.c_size_t, []),
+    "umr_nmr_lighting_forward": (ctypes.c_int, [ctypes.c_void_p] * 6 + [ctypes.POINTER(UmrNmrLightParams), ctypes.c_void_p]),
+    "umr_nmr_lighting_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 3),
+    "umr_nmr_lighting_backward": (ctypes.c_int, [ctypes.c_void_p] * 9 + [ctypes.POINTER(UmrNmrLightParams), ctypes.c_void_p,
+                                                                        ctypes.c_void_p]),
     "umr_voxelize_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 2),
     "umr_voxelize": (ctypes.c_int, [c_f32p, ctypes.c_int32, c_f32p] + [ctypes.c_int32] * 3 + [ctypes.c_double, ctypes.c_void_p,
                                                                                            ctypes.c_void_p]),
@@ -263,7 +278,8 @@ def load():
                 fn.argtypes = args
             if (lib.umr_sizeof_raster_params() != ctypes.sizeof(UmrRasterParams)
                     or lib.umr_sizeof_project_params() != ctypes.sizeof(UmrProjectParams)
-                    or lib.umr_sizeof_nmr_params() != ctypes.sizeof(UmrNmrParams)):
+                    or lib.umr_sizeof_nmr_params() != ctypes.sizeof(UmrNmrParams)
+                    or lib.umr_sizeof_nmr_light_params() != ctypes.sizeof(UmrNmrLightParams)):
                 raise UmrLibraryError("libumr_b200.so was built from a different include/umr_b200.h than this binding "
                                       "(parameter struct sizes differ): rebuild with `python -m umr_b200.build --force`")
             _lib = lib

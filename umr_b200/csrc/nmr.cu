@@ -13,6 +13,8 @@
 //   k_nmr_bwd_tex  thread = output pixel: the texture adjoint of k_nmr_shade, red.global into [B/G, F, T^3, 3].
 //   k_nmr_shade_raster / k_nmr_grad_faces  the functional rasteriser's geometry gradient (DESIGN.md §14): the raster-
 //                  resolution colour plane, then one warp per face for NMR's edge term and the depth term.
+//   k_nmr_light_fwd / k_nmr_light_bwd / k_nmr_light_reduce  neural_renderer.lighting (DESIGN.md §15), float and double:
+//                  textures * light per face, and its gradients with one warp per face and no atomics.
 //
 // Compiled with -fmad=false (umr_b200/build.py): every product and sum rounds once, in the contract's order.
 #include <cuda_runtime.h>
@@ -48,6 +50,52 @@ inline size_t box_bytes(int B, int Fc) { return align256((size_t)B * Fc * sizeof
 __device__ __forceinline__ float pixel_coord(int i, int S) { return __fdiv_rn((float)(2 * i + 1 - S), (float)S); }
 
 // ---------------------------------------------------------------------------------------------
+// per-face light (DESIGN.md §7 step 2), shared by k_nmr_prep and the lighting kernels (§15)
+// ---------------------------------------------------------------------------------------------
+template <typename T> __device__ __forceinline__ T light_eps();
+template <> __device__ __forceinline__ float light_eps<float>() { return 1e-5f; }
+template <> __device__ __forceinline__ double light_eps<double>() { return 1e-5; }
+
+// the intermediates the lighting backward chains through
+template <typename T>
+struct LightParts {
+    T a[3], b[3];  // v0 - v1, v2 - v1
+    T nrm, den;    // |cross|, max(|cross|, eps)
+    T n[3];        // normal
+    T cs;          // relu(n . d)
+};
+
+// n = normalize(cross(v0 - v1, v2 - v1), eps=1e-5), light = Ia*ca + Id*(cd*relu(n.d)); a term whose intensity is 0 is
+// not added
+template <typename T>
+__device__ __forceinline__ void face_light(const T v[3][3], T Ia, T Id, const T* ca, const T* cd, const T* dir, T l[3],
+                                           LightParts<T>* q) {
+    const T ax = v[0][0] - v[1][0], ay = v[0][1] - v[1][1], az = v[0][2] - v[1][2];
+    const T bx = v[2][0] - v[1][0], by = v[2][1] - v[1][1], bz = v[2][2] - v[1][2];
+    const T c0 = ay * bz - az * by, c1 = az * bx - ax * bz, c2 = ax * by - ay * bx;
+    const T nrm = sqrt((c0 * c0 + c1 * c1) + c2 * c2);
+    const T den = fmax(nrm, light_eps<T>());
+    const T n0 = c0 / den, n1 = c1 / den, n2 = c2 / den;
+    T cs = (n0 * dir[0] + n1 * dir[1]) + n2 * dir[2];
+    cs = cs < T(0) ? T(0) : cs;  // relu (NaN stays NaN)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        T lc = T(0);
+        if (Ia != T(0)) lc = lc + Ia * ca[c];
+        if (Id != T(0)) lc = lc + Id * (cd[c] * cs);
+        l[c] = lc;
+    }
+    if (q) {  // NULL where only the light is wanted (k_nmr_prep)
+        q->a[0] = ax; q->a[1] = ay; q->a[2] = az;
+        q->b[0] = bx; q->b[1] = by; q->b[2] = bz;
+        q->nrm = nrm;
+        q->den = den;
+        q->n[0] = n0; q->n[1] = n1; q->n[2] = n2;
+        q->cs = cs;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // prep
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_nmr_prep(const float* __restrict__ verts, const int32_t* __restrict__ faces,
@@ -71,22 +119,12 @@ __global__ void __launch_bounds__(128) k_nmr_prep(const float* __restrict__ vert
     float out[REC];
 #pragma unroll
     for (int k = 0; k < REC; ++k) out[k] = 0.f;
-    // light from the vertices before look_at: normalize(cross(v0 - v1, v2 - v1), eps=1e-5)
+    // light from the vertices before look_at
     {
-        const float ax = v[0][0] - v[1][0], ay = v[0][1] - v[1][1], az = v[0][2] - v[1][2];
-        const float bx = v[2][0] - v[1][0], by = v[2][1] - v[1][1], bz = v[2][2] - v[1][2];
-        const float c0 = ay * bz - az * by, c1 = az * bx - ax * bz, c2 = ax * by - ay * bx;
-        const float den = fmaxf(sqrtf((c0 * c0 + c1 * c1) + c2 * c2), 1e-5f);
-        const float n0 = c0 / den, n1 = c1 / den, n2 = c2 / den;
-        float cs = (n0 * K.dir[0] + n1 * K.dir[1]) + n2 * K.dir[2];
-        cs = cs < 0.f ? 0.f : cs;  // relu (NaN stays NaN)
+        float l[3];
+        face_light<float>(v, K.Ia, K.Id, K.ca, K.cd, K.dir, l, nullptr);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            float l = 0.f;
-            if (K.Ia != 0.f) l = l + K.Ia * K.ca[c];
-            if (K.Id != 0.f) l = l + K.Id * (K.cd[c] * cs);
-            out[R_L + c] = l;
-        }
+        for (int c = 0; c < 3; ++c) out[R_L + c] = l[c];
     }
     const float Sf = (float)K.S;
     float px[3], py[3];
@@ -728,6 +766,232 @@ __global__ void __launch_bounds__(256) k_nmr_grad_faces(const float* __restrict_
 }
 
 // ---------------------------------------------------------------------------------------------
+// neural_renderer.lighting (DESIGN.md §15): lit = textures * light[b, f], float and double
+// ---------------------------------------------------------------------------------------------
+template <typename T>
+struct LightArgs {
+    const T* faces;  // [B,F,3,3]
+    const T* tex;    // [B,F,n3]
+    const T *ca, *cd, *dir;
+    int sca, scd, sdir;  // batch strides of ca, cd, dir: 0 or 3
+    int F, n3;           // n3 = T^3 * 3
+    long long N;         // B * F * n3
+    T Ia, Id;
+};
+
+// light of face bf = b * F + f
+template <typename T>
+__device__ __forceinline__ void load_light(const LightArgs<T>& A, int bf, T l[3], LightParts<T>* q) {
+    const int b = bf / A.F;
+    T v[3][3], ca[3], cd[3], dir[3];
+    const T* fv = A.faces + (size_t)bf * 9;
+#pragma unroll
+    for (int k = 0; k < 9; ++k) v[k / 3][k % 3] = __ldg(fv + k);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        ca[c] = __ldg(A.ca + (size_t)b * A.sca + c);
+        cd[c] = __ldg(A.cd + (size_t)b * A.scd + c);
+        dir[c] = __ldg(A.dir + (size_t)b * A.sdir + c);
+    }
+    face_light(v, A.Ia, A.Id, ca, cd, dir, l, q);
+}
+
+constexpr int LT_CTA = 256;
+constexpr int LT_VPT = 4;  // 16-byte vectors per thread
+
+// Forward: each CTA takes LT_CTA * LT_VPT vectors of the flat [B*F*n3] texel array.  Its threads first compute the light
+// of every face that range touches into shared memory, then multiply the texels, 16-byte loads and stores when VEC
+// (textures and output 16-byte aligned), element by element otherwise and in the ragged tail.
+template <typename T>
+__host__ __device__ constexpr int lt_elems() { return LT_CTA * LT_VPT * (16 / (int)sizeof(T)); }
+
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(LT_CTA) k_nmr_light_fwd(LightArgs<T> A, T* __restrict__ out) {
+    constexpr int W = 16 / (int)sizeof(T);
+    constexpr int E = lt_elems<T>();
+    __shared__ T s_l[E / 3 + 2][3];  // n3 >= 3: at most E / 3 + 2 faces meet the range
+    const long long e0 = (long long)blockIdx.x * E;
+    const long long e1 = min(e0 + E, A.N);
+    const int fa = (int)(e0 / A.n3), nf = (int)((e1 - 1) / A.n3) - fa + 1;
+    for (int i = threadIdx.x; i < nf; i += LT_CTA) {
+        T l[3];
+        load_light<T>(A, fa + i, l, nullptr);
+        s_l[i][0] = l[0]; s_l[i][1] = l[1]; s_l[i][2] = l[2];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < LT_VPT; ++k) {
+        const long long e = e0 + ((long long)k * LT_CTA + threadIdx.x) * W;
+        if (e >= e1) break;
+        int fi = (int)(e / A.n3);
+        int r = (int)(e - (long long)fi * A.n3);
+        fi -= fa;
+        int ch = r % 3;
+        T x[W];
+        const bool full = VEC && e + W <= e1;
+        if (full) {
+            if constexpr (sizeof(T) == 4) {
+                const float4 t = __ldg(reinterpret_cast<const float4*>(A.tex + e));
+                x[0] = t.x; x[1] = t.y; x[2] = t.z; x[3] = t.w;
+            } else {
+                const double2 t = __ldg(reinterpret_cast<const double2*>(A.tex + e));
+                x[0] = t.x; x[1] = t.y;
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < W; ++j) x[j] = e + j < e1 ? __ldg(A.tex + e + j) : T(0);
+        }
+#pragma unroll
+        for (int j = 0; j < W; ++j) {
+            if (e + j < e1) x[j] = x[j] * s_l[fi][ch];
+            if (++r == A.n3) { r = 0; ++fi; }
+            ch = ch == 2 ? 0 : ch + 1;  // n3 is a multiple of 3: a face starts on channel 0
+        }
+        if (full) {
+            if constexpr (sizeof(T) == 4) *reinterpret_cast<float4*>(out + e) = make_float4(x[0], x[1], x[2], x[3]);
+            else *reinterpret_cast<double2*>(out + e) = make_double2(x[0], x[1]);
+        } else {
+#pragma unroll
+            for (int j = 0; j < W; ++j)
+                if (e + j < e1) out[e + j] = x[j];
+        }
+    }
+}
+
+// Backward: one warp per (image, face), the only writer of that face's outputs.  grad_tex = light * g; per channel
+// s_c = sum of tex * g, each lane over its elements in ascending order, then a fixed xor-shuffle tree.  Lane 0 chains
+// s through the light (relu, normalize, cross) into grad_faces [B,F,3,3] and the per-face partials of the light
+// parameters, part [B][9][F] (ca, cd, dir), reduced by k_nmr_light_reduce.  No atomics.
+template <typename T>
+__global__ void __launch_bounds__(256) k_nmr_light_bwd(LightArgs<T> A, long long nface, const T* __restrict__ g,
+                                                       T* __restrict__ grad_tex, T* __restrict__ grad_faces,
+                                                       T* __restrict__ part) {
+    const int lane = threadIdx.x & 31;
+    const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (gw >= nface) return;  // whole warps
+    const int bf = (int)gw;
+    T l[3];
+    LightParts<T> q;
+    load_light<T>(A, bf, l, &q);
+    const size_t base = (size_t)bf * A.n3;
+    const bool need_s = grad_faces || part;
+    // lane l's elements l + 32 k: channel (l + 2 k) mod 3, so phase k mod 3 keeps one channel per lane
+    T acc[3] = {T(0), T(0), T(0)};
+    for (int k0 = 0; lane + 32 * k0 < A.n3; k0 += 3) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            const int e = lane + 32 * (k0 + j);
+            if (e < A.n3) {
+                const int ch = (lane + 2 * j) % 3;
+                const T gv = __ldg(g + base + e);
+                if (grad_tex) grad_tex[base + e] = l[ch] * gv;
+                if (need_s) acc[j] = acc[j] + __ldg(A.tex + base + e) * gv;
+            }
+        }
+    }
+    if (!need_s) return;
+    T s[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        // the phase j that holds channel c on this lane: (lane + 2 j) mod 3 == c
+        const int j = ((c - lane % 3 + 3) * 2) % 3;
+        s[c] = j == 0 ? acc[0] : (j == 1 ? acc[1] : acc[2]);
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) s[c] = s[c] + __shfl_xor_sync(0xffffffffu, s[c], off);
+    }
+    if (lane != 0) return;
+    const int b = bf / A.F, f = bf - b * A.F;
+    T gcs = T(0), gca[3], gcd[3], gdir[3], gv[3][3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        gca[c] = A.Ia != T(0) ? A.Ia * s[c] : T(0);
+        gcd[c] = A.Id != T(0) ? (A.Id * s[c]) * q.cs : T(0);
+        if (A.Id != T(0)) gcs = gcs + (A.Id * s[c]) * __ldg(A.cd + (size_t)b * A.scd + c);
+    }
+    if (A.Id != T(0)) {
+        const T gnd = q.cs <= T(0) ? T(0) : gcs;  // relu: no gradient where the output is 0 (NaN passes)
+        T gn[3], gc[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            gdir[k] = gnd * q.n[k];
+            gn[k] = gnd * __ldg(A.dir + (size_t)b * A.sdir + k);
+        }
+        // normalize: n = c / max(|c|, eps); the norm's gradient passes only where |c| >= eps
+        const T t = (gn[0] * q.n[0] + gn[1] * q.n[1]) + gn[2] * q.n[2];
+        const bool pass = q.nrm >= light_eps<T>();
+#pragma unroll
+        for (int k = 0; k < 3; ++k) gc[k] = (pass ? gn[k] - t * q.n[k] : gn[k]) / q.den;
+        // c = a x b: grad a = b x gc, grad b = gc x a; v0 = a + v1, v2 = b + v1
+        const T* a = q.a;
+        const T* bb = q.b;
+        const T ga[3] = {bb[1] * gc[2] - bb[2] * gc[1], bb[2] * gc[0] - bb[0] * gc[2], bb[0] * gc[1] - bb[1] * gc[0]};
+        const T gb[3] = {gc[1] * a[2] - gc[2] * a[1], gc[2] * a[0] - gc[0] * a[2], gc[0] * a[1] - gc[1] * a[0]};
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            gv[0][k] = ga[k];
+            gv[1][k] = -ga[k] - gb[k];
+            gv[2][k] = gb[k];
+        }
+    } else {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) { gdir[k] = T(0); gv[0][k] = gv[1][k] = gv[2][k] = T(0); }
+    }
+    if (grad_faces) {
+        T* o = grad_faces + (size_t)bf * 9;
+#pragma unroll
+        for (int k = 0; k < 9; ++k) o[k] = gv[k / 3][k % 3];
+    }
+    if (part) {
+        T* p = part + (size_t)b * 9 * A.F + f;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            p[(size_t)c * A.F] = gca[c];
+            p[(size_t)(3 + c) * A.F] = gcd[c];
+            p[(size_t)(6 + c) * A.F] = gdir[c];
+        }
+    }
+}
+
+// grad_light [B,9] = sum over f ascending of part[b][k][f], one warp per (image, k).  The lanes load tiles of
+// 32 * LR_TILE consecutive partials, the next tile in flight while every lane folds the current one in ascending order
+// from shuffles; only the F adds are serial.  It runs only when a light parameter needs a gradient.
+constexpr int LR_TILE = 8;
+
+template <typename T>
+__global__ void __launch_bounds__(128) k_nmr_light_reduce(const T* __restrict__ part, T* __restrict__ grad_light, int B,
+                                                          int F) {
+    const int lane = threadIdx.x & 31;
+    const long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (w >= (long long)B * 9) return;  // whole warps
+    const T* p = part + (size_t)w * F;
+    auto load = [&](T x[LR_TILE], int f0) {
+#pragma unroll
+        for (int j = 0; j < LR_TILE; ++j) {
+            const int f = f0 + 32 * j + lane;
+            x[j] = f < F ? __ldg(p + f) : T(0);
+        }
+    };
+    T s = T(0), x[LR_TILE], nx[LR_TILE];
+    load(x, 0);
+    for (int f0 = 0; f0 < F; f0 += 32 * LR_TILE) {
+        load(nx, f0 + 32 * LR_TILE);
+        if (F - f0 >= 32 * LR_TILE) {
+#pragma unroll
+            for (int j = 0; j < LR_TILE; ++j)
+#pragma unroll
+                for (int l = 0; l < 32; ++l) s = s + __shfl_sync(0xffffffffu, x[j], l);
+        } else {
+#pragma unroll
+            for (int j = 0; j < LR_TILE; ++j)
+                for (int l = 0; l < 32 && f0 + 32 * j + l < F; ++l) s = s + __shfl_sync(0xffffffffu, x[j], l);
+        }
+#pragma unroll
+        for (int j = 0; j < LR_TILE; ++j) x[j] = nx[j];
+    }
+    if (lane == 0) grad_light[w] = s;
+}
+
+// ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
 static int check(const UmrNmrParams* p, bool need_tex) {
@@ -905,4 +1169,119 @@ extern "C" int umr_nmr_backward_faces(const float* vertices, const int32_t* face
     k_nmr_grad_faces<<<(unsigned)((nthr + 255) / 256), 256, 0, stream>>>(rec, box, G, grad_face_vertices, eps, K);
     umr::count_launch();
     return (int)cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------
+// lighting (include/umr_b200.h, DESIGN.md §15)
+// ---------------------------------------------------------------------------------------------
+static int light_check(const UmrNmrLightParams* p, long long& n3, long long& N) {
+    if (!p) return UMR_ERR_BAD_ARG;
+    if (p->batch_size < 1 || p->num_faces < 1 || p->texture_res < 1 || p->reserved != 0) return UMR_ERR_BAD_ARG;
+    if (p->dtype != UMR_DTYPE_FLOAT32 && p->dtype != UMR_DTYPE_FLOAT64) return UMR_ERR_BAD_ARG;
+    for (int s : {p->color_ambient_bstride, p->color_directional_bstride, p->direction_bstride})
+        if (s != 0 && s != 3) return UMR_ERR_BAD_ARG;
+    const long long T = p->texture_res;
+    if (T > 1024) return UMR_ERR_TOO_LARGE;
+    n3 = T * T * T * 3;
+    if (n3 >= (1ll << 31)) return UMR_ERR_TOO_LARGE;
+    const long long BF = (long long)p->batch_size * p->num_faces;
+    if (BF * 9 >= (1ll << 31) || BF * n3 >= (1ll << 31)) return UMR_ERR_TOO_LARGE;
+    N = BF * n3;
+    return UMR_OK;
+}
+
+static bool aligned(const void* ptr, size_t a) { return ((uintptr_t)ptr & (a - 1)) == 0; }
+
+template <typename T>
+static LightArgs<T> light_args(const void* faces, const void* textures, const void* ca, const void* cd, const void* dir,
+                               const UmrNmrLightParams* p, long long n3, long long N) {
+    LightArgs<T> A;
+    A.faces = (const T*)faces;
+    A.tex = (const T*)textures;
+    A.ca = (const T*)ca;
+    A.cd = (const T*)cd;
+    A.dir = (const T*)dir;
+    A.sca = p->color_ambient_bstride;
+    A.scd = p->color_directional_bstride;
+    A.sdir = p->direction_bstride;
+    A.F = p->num_faces;
+    A.n3 = (int)n3;
+    A.N = N;
+    A.Ia = (T)p->intensity_ambient;
+    A.Id = (T)p->intensity_directional;
+    return A;
+}
+
+template <typename T>
+static int light_forward(const LightArgs<T>& A, T* out, cudaStream_t stream) {
+    const unsigned grid = (unsigned)((A.N + lt_elems<T>() - 1) / lt_elems<T>());
+    if (aligned(A.tex, 16) && aligned(out, 16)) k_nmr_light_fwd<T, true><<<grid, LT_CTA, 0, stream>>>(A, out);
+    else k_nmr_light_fwd<T, false><<<grid, LT_CTA, 0, stream>>>(A, out);
+    umr::count_launch();
+    return (int)cudaGetLastError();
+}
+
+template <typename T>
+static int light_backward(const LightArgs<T>& A, int B, const T* g, T* grad_faces, T* grad_tex, T* grad_light, T* part,
+                          cudaStream_t stream) {
+    const long long nface = (long long)B * A.F;
+    k_nmr_light_bwd<T><<<(unsigned)((nface * 32 + 255) / 256), 256, 0, stream>>>(A, nface, g, grad_tex, grad_faces,
+                                                                                  grad_light ? part : nullptr);
+    umr::count_launch();
+    if (grad_light) {
+        k_nmr_light_reduce<T><<<(unsigned)(((long long)B * 9 * 32 + 127) / 128), 128, 0, stream>>>(part, grad_light, B, A.F);
+        umr::count_launch();
+    }
+    return (int)cudaGetLastError();
+}
+
+extern "C" size_t umr_sizeof_nmr_light_params(void) { return sizeof(UmrNmrLightParams); }
+
+extern "C" size_t umr_nmr_lighting_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t dtype) {
+    if (batch_size < 1 || num_faces < 1 || (dtype != UMR_DTYPE_FLOAT32 && dtype != UMR_DTYPE_FLOAT64)) return 0;
+    const long long BF = (long long)batch_size * num_faces;
+    if (BF * 9 >= (1ll << 31)) return 0;
+    return align256((size_t)BF * 9 * (dtype == UMR_DTYPE_FLOAT64 ? sizeof(double) : sizeof(float)));
+}
+
+extern "C" int umr_nmr_lighting_forward(const void* faces, const void* textures, const void* color_ambient,
+                                        const void* color_directional, const void* direction, void* lit_textures,
+                                        const UmrNmrLightParams* p, void* stream_) {
+    long long n3 = 0, N = 0;
+    int rc = light_check(p, n3, N);
+    if (rc) return rc;
+    const size_t es = p->dtype == UMR_DTYPE_FLOAT64 ? sizeof(double) : sizeof(float);
+    for (const void* b : {faces, textures, color_ambient, color_directional, direction, (const void*)lit_textures})
+        if (!b || !aligned(b, es)) return UMR_ERR_BAD_ARG;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    if (p->dtype == UMR_DTYPE_FLOAT64)
+        return light_forward(light_args<double>(faces, textures, color_ambient, color_directional, direction, p, n3, N),
+                             (double*)lit_textures, stream);
+    return light_forward(light_args<float>(faces, textures, color_ambient, color_directional, direction, p, n3, N),
+                         (float*)lit_textures, stream);
+}
+
+extern "C" int umr_nmr_lighting_backward(const void* faces, const void* textures, const void* color_ambient,
+                                         const void* color_directional, const void* direction, const void* grad_lit,
+                                         void* grad_faces, void* grad_textures, void* grad_light,
+                                         const UmrNmrLightParams* p, void* workspace, void* stream_) {
+    long long n3 = 0, N = 0;
+    int rc = light_check(p, n3, N);
+    if (rc) return rc;
+    const size_t es = p->dtype == UMR_DTYPE_FLOAT64 ? sizeof(double) : sizeof(float);
+    for (const void* b : {faces, textures, color_ambient, color_directional, direction, grad_lit})
+        if (!b || !aligned(b, es)) return UMR_ERR_BAD_ARG;
+    if (!grad_faces && !grad_textures && !grad_light) return UMR_ERR_BAD_ARG;
+    for (const void* b : {(const void*)grad_faces, (const void*)grad_textures, (const void*)grad_light})
+        if (b && !aligned(b, es)) return UMR_ERR_BAD_ARG;
+    if (grad_light && (!workspace || !aligned(workspace, 256))) return UMR_ERR_BAD_ARG;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const int B = p->batch_size;
+    if (p->dtype == UMR_DTYPE_FLOAT64)
+        return light_backward(light_args<double>(faces, textures, color_ambient, color_directional, direction, p, n3, N),
+                              B, (const double*)grad_lit, (double*)grad_faces, (double*)grad_textures,
+                              (double*)grad_light, (double*)workspace, stream);
+    return light_backward(light_args<float>(faces, textures, color_ambient, color_directional, direction, p, n3, N), B,
+                          (const float*)grad_lit, (float*)grad_faces, (float*)grad_textures, (float*)grad_light,
+                          (float*)workspace, stream);
 }

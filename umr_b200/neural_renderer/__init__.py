@@ -31,12 +31,22 @@ Equivalence of this contract to the upstream package is not verified (its source
 The functional rasterisers (`rasterize_rgbad`, `rasterize`, `rasterize_silhouettes`, `rasterize_depth`,
 `vertices_to_faces`; rasterize.py) take face coordinates already in NDC and give them NMR's approximate geometry
 gradient (DESIGN.md §14).  `Renderer` keeps its texture-only gradient.
+
+The functions that produce their inputs complete NMR's functional pipeline (DESIGN.md §15): the cameras `look_at`,
+`look`, `perspective`, `projection` and `get_points_from_angles` (camera.py, torch), `lighting` (lighting.py, sm_90a
+kernels, float32 and float64, returning a new tensor where upstream multiplies the textures in place) and `load_obj` /
+`save_obj` for geometry (obj_io.py).  An NMR example then runs as: load_obj, get_points_from_angles, look_at,
+perspective, lighting on the world-space faces, vertices_to_faces, rasterize.
 """
 from .rasterize import (DEFAULT_ANTI_ALIASING, DEFAULT_BACKGROUND_COLOR, DEFAULT_EPS, DEFAULT_FAR, DEFAULT_IMAGE_SIZE,
                         DEFAULT_NEAR, rasterize, rasterize_depth, rasterize_rgbad, rasterize_silhouettes,
                         vertices_to_faces)
+from .camera import get_points_from_angles, look, look_at, perspective, projection
+from .lighting import lighting
+from .obj_io import load_obj, save_obj
 from .renderer import Renderer
 
 __all__ = ["Renderer", "rasterize_rgbad", "rasterize", "rasterize_silhouettes", "rasterize_depth", "vertices_to_faces",
+           "look_at", "look", "perspective", "projection", "get_points_from_angles", "lighting", "load_obj", "save_obj",
            "DEFAULT_IMAGE_SIZE", "DEFAULT_ANTI_ALIASING", "DEFAULT_NEAR", "DEFAULT_FAR", "DEFAULT_EPS",
            "DEFAULT_BACKGROUND_COLOR"]
