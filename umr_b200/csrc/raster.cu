@@ -241,7 +241,7 @@ __device__ __forceinline__ void red_p2f_fixed(unsigned long long* acc, float x, 
 // ---------------------------------------------------------------------------------------------
 // tile machinery shared by forward and backward
 // ---------------------------------------------------------------------------------------------
-constexpr int PT = 16;          // pixel-tile side of the pair-parallel backward kernel (32 is the A/B alternative)
+constexpr int PT = 16;          // pixel-tile side of the pair-parallel backward kernel
 static_assert(PT * PT == CTA, "k_raster_bwd_det stages one per-pixel slot per thread; bwd_pair_acc reads them with stride PT * PT");
 constexpr int BOX_PIECE = 2048;  // cull boxes staged per TMA bulk copy (32 KB)
 
@@ -942,7 +942,7 @@ __device__ __forceinline__ void bwd_pairs_tile(const float* __restrict__ rec_all
     uint16_t* s_list = reinterpret_cast<uint16_t*>(smem_raw + smem_list_off(K.F));
     __shared__ int s_warp_cnt[NWARP];
     __shared__ float s_ext[4];
-    // PT x PT pixel tile (PT = 32 puts 4x the pairs in a chunk).
+    // PT x PT pixel tile.
     using PP = PixPlanes<RGB, NC>;
     constexpr int NPL = PP::NPL, NV = PP::NV;
     __shared__ float s_pix[NV][PT * PT];   // g[NC], g_alpha, C[NC], alpha, ssum, smax of the tile's pixels (row-major; PixPlanes)
@@ -1193,32 +1193,12 @@ __global__ void k_p2f_finalize_det(const unsigned long long* __restrict__ acc, f
 #include "raster_fwd3.cuh"
 #include "raster_fwd4.cuh"
 
+#include "raster_host.cuh"
+
 // =============================================================================================
 // C ABI
 // =============================================================================================
 using namespace umr;
-
-// k_raster_bwd2 instantiation for the call: texture-only (grad_faces == NULL) and warp-level texel pre-reduction variants
-// exist for the texture-gradient kernels only; SP: the split backward (softmax, both gradients)
-template <int RGBM, bool TG, int TS, typename IdxT, bool SP = false>
-static void launch_bwd2(dim3 grid, cudaStream_t stream, bool pre, const float* rec, const float* textures, const float* soft_colors,
-                        const float* aggrs_info, const float* grad_images, float* grad_faces, float* grad_textures,
-                        const Consts<float>& K, const PairBuf& pb) {
-#define UMR_BWD2_GO(GEOMV, PREV) \
-    k_raster_bwd2<RGBM, TG, TS, 3, GEOMV, PREV, IdxT, SP><<<grid, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, \
-                                                                                        grad_images, grad_faces, grad_textures, K, pb)
-    if constexpr (SP) {
-        if (pre) UMR_BWD2_GO(true, true); else UMR_BWD2_GO(true, false);
-    } else if constexpr (TG && RGBM == 1) {
-        if (pre) { if (grad_faces) UMR_BWD2_GO(true, true); else UMR_BWD2_GO(false, true); }
-        else { if (grad_faces) UMR_BWD2_GO(true, false); else UMR_BWD2_GO(false, false); }
-    } else if constexpr (TG) {
-        if (grad_faces) UMR_BWD2_GO(true, false); else UMR_BWD2_GO(false, false);
-    } else {
-        UMR_BWD2_GO(true, false);
-    }
-#undef UMR_BWD2_GO
-}
 
 // Which forward serves the UMR configuration: 4 = k_raster_fwd4 (32x32 tiles, dynamic 8x4 pixel blocks; tile list in
 // shared memory sized by F, longer coarse lists take a windowed slow path), 3 = k_raster_fwd3 (16x16 tiles, windowed
@@ -1254,8 +1234,7 @@ static int pair_texel_bits(const UmrRasterParams* p) {
 // device pointers into the caller's pair buffer (cap == 0: no saving; also when T2 does not fit the record's texel field,
 // so the backward recomputes every tile)
 static PairBuf make_pairbuf(const UmrRasterParams* p, int S) {
-    PairBuf pb;
-    pb.ctrl = nullptr; pb.tile_head = nullptr; pb.ulist = nullptr; pb.blk_hdr = nullptr; pb.recs = nullptr; pb.cap = 0;
+    PairBuf pb{};
     if (!p->pair_buffer || p->pair_buffer_bytes == 0 || ((uintptr_t)p->pair_buffer & 255) != 0) return pb;
     if (p->texture_size > (1 << pair_texel_bits(p))) return pb;
     size_t cap = pair_capacity(p->batch_size, S, (size_t)p->pair_buffer_bytes);
@@ -1276,57 +1255,6 @@ static PairBuf make_pairbuf(const UmrRasterParams* p, int S) {
 // It only pays for very large faces; every UMR shape is far below the thresholds (6 at C2, 23 at C5, 91 at C3), where the
 // plain vector REDs are faster.
 constexpr double TEXGRAD_PRE_RATIO_FULL = 160.0, TEXGRAD_PRE_RATIO_TEXONLY = 120.0;
-static bool is_generic(const UmrRasterParams* p);
-static int check_params(const UmrRasterParams* p) {
-    if (!p) return UMR_ERR_BAD_ARG;
-    if (p->batch_size <= 0 || p->num_faces <= 0 || p->texture_size <= 0 || p->image_size <= 0)
-        return UMR_ERR_BAD_ARG;
-    if (p->num_faces > UMR_RASTER_MAX_FACES || p->batch_size > 65535) return UMR_ERR_TOO_LARGE;
-    if (p->func_id_dist < 0 || p->func_id_dist > 2 || p->func_id_alpha < 0 || p->func_id_alpha > 2 ||
-        p->texture_sample_type < 0 || p->texture_sample_type > 1)
-        return UMR_ERR_UNSUPPORTED;
-    if (p->texture_sample_type == UMR_TEX_VERTEX && p->texture_size != 3) return UMR_ERR_BAD_ARG;  // [B,F,3,3]
-    if (p->shared_textures > 1 && p->batch_size % p->shared_textures != 0) return UMR_ERR_BAD_ARG;
-    if (p->func_id_rgb != UMR_RGB_HARD && p->func_id_rgb != UMR_RGB_SOFTMAX) return UMR_ERR_UNSUPPORTED;
-    if (p->color_channels != 0 && p->color_channels != 3 && p->color_channels != 4) return UMR_ERR_BAD_ARG;
-    // 4 colour channels (the part-map render): UMR's own configuration only
-    if (p->color_channels == 4 && (is_generic(p) || p->func_id_rgb != UMR_RGB_SOFTMAX)) return UMR_ERR_UNSUPPORTED;
-    return UMR_OK;
-}
-
-// the UMR configuration has specialised kernels; every other mode combination takes the generic ones
-static bool is_generic(const UmrRasterParams* p) {
-    return p->func_id_dist != UMR_DIST_EUCLIDEAN || p->func_id_alpha != UMR_ALPHA_PROD ||
-           p->texture_sample_type != UMR_TEX_SURFACE;
-}
-
-static Consts<float> make_consts(const UmrRasterParams* p) {
-    Consts<float> K;
-    K.thr = p->dist_eps * p->sigma_val;  // kernel.cu:333 (float * float)
-    K.sigma = p->sigma_val;
-    K.gamma = p->gamma_val;
-    K.near_ = p->near_plane;
-    K.far_ = p->far_plane;
-    K.inv_unused = 0.f;
-    K.r_sigma = (float)(1.0 / (double)p->sigma_val);
-    K.r_gamma = (float)(1.0 / (double)p->gamma_val);
-    K.r_fn = (float)(1.0 / ((double)p->far_plane - (double)p->near_plane));
-    K.r_nf = (float)(1.0 / ((double)p->near_plane - (double)p->far_plane));
-    K.F = p->num_faces;
-    K.T2 = p->texture_size;
-    K.R = (int)sqrt((double)p->texture_size);  // kernel.cu:685
-    K.IS = p->image_size;
-    K.aa = p->anti_aliasing ? 1 : 0;
-    K.S = p->image_size * (K.aa ? 2 : 1);
-    K.double_side = p->double_side ? 1 : 0;
-    K.dist = p->func_id_dist;
-    K.alpha = p->func_id_alpha;
-    K.tex = p->texture_sample_type;
-    K.vec_store = 0;
-    K.tex_bs = (size_t)p->num_faces * p->texture_size * (p->color_channels == 4 ? 4 : 3);
-    K.tex_div = p->shared_textures > 1 ? p->shared_textures : 1;
-    return K;
-}
 
 // Opt every raster kernel into the full dynamic shared-memory range ONCE per device (not per call:
 // the call may be inside a CUDA-graph capture).  A 65536-face window needs 8 KB + 32 KB + 128 KB.
@@ -1339,26 +1267,27 @@ static int ensure_smem_attrs() {
     int optin = 0;
     e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     if (e != cudaSuccess) return (int)e;
-    cudaFuncAttributes fa;
-#define UMR_SET(K)                                                                                  \
-    e = cudaFuncGetAttributes(&fa, K);                                                               \
-    if (e != cudaSuccess) return (int)e;                                                             \
-    e = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize,                         \
-                             optin - (int)fa.sharedSizeBytes);                                       \
-    if (e != cudaSuccess) return (int)e;
-    UMR_SET((k_raster_fwd<0>)) UMR_SET((k_raster_fwd<1>)) UMR_SET((k_raster_fwd<1, true>))
-    UMR_SET((k_raster_fwd4<0>)) UMR_SET((k_raster_fwd4<1>))
-    UMR_SET((k_raster_fwd4<0, uint32_t>)) UMR_SET((k_raster_fwd4<1, uint32_t>))
-    UMR_SET((k_raster_bwd<0, false>)) UMR_SET((k_raster_bwd<0, true>))
-    UMR_SET((k_raster_bwd<1, false>)) UMR_SET((k_raster_bwd<1, true>))
-    UMR_SET((k_raster_bwd_pairs<0, false>)) UMR_SET((k_raster_bwd_pairs<0, true>))
-    UMR_SET((k_raster_bwd_pairs<1, false>)) UMR_SET((k_raster_bwd_pairs<1, true>))
-    UMR_SET((k_raster_bwd_pairs_list<0, false>)) UMR_SET((k_raster_bwd_pairs_list<0, true>))
-    UMR_SET((k_raster_bwd_pairs_list<1, false>)) UMR_SET((k_raster_bwd_pairs_list<1, true>))
-    UMR_SET((k_raster_bwd_pairs<1, true, 3, true>)) UMR_SET((k_raster_bwd_pairs_list<1, true, 3, true>))
-    UMR_SET((k_raster_fwd4<RGB_SIL>)) UMR_SET((k_raster_fwd4<RGB_SIL, uint32_t>))
-    UMR_SET((k_raster_bwd_pairs<RGB_SIL, false>)) UMR_SET((k_raster_bwd_pairs_list<RGB_SIL, false>))
-#undef UMR_SET
+    const void* const kernels[] = {
+        (const void*)k_raster_fwd<0>, (const void*)k_raster_fwd<1>, (const void*)k_raster_fwd<1, true>,
+        (const void*)k_raster_fwd4<0>, (const void*)k_raster_fwd4<1>,
+        (const void*)k_raster_fwd4<0, uint32_t>, (const void*)k_raster_fwd4<1, uint32_t>,
+        (const void*)k_raster_bwd<0, false>, (const void*)k_raster_bwd<0, true>,
+        (const void*)k_raster_bwd<1, false>, (const void*)k_raster_bwd<1, true>,
+        (const void*)k_raster_bwd_pairs<0, false>, (const void*)k_raster_bwd_pairs<0, true>,
+        (const void*)k_raster_bwd_pairs<1, false>, (const void*)k_raster_bwd_pairs<1, true>,
+        (const void*)k_raster_bwd_pairs_list<0, false>, (const void*)k_raster_bwd_pairs_list<0, true>,
+        (const void*)k_raster_bwd_pairs_list<1, false>, (const void*)k_raster_bwd_pairs_list<1, true>,
+        (const void*)k_raster_bwd_pairs<1, true, 3, true>, (const void*)k_raster_bwd_pairs_list<1, true, 3, true>,
+        (const void*)k_raster_fwd4<RGB_SIL>, (const void*)k_raster_fwd4<RGB_SIL, uint32_t>,
+        (const void*)k_raster_bwd_pairs<RGB_SIL, false>, (const void*)k_raster_bwd_pairs_list<RGB_SIL, false>,
+    };
+    for (const void* k : kernels) {
+        cudaFuncAttributes fa;
+        e = cudaFuncGetAttributes(&fa, k);
+        if (e != cudaSuccess) return (int)e;
+        e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, optin - (int)fa.sharedSizeBytes);
+        if (e != cudaSuccess) return (int)e;
+    }
     done[dev] = true;
     return 0;
 }
@@ -1384,140 +1313,231 @@ static size_t raster_dyn_smem(int F) {
     return smem_list_off(F) + (((size_t)W * 2 + 15) & ~(size_t)15);
 }
 
-// Coarse binning for the UMR-configuration kernels: u16 lists of F entries per bin, or (F > 65535) the wide pool, whose
-// cursor is reset first.
-static int launch_bin_coarse(const float4* box, const uint32_t* ubox, void* clist, int* ccount, int B, int F, int S,
-                             const WorkspaceLayout& L, cudaStream_t stream) {
-    const int ncb = (S + CB - 1) / CB;
-    const size_t smem = (size_t)(F < BOX_PIECE ? F : BOX_PIECE) * 16;
-    if (F <= NARROW_MAX_FACES) {
-        k_bin_coarse<uint16_t><<<dim3(ncb, ncb, B), CTA, smem, stream>>>(box, ubox, (uint16_t*)clist, ccount, F, S);
-        return 0;
-    }
-    const size_t nbin = (size_t)B * ncb * ncb;
-    cudaError_t e = cudaMemsetAsync(ccount + 2 * nbin, 0, sizeof(unsigned long long), stream);
-    if (e != cudaSuccess) return (int)e;
-    k_bin_coarse<uint32_t><<<dim3(ncb, ncb, B), CTA, smem, stream>>>(box, ubox, (uint32_t*)clist, ccount, F, S, L.clist_cap);
-    return 0;
-}
-
 // Deterministic-mode workspace: the default layout, then the fixed-point p2f accumulators (P2F_DET_WORDS int64 per face).
 static size_t det_acc_bytes(int B, int F) { return align256((size_t)B * F * P2F_DET_WORDS * sizeof(unsigned long long)); }
-// Rasters past the launch limit of the 16x16-tile grid (gridDim.y <= 65535) are refused; the p2f limb bound holds below it.
-constexpr int DET_MAX_RASTER = 65535 * TILE;
 
 extern "C" size_t umr_raster_workspace_bytes_deterministic(int32_t B, int32_t F, int32_t image_size, int32_t anti_aliasing) {
     if (B <= 0 || F <= 0 || image_size <= 0) return 0;
     return umr_raster_workspace_bytes(B, F, image_size, anti_aliasing) + det_acc_bytes(B, F);
 }
 
-// det: the deterministic mode (UMR's configuration only): 16x16-tile forward whatever tile_mode says, no pair buffer,
-// fixed-point p2f accumulators after the default workspace layout
-static int raster_forward(const float* face_vertices, const float* textures, float* images, float* soft_colors,
-                          float* aggrs_info, float* p2f_info, const UmrRasterParams* p, void* workspace, void* stream_,
-                          bool det) {
-    int rc = check_params(p);
-    if (rc) return rc;
-    if (det && (int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;
-    if (!face_vertices || !textures || !images || !aggrs_info || !workspace) return UMR_ERR_BAD_ARG;
-    if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
-    cudaStream_t stream = (cudaStream_t)stream_;
-    rc = ensure_smem_attrs();
-    if (rc) return rc;
-    const int B = p->batch_size, F = p->num_faces;
-    Consts<float> K = make_consts(p);
-    if (!K.aa && soft_colors == nullptr) soft_colors = images;
-    K.vec_store = (K.aa && (K.S % 8) == 0 && (((uintptr_t)images | (uintptr_t)soft_colors | (uintptr_t)aggrs_info) & 15) == 0) ? 1 : 0;
-    const WorkspaceLayout L = ws_layout(B, F, K.S);
+// What a float32 call derives from its parameters and workspace.  The pair backward's tiles are the forward's 16x16 ones.
+static_assert(PT == TILE, "grid16 serves the 16x16-tile forward and the pair backward");
+struct RasterCall {
+    const UmrRasterParams* p;
+    cudaStream_t stream;
+    int B, F, S;
+    bool wide;     // F > NARROW_MAX_FACES: the 32-bit face-index instantiations
+    bool gen;      // a generic mode (is_generic)
+    bool softmax;  // softmax colours (else hard)
+    bool nc4;      // the 4-channel part-map render
+    Consts<float> K;
+    WorkspaceLayout L;
+    float* rec;
+    float4* box;
+    uint32_t* ubox;
+    int* ccount;
+    void* clist;
+    PairBuf pb;          // cap == 0: no pair records saved or read
+    dim3 grid16, grid32;  // 16x16 and 32x32 tiles of the raster
+    int ncb;             // coarse bins per raster side
+};
+
+// pairs: the call may use the caller's pair buffer (the default mode in UMR's configuration)
+static RasterCall raster_call(const UmrRasterParams* p, void* workspace, void* stream, bool pairs) {
+    RasterCall c;
+    c.p = p;
+    c.stream = (cudaStream_t)stream;
+    c.K = make_consts<float>(p);
+    c.B = p->batch_size;
+    c.F = p->num_faces;
+    c.S = c.K.S;
+    c.wide = c.F > NARROW_MAX_FACES;
+    c.gen = is_generic(p);
+    c.softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
+    c.nc4 = p->color_channels == 4;
+    c.L = ws_layout(c.B, c.F, c.S);
     char* ws = (char*)workspace;
-    float* rec = (float*)(ws + L.rec_off);
-    float4* box = (float4*)(ws + L.box_off);
-    float* p2f_acc = (float*)(ws + L.p2f_off);
-    uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
-    int* ccount = (int*)(ws + L.ccount_off);
-    void* clist = ws + L.clist_off;
-    const bool wide = F > NARROW_MAX_FACES;
-    const size_t n = (size_t)B * F;
-    const float r = sqrtf(K.thr);  // kernel.cu:355 sqrt(threshold) in float
-    {
-        cudaError_t e0 = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
-        if (e0 != cudaSuccess) return (int)e0;
+    c.rec = (float*)(ws + c.L.rec_off);
+    c.box = (float4*)(ws + c.L.box_off);
+    c.ubox = (uint32_t*)(ws + c.L.ubox_off);
+    c.ccount = (int*)(ws + c.L.ccount_off);
+    c.clist = ws + c.L.clist_off;
+    c.pb = pairs ? make_pairbuf(p, c.S) : PairBuf{};
+    c.grid16 = dim3((c.S + TILE - 1) / TILE, (c.S + TILE - 1) / TILE, c.B);
+    c.grid32 = dim3((c.S + T4 - 1) / T4, (c.S + T4 - 1) / T4, c.B);
+    c.ncb = (c.S + CB - 1) / CB;
+    return c;
+}
+
+// The face records and the images' union cull boxes (zeroed first).  only_if_nonzero: k_prep returns at once when the
+// word it points to is 0 (records that only the recompute fallback reads, and no tile left for it).
+static int prep(const RasterCall& c, const float* face_vertices, const uint32_t* only_if_nonzero) {
+    cudaError_t e = cudaMemsetAsync(c.ubox, 0, (size_t)c.B * 4 * sizeof(uint32_t), c.stream);
+    if (e != cudaSuccess) return (int)e;
+    launch(k_prep, dim3((c.F + 255) / 256, c.B), 256, 0, c.stream, face_vertices, c.rec, c.box, c.ubox, c.F,
+           sqrtf(c.K.thr), only_if_nonzero);  // r: kernel.cu:355 sqrt(threshold) in float
+    return 0;
+}
+
+// Coarse binning for the UMR-configuration kernels, after the pair buffer's counters are reset: u16 lists of F entries per
+// bin, or (F > 65535) the wide pool, whose cursor is reset first.
+static int bin_coarse(const RasterCall& c) {
+    cudaError_t e = c.pb.cap > 0 ? cudaMemsetAsync(c.pb.ctrl, 0, 16, c.stream) : cudaSuccess;
+    if (e != cudaSuccess) return (int)e;
+    const dim3 grid(c.ncb, c.ncb, c.B);
+    const size_t smem = (size_t)(c.F < BOX_PIECE ? c.F : BOX_PIECE) * 16;
+    if (!c.wide) {
+        launch(k_bin_coarse<uint16_t>, grid, CTA, smem, c.stream, c.box, c.ubox, (uint16_t*)c.clist, c.ccount, c.F, c.S,
+               (size_t)0);
+        return 0;
     }
-    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, r);
-    count_launch();
-    const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
-    const bool want_p2f = p2f_info != nullptr;
-    if (det) p2f_acc = (float*)(ws + L.total);
-    if (want_p2f && softmax) {
-        cudaError_t e = cudaMemsetAsync(p2f_acc, 0, det ? n * P2F_DET_WORDS * sizeof(unsigned long long) : n * 4 * sizeof(float),
-                                        stream);
+    e = cudaMemsetAsync(c.ccount + 2 * (size_t)c.B * c.ncb * c.ncb, 0, sizeof(unsigned long long), c.stream);
+    if (e != cudaSuccess) return (int)e;
+    launch(k_bin_coarse<uint32_t>, grid, CTA, smem, c.stream, c.box, c.ubox, (uint32_t*)c.clist, c.ccount, c.F, c.S,
+           c.L.clist_cap);
+    return 0;
+}
+
+// f(IdxT{}) with the face-index type of the UMR-configuration kernels
+template <class Fn>
+static void with_index(bool wide, Fn&& f) {
+    if (wide) f(uint32_t{});
+    else f(uint16_t{});
+}
+
+// grid of the recompute backward's list-driven launch: 3 resident CTAs per SM walk the unsaved-tile list
+static int list_grid(const RasterCall& c, unsigned* grid) {
+    int sms = 0;
+    int rc = sm_count(&sms);
+    if (rc) return rc;
+    const size_t ntiles = (size_t)c.grid16.x * c.grid16.y * c.B, list_max = (size_t)3 * sms;
+    *grid = (unsigned)(ntiles < list_max ? ntiles : list_max);
+    return 0;
+}
+
+// zero the gradients the backward accumulates into (NULL: not computed, or written whole)
+static int zero_grads(const RasterCall& c, float* grad_faces, float* grad_textures) {
+    const size_t n = (size_t)c.B * c.F;
+    cudaError_t e = grad_faces ? cudaMemsetAsync(grad_faces, 0, n * 9 * sizeof(float), c.stream) : cudaSuccess;
+    if (e == cudaSuccess && grad_textures)
+        e = cudaMemsetAsync(grad_textures, 0, (n / c.K.tex_div) * c.p->texture_size * 3 * sizeof(float), c.stream);
+    return (int)e;
+}
+
+// the buffers of a float backward kernel (a silhouette's: its alpha plane and alpha gradient only)
+struct BwdArgs {
+    const float *textures, *colors_hi, *aggrs, *grad_images;
+    float *grad_faces, *grad_tex;
+};
+
+// k_raster_bwd2 for the call: texture-only (grad_faces == NULL) and warp-level texel pre-reduction variants exist for the
+// texture-gradient kernels only, the pre-reduction for softmax colours only; SP: the split backward (softmax, both gradients)
+template <int RGBM, bool TG, int NC, bool SP, int TS, typename IdxT>
+static void launch_bwd2(const RasterCall& c, dim3 grid, bool pre, const BwdArgs& a) {
+    auto go = [&](auto geom, auto prev) {
+        launch(k_raster_bwd2<RGBM, TG, TS, NC, decltype(geom)::value, decltype(prev)::value, IdxT, SP>, grid, BWD2_THREADS, 0,
+               c.stream, c.rec, a.textures, a.colors_hi, a.aggrs, a.grad_images, a.grad_faces, a.grad_tex, c.K, c.pb);
+    };
+    using Y = std::true_type;
+    using N = std::false_type;
+    const bool geom = a.grad_faces != nullptr;
+    if constexpr (SP) {
+        if (pre) go(Y{}, Y{}); else go(Y{}, N{});
+    } else if constexpr (TG && RGBM == 1) {
+        if (pre) { if (geom) go(Y{}, Y{}); else go(N{}, Y{}); }
+        else { if (geom) go(Y{}, N{}); else go(N{}, N{}); }
+    } else if constexpr (TG) {
+        if (geom) go(Y{}, N{}); else go(N{}, N{});
+    } else {
+        go(Y{}, N{});
+    }
+}
+
+// The backward of UMR's configuration.  With a pair buffer: the streamed backward over the pairs the forward saved, on the
+// forward's tiles (the 4-channel render's are always 16x16), then the recompute backward for the tiles it could not save;
+// without one, the recompute backward for every tile.
+template <int RGBM, bool TG, int NC, bool SP>
+static void launch_pairs_backward(const RasterCall& c, unsigned list_grid, bool pre, const BwdArgs& a) {
+    const size_t smem = raster_dyn_smem(c.F);
+    if (c.pb.cap == 0) {
+        launch(k_raster_bwd_pairs<RGBM, TG, NC, SP>, c.grid16, CTA, smem, c.stream, c.rec, c.box, a.textures, a.colors_hi,
+               a.aggrs, a.grad_images, a.grad_faces, a.grad_tex, c.ubox, c.K);
+        return;
+    }
+    with_index(c.wide, [&](auto idx) {
+        using IDX = decltype(idx);
+        if constexpr (NC == 3) {
+            if (forward_impl(c.p->tile_mode) == 4) {
+                launch_bwd2<RGBM, TG, NC, SP, 32, IDX>(c, c.grid32, pre, a);
+                return;
+            }
+        }
+        launch_bwd2<RGBM, TG, NC, SP, 16, IDX>(c, c.grid16, pre, a);
+    });
+    launch(k_raster_bwd_pairs_list<RGBM, TG, NC, SP>, list_grid, CTA, smem, c.stream, c.rec, c.box, a.textures, a.colors_hi,
+           a.aggrs, a.grad_images, a.grad_faces, a.grad_tex, c.ubox, c.K, c.pb.ctrl + 1, c.pb.ulist, (int)c.grid16.x,
+           (int)c.grid16.y);
+}
+
+// det: the deterministic mode (every mode check_params accepts): 16x16-tile forward whatever tile_mode says, no pair
+// buffer, fixed-point p2f accumulators after the default workspace layout
+static int raster_forward(const float* face_vertices, const float* textures, float* images, float* soft_colors,
+                          float* aggrs_info, float* p2f_info, const UmrRasterParams* p, void* workspace, void* stream,
+                          bool det) {
+    int rc = check_params<float>(p);
+    if (rc) return rc;
+    if (det && raster_side(p) > GATHER_MAX_RASTER) return UMR_ERR_TOO_LARGE;
+    if (!face_vertices || !textures || !images || !aggrs_info || !workspace) return UMR_ERR_BAD_ARG;
+    if (misaligned(workspace, 256)) return UMR_ERR_BAD_ARG;
+    if ((rc = ensure_smem_attrs())) return rc;
+    RasterCall c = raster_call(p, workspace, stream, !det && !is_generic(p));
+    if (!c.K.aa && soft_colors == nullptr) soft_colors = images;
+    c.K.vec_store = (c.K.aa && (c.S % 8) == 0 && (((uintptr_t)images | (uintptr_t)soft_colors | (uintptr_t)aggrs_info) & 15) == 0) ? 1 : 0;
+    if ((rc = prep(c, face_vertices, nullptr))) return rc;
+    // p2f sums: float accumulators in the workspace, or the deterministic mode's fixed-point words after it
+    const size_t n = (size_t)c.B * c.F;
+    void* acc = (char*)workspace + (det ? c.L.total : c.L.p2f_off);
+    float* pacc = (c.softmax && p2f_info) ? (float*)acc : nullptr;
+    if (pacc) {
+        cudaError_t e = cudaMemsetAsync(acc, 0, det ? n * P2F_DET_WORDS * sizeof(unsigned long long) : n * 4 * sizeof(float),
+                                        c.stream);
         if (e != cudaSuccess) return (int)e;
     }
-    const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
-    const size_t smem = raster_dyn_smem(F);
-    const bool gen = is_generic(p);
-    float* pacc = (softmax && want_p2f) ? p2f_acc : nullptr;
-    if (!gen) {
-        // round-2 pipeline: coarse bins -> tiled forward (saves pair records when a pair buffer is given)
-        const int ncb = (K.S + CB - 1) / CB;
-        const PairBuf pb = det ? PairBuf{nullptr, nullptr, nullptr, nullptr, nullptr, 0u} : make_pairbuf(p, K.S);
-        if (pb.cap > 0) {
-            cudaError_t e = cudaMemsetAsync(pb.ctrl, 0, 16, stream);
-            if (e != cudaSuccess) return (int)e;
-        }
-        count_launch(2);
-        rc = launch_bin_coarse(box, ubox, clist, ccount, B, F, K.S, L, stream);
-        if (rc) return rc;
-        if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-        const bool nc4 = p->color_channels == 4;
-        const int impl = (nc4 || det) ? 3 : forward_impl(p->tile_mode);
-#define UMR_FWD_ARGS(IDX) rec, box, (const IDX*)clist, ccount, textures, images, soft_colors, aggrs_info, pacc, ubox, K, p->eps, \
-                     p->background_color[0], p->background_color[1], p->background_color[2], pb, ncb
-#define UMR_FWD(IDX)                                                                                                        \
-        if (det && nc4) {                                                                                                   \
-            k_raster_fwd3<1, 4, IDX, true><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX), p->background_extra);               \
-        } else if (det && softmax) {                                                                                        \
-            k_raster_fwd3<1, 3, IDX, true><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX));                                    \
-        } else if (nc4) {                                                                                                   \
-            k_raster_fwd3<1, 4, IDX><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX), p->background_extra);                     \
-        } else if (impl == 3) {                                                                                             \
-            if (softmax) k_raster_fwd3<1, 3, IDX><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX));                             \
-            else k_raster_fwd3<0, 3, IDX><<<grid, CTA, 0, stream>>>(UMR_FWD_ARGS(IDX));                                     \
-        } else {                                                                                                            \
-            const dim3 grid32((K.S + T4 - 1) / T4, (K.S + T4 - 1) / T4, B);                                                 \
-            const size_t sm4 = fwd4_dyn_smem(F, sizeof(IDX));                                                               \
-            if (softmax) k_raster_fwd4<1, IDX><<<grid32, CTA, sm4, stream>>>(UMR_FWD_ARGS(IDX));                            \
-            else k_raster_fwd4<0, IDX><<<grid32, CTA, sm4, stream>>>(UMR_FWD_ARGS(IDX));                                    \
-        }
-        if (wide) { UMR_FWD(uint32_t) } else { UMR_FWD(uint16_t) }
-#undef UMR_FWD
-#undef UMR_FWD_ARGS
-        if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+    const float* bg = p->background_color;
+    if (c.gen) {
+        record(p->ev_kernel_start, c.stream);
+        launch(c.softmax ? (det ? k_raster_fwd<1, true> : k_raster_fwd<1>) : k_raster_fwd<0>, c.grid16, CTA,
+               raster_dyn_smem(c.F), c.stream, c.rec, c.box, textures, images, soft_colors, aggrs_info, pacc, c.ubox, c.K,
+               p->eps, bg[0], bg[1], bg[2]);
     } else {
-    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-    count_launch();
-#define UMR_LAUNCH_FWD(RGBM)                                                                                 \
-    if (det && RGBM == 1) k_raster_fwd<1, true><<<grid, CTA, smem, stream>>>(rec, box, textures, images, soft_colors,      \
-                                                    aggrs_info, pacc, ubox, K, p->eps, p->background_color[0],       \
-                                                    p->background_color[1], p->background_color[2]);                 \
-    else k_raster_fwd<RGBM><<<grid, CTA, smem, stream>>>(rec, box, textures, images, soft_colors, aggrs_info, pacc, ubox, \
-                                                    K, p->eps, p->background_color[0], p->background_color[1],       \
-                                                    p->background_color[2])
-    if (softmax) UMR_LAUNCH_FWD(1); else UMR_LAUNCH_FWD(0);
-#undef UMR_LAUNCH_FWD
-    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+        // coarse bins -> tiled forward (saves pair records when a pair buffer is given)
+        if ((rc = bin_coarse(c))) return rc;
+        record(p->ev_kernel_start, c.stream);
+        with_index(c.wide, [&](auto idx) {
+            using IDX = decltype(idx);
+            if (c.nc4 || det || forward_impl(p->tile_mode) == 3) {
+                auto fwd3 = c.nc4 ? (det ? k_raster_fwd3<1, 4, IDX, true> : k_raster_fwd3<1, 4, IDX>)
+                            : c.softmax ? (det ? k_raster_fwd3<1, 3, IDX, true> : k_raster_fwd3<1, 3, IDX>)
+                                        : k_raster_fwd3<0, 3, IDX>;
+                launch(fwd3, c.grid16, CTA, 0, c.stream, c.rec, c.box, (const IDX*)c.clist, c.ccount, textures, images,
+                       soft_colors, aggrs_info, pacc, c.ubox, c.K, p->eps, bg[0], bg[1], bg[2], c.pb, c.ncb,
+                       c.nc4 ? p->background_extra : 0.f, nullptr);
+            } else {
+                launch(c.softmax ? k_raster_fwd4<1, IDX> : k_raster_fwd4<0, IDX>, c.grid32, CTA, fwd4_dyn_smem(c.F, sizeof(IDX)),
+                       c.stream, c.rec, c.box, (const IDX*)c.clist, c.ccount, textures, images, soft_colors, aggrs_info, pacc,
+                       c.ubox, c.K, p->eps, bg[0], bg[1], bg[2], c.pb, c.ncb);
+            }
+        });
     }
-    if (want_p2f) {
-        if (softmax) {
-            count_launch();
-            if (det)
-                k_p2f_finalize_det<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>((const unsigned long long*)p2f_acc, p2f_info, n);
-            else
-                k_p2f_finalize<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p2f_acc, p2f_info, n);
-        } else {  // hard mode never accumulates p2f (kernel.cu:417-431 is softmax-only) -> zeros
-            cudaError_t e = cudaMemsetAsync(p2f_info, 0, n * 2 * sizeof(float), stream);
-            if (e != cudaSuccess) return (int)e;
-        }
+    record(p->ev_kernel_stop, c.stream);
+    if (pacc) {
+        const unsigned grid = (unsigned)((n + 255) / 256);
+        if (det) launch(k_p2f_finalize_det, grid, 256, 0, c.stream, (const unsigned long long*)acc, p2f_info, n);
+        else launch(k_p2f_finalize, grid, 256, 0, c.stream, (const float*)acc, p2f_info, n);
+    } else if (p2f_info) {  // hard mode never accumulates p2f (kernel.cu:417-431 is softmax-only) -> zeros
+        cudaError_t e = cudaMemsetAsync(p2f_info, 0, n * 2 * sizeof(float), c.stream);
+        if (e != cudaSuccess) return (int)e;
     }
     return (int)cudaGetLastError();
 }
@@ -1538,49 +1558,31 @@ extern "C" int umr_raster_forward_deterministic(const float* face_vertices, cons
 // (depth_min, float(face_index_min)) exactly as umr_raster_forward writes them with func_id_rgb = UMR_RGB_HARD.
 extern "C" int umr_raster_visibility(const float* face_vertices, float* aggrs_info, uint8_t* visible_faces,
                                      const UmrRasterParams* p, void* workspace, void* stream_) {
-    int rc = check_params(p);
+    int rc = check_params<float>(p);
     if (rc) return rc;
     if (!face_vertices || (!aggrs_info && !visible_faces) || !workspace) return UMR_ERR_BAD_ARG;
-    if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
+    if (misaligned(workspace, 256)) return UMR_ERR_BAD_ARG;
     if (is_generic(p)) return UMR_ERR_UNSUPPORTED;  // euclidean distance / prod alpha / surface textures: UMR's configuration
-    cudaStream_t stream = (cudaStream_t)stream_;
-    rc = ensure_smem_attrs();
-    if (rc) return rc;
-    const int B = p->batch_size, F = p->num_faces;
-    Consts<float> K = make_consts(p);
-    K.vec_store = (K.aa && (K.S % 8) == 0 && ((uintptr_t)aggrs_info & 15) == 0) ? 1 : 0;
-    const WorkspaceLayout L = ws_layout(B, F, K.S);
-    char* ws = (char*)workspace;
-    float* rec = (float*)(ws + L.rec_off);
-    float4* box = (float4*)(ws + L.box_off);
-    uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
-    int* ccount = (int*)(ws + L.ccount_off);
-    void* clist = ws + L.clist_off;
-    cudaError_t e0 = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
-    if (e0 != cudaSuccess) return (int)e0;
+    if ((rc = ensure_smem_attrs())) return rc;
+    RasterCall c = raster_call(p, workspace, stream_, false);
+    c.K.vec_store = (c.K.aa && (c.S % 8) == 0 && ((uintptr_t)aggrs_info & 15) == 0) ? 1 : 0;
     if (visible_faces) {
-        e0 = cudaMemsetAsync(visible_faces, 0, (size_t)B * F, stream);
-        if (e0 != cudaSuccess) return (int)e0;
+        cudaError_t e = cudaMemsetAsync(visible_faces, 0, (size_t)c.B * c.F, c.stream);
+        if (e != cudaSuccess) return (int)e;
     }
-    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr));
-    const int ncb = (K.S + CB - 1) / CB;
-    rc = launch_bin_coarse(box, ubox, clist, ccount, B, F, K.S, L, stream);
-    if (rc) return rc;
-    const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
-    const PairBuf none{nullptr, nullptr, nullptr, nullptr, nullptr, 0u};
-    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-#define UMR_VIS(IDX)                                                                                                          \
-    if (visible_faces && !aggrs_info)   /* only the visible-face bytes: face-parallel z-buffer per 64x64 bin */              \
-        k_visible_faces<IDX><<<dim3(ncb, ncb, B), CTA, 0, stream>>>(rec, (const IDX*)clist, ccount, visible_faces, K);       \
-    else                                                                                                                      \
-        k_raster_fwd3<2, 3, IDX><<<grid, CTA, 0, stream>>>(rec, box, (const IDX*)clist, ccount, /*textures*/ nullptr,        \
-                                                           /*images*/ nullptr, /*colors_hi*/ nullptr, aggrs_info,             \
-                                                           /*p2f*/ nullptr, ubox, K, p->eps, 0.f, 0.f, 0.f, none, ncb, 0.f,   \
-                                                           visible_faces);
-    if (F > NARROW_MAX_FACES) { UMR_VIS(uint32_t) } else { UMR_VIS(uint16_t) }
-#undef UMR_VIS
-    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
-    count_launch(3);
+    if ((rc = prep(c, face_vertices, nullptr)) || (rc = bin_coarse(c))) return rc;
+    record(p->ev_kernel_start, c.stream);
+    with_index(c.wide, [&](auto idx) {
+        using IDX = decltype(idx);
+        if (visible_faces && !aggrs_info)  // only the visible-face bytes: face-parallel z-buffer per 64x64 bin
+            launch(k_visible_faces<IDX>, dim3(c.ncb, c.ncb, c.B), CTA, 0, c.stream, c.rec, (const IDX*)c.clist, c.ccount,
+                   visible_faces, c.K);
+        else
+            launch(k_raster_fwd3<2, 3, IDX>, c.grid16, CTA, 0, c.stream, c.rec, c.box, (const IDX*)c.clist, c.ccount,
+                   /*textures*/ nullptr, /*images*/ nullptr, /*colors_hi*/ nullptr, aggrs_info, /*p2f*/ nullptr, c.ubox, c.K,
+                   p->eps, 0.f, 0.f, 0.f, c.pb, c.ncb, 0.f, visible_faces);
+    });
+    record(p->ev_kernel_stop, c.stream);
     return (int)cudaGetLastError();
 }
 
@@ -1589,121 +1591,47 @@ static bool split_refused(const UmrRasterParams* p, const float* grad_faces, con
     return !grad_faces || !grad_textures || is_generic(p) || p->color_channels == 4;
 }
 
-// split: umr_raster_backward_split (the caller has checked split_refused)
+// split: umr_raster_backward_split
 static int raster_backward(const float* face_vertices, const float* textures, const float* soft_colors, const float* aggrs_info,
                            const float* grad_images, float* grad_faces, float* grad_textures, const UmrRasterParams* p,
                            void* workspace, void* stream_, bool split) {
+    int rc = check_params<float>(p);
+    if (rc) return rc;
+    if (split && split_refused(p, grad_faces, grad_textures)) return UMR_ERR_BAD_ARG;
     if (!face_vertices || !textures || !soft_colors || !aggrs_info || !grad_images || !workspace) return UMR_ERR_BAD_ARG;
     if (!grad_faces && !grad_textures) return UMR_ERR_BAD_ARG;  // nothing to compute
-    if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
-    const bool nc4 = p->color_channels == 4;
-    if (nc4 && grad_textures) return UMR_ERR_UNSUPPORTED;  // part maps are constants (loss_utils.py:367-381)
-    cudaStream_t stream = (cudaStream_t)stream_;
-    int rc = ensure_smem_attrs();
-    if (rc) return rc;
-    const int B = p->batch_size, F = p->num_faces;
-    const Consts<float> K = make_consts(p);
-    const WorkspaceLayout L = ws_layout(B, F, K.S);
-    char* ws = (char*)workspace;
-    float* rec = (float*)(ws + L.rec_off);
-    float4* box = (float4*)(ws + L.box_off);
-    uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
-    const size_t n = (size_t)B * F;
-    const bool wide = F > NARROW_MAX_FACES;
-    const float r = sqrtf(K.thr);
-    // the workspace is scratch (another render may have used it since forward): rebuild the records
-    cudaError_t e = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
-    if (e != cudaSuccess) return (int)e;
-    const bool gen = is_generic(p);
-    const PairBuf pb = gen ? PairBuf{nullptr, nullptr, nullptr, nullptr, nullptr, 0u} : make_pairbuf(p, K.S);
+    if (misaligned(workspace, 256)) return UMR_ERR_BAD_ARG;
+    if (p->color_channels == 4 && grad_textures) return UMR_ERR_UNSUPPORTED;  // part maps are constants (loss_utils.py:367-381)
+    if (!grad_faces && is_generic(p)) return UMR_ERR_UNSUPPORTED;  // texture-only backward: streaming / pair kernels only
+    if ((rc = ensure_smem_attrs())) return rc;
+    const RasterCall c = raster_call(p, workspace, stream_, !is_generic(p));
     // The streamed backward re-derives its z-gradient factors from the records whenever it forms the colour terms of the
     // vertex gradients; a texture-only or split backward with a pair buffer needs them only for the recompute fallback, so
     // k_prep returns at once there when no tile is unsaved.
-    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, r,
-                                                         (pb.cap > 0 && (!grad_faces || split)) ? pb.ctrl + 1 : nullptr);
-    count_launch();
-    if (grad_faces) {
-        e = cudaMemsetAsync(grad_faces, 0, n * 9 * sizeof(float), stream);
-        if (e != cudaSuccess) return (int)e;
-    } else if (gen) {
-        return UMR_ERR_UNSUPPORTED;  // texture-only backward: streaming / pair kernels only
-    }
-    if (grad_textures) {
-        e = cudaMemsetAsync(grad_textures, 0, (n / (p->shared_textures > 1 ? p->shared_textures : 1)) * p->texture_size * 3 * sizeof(float), stream);
-        if (e != cudaSuccess) return (int)e;
-    }
-    const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
-    const size_t smem = raster_dyn_smem(F);
-    const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
-#define UMR_LAUNCH_BWD(RGBM, TG, SP)                                                                          \
-    do {                                                                                                      \
-        if (gen)                                                                                              \
-            k_raster_bwd<RGBM, TG><<<grid, CTA, smem, stream>>>(rec, box, textures, soft_colors, aggrs_info,    \
-                                                                grad_images, grad_faces, grad_textures, ubox, K); \
-        else {                                                                                                \
-            if (pb.cap > 0) {                                                                                 \
-                count_launch();                                                                               \
-                if (forward_impl(p->tile_mode) == 4 && wide)                                                  \
-                    launch_bwd2<RGBM, TG, 32, uint32_t, SP>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
-                                                            grad_images, grad_faces, grad_textures, K, pb);   \
-                else if (forward_impl(p->tile_mode) == 4)                                                     \
-                    launch_bwd2<RGBM, TG, 32, uint16_t, SP>(grid32, stream, tex_pre, rec, textures, soft_colors, aggrs_info, \
-                                                            grad_images, grad_faces, grad_textures, K, pb);   \
-                else if (wide)                                                                                \
-                    launch_bwd2<RGBM, TG, 16, uint32_t, SP>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, \
-                                                            aggrs_info, grad_images, grad_faces, grad_textures, K, pb); \
-                else                                                                                          \
-                    launch_bwd2<RGBM, TG, 16, uint16_t, SP>(grid_pairs, stream, tex_pre, rec, textures, soft_colors, \
-                                                            aggrs_info, grad_images, grad_faces, grad_textures, K, pb); \
-            }                                                                                                 \
-            if (pb.cap > 0)                                                                                   \
-                k_raster_bwd_pairs_list<RGBM, TG, 3, SP><<<list_grid, CTA, smem, stream>>>(                   \
-                    rec, box, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, ubox, K, \
-                    pb.ctrl + 1, pb.ulist, (int)grid_pairs.x, (int)grid_pairs.y);                             \
-            else                                                                                              \
-                k_raster_bwd_pairs<RGBM, TG, 3, SP><<<grid_pairs, CTA, smem, stream>>>(rec, box, textures, soft_colors, \
-                                                              aggrs_info, grad_images, grad_faces, grad_textures, ubox, K); \
-        }                                                                                                     \
-    } while (0)
-    const dim3 grid_pairs((K.S + PT - 1) / PT, (K.S + PT - 1) / PT, B);
-    const dim3 grid32((K.S + T4 - 1) / T4, (K.S + T4 - 1) / T4, B);
+    if ((rc = prep(c, face_vertices, (c.pb.cap > 0 && (!grad_faces || split)) ? c.pb.ctrl + 1 : nullptr)) ||
+        (rc = zero_grads(c, grad_faces, grad_textures)))
+        return rc;
+    unsigned lg = 0;
+    if ((rc = list_grid(c, &lg))) return rc;
     // texel-gradient pre-reduction inside the warp (k_raster_bwd2<..., PRE>): pays when many pixels of an 8x4 block land
     // on one texel, i.e. when a face covers many more raster pixels than it has texels.
-    const bool tex_pre = (double)K.S * K.S >= (grad_faces ? TEXGRAD_PRE_RATIO_FULL : TEXGRAD_PRE_RATIO_TEXONLY) *
-                                                  (double)F * p->texture_size;
-    const size_t ntiles = (size_t)grid_pairs.x * grid_pairs.y * B;
-    int sms = 0;
-    rc = sm_count(&sms);
-    if (rc) return rc;
-    const size_t list_max = (size_t)3 * sms;  // 3 resident CTAs per SM walk the unsaved-tile list
-    const unsigned list_grid = (unsigned)(ntiles < list_max ? ntiles : list_max);
-    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-    count_launch();
-    if (nc4) {  // 16x16 tiles, softmax, no texture gradient (check_params / above)
-        if (pb.cap > 0) {
-            count_launch();
-            if (wide)
-                k_raster_bwd2<1, false, 16, 4, true, false, uint32_t><<<grid_pairs, BWD2_THREADS, 0, stream>>>(
-                    rec, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, K, pb);
-            else
-                k_raster_bwd2<1, false, 16, 4><<<grid_pairs, BWD2_THREADS, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images, grad_faces,
-                                                                                grad_textures, K, pb);
-            k_raster_bwd_pairs_list<1, false, 4><<<list_grid, CTA, smem, stream>>>(rec, box, textures, soft_colors, aggrs_info, grad_images,
-                                                                                   grad_faces, grad_textures, ubox, K, pb.ctrl + 1,
-                                                                                   pb.ulist, (int)grid_pairs.x, (int)grid_pairs.y);
-        } else {
-            k_raster_bwd_pairs<1, false, 4><<<grid_pairs, CTA, smem, stream>>>(rec, box, textures, soft_colors, aggrs_info, grad_images,
-                                                                               grad_faces, grad_textures, ubox, K);
-        }
-    } else if (softmax) {
-        if (split) UMR_LAUNCH_BWD(1, true, true);
-        else if (grad_textures) UMR_LAUNCH_BWD(1, true, false);
-        else UMR_LAUNCH_BWD(1, false, false);
-    } else {  // hard colours: the vertex gradients have no colour terms, so the split backward is the full one
-        if (grad_textures) UMR_LAUNCH_BWD(0, true, false); else UMR_LAUNCH_BWD(0, false, false);
-    }
-#undef UMR_LAUNCH_BWD
-    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+    const bool pre = (double)c.S * c.S >= (grad_faces ? TEXGRAD_PRE_RATIO_FULL : TEXGRAD_PRE_RATIO_TEXONLY) *
+                                              (double)c.F * p->texture_size;
+    const BwdArgs a{textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures};
+    record(p->ev_kernel_start, c.stream);
+    if (c.gen)
+        launch(c.softmax ? (grad_textures ? k_raster_bwd<1, true> : k_raster_bwd<1, false>)
+                         : (grad_textures ? k_raster_bwd<0, true> : k_raster_bwd<0, false>),
+               c.grid16, CTA, raster_dyn_smem(c.F), c.stream, c.rec, c.box, textures, soft_colors, aggrs_info, grad_images,
+               grad_faces, grad_textures, c.ubox, c.K);
+    else if (c.nc4) launch_pairs_backward<1, false, 4, false>(c, lg, pre, a);  // softmax, no texture gradient (above)
+    else if (c.softmax && split) launch_pairs_backward<1, true, 3, true>(c, lg, pre, a);
+    else if (c.softmax && grad_textures) launch_pairs_backward<1, true, 3, false>(c, lg, pre, a);
+    else if (c.softmax) launch_pairs_backward<1, false, 3, false>(c, lg, pre, a);
+    // hard colours: the vertex gradients have no colour terms, so the split backward is the full one
+    else if (grad_textures) launch_pairs_backward<0, true, 3, false>(c, lg, pre, a);
+    else launch_pairs_backward<0, false, 3, false>(c, lg, pre, a);
+    record(p->ev_kernel_stop, c.stream);
     return (int)cudaGetLastError();
 }
 
@@ -1711,8 +1639,6 @@ extern "C" int umr_raster_backward(const float* face_vertices, const float* text
                                    const float* soft_colors, const float* aggrs_info,
                                    const float* grad_images, float* grad_faces, float* grad_textures,
                                    const UmrRasterParams* p, void* workspace, void* stream_) {
-    int rc = check_params(p);
-    if (rc) return rc;
     return raster_backward(face_vertices, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, p, workspace,
                            stream_, false);
 }
@@ -1721,9 +1647,6 @@ extern "C" int umr_raster_backward_split(const float* face_vertices, const float
                                          const float* soft_colors, const float* aggrs_info,
                                          const float* grad_images, float* grad_faces, float* grad_textures,
                                          const UmrRasterParams* p, void* workspace, void* stream_) {
-    int rc = check_params(p);
-    if (rc) return rc;
-    if (split_refused(p, grad_faces, grad_textures)) return UMR_ERR_BAD_ARG;
     return raster_backward(face_vertices, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, p, workspace,
                            stream_, true);
 }
@@ -1733,50 +1656,27 @@ extern "C" int umr_raster_backward_split(const float* face_vertices, const float
 static int raster_backward_det(const float* face_vertices, const float* textures, const float* soft_colors,
                                const float* aggrs_info, const float* grad_images, float* grad_faces, float* grad_textures,
                                const UmrRasterParams* p, void* workspace, void* stream_, bool split) {
-    if ((int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;  // as the forward
+    int rc = check_params<float>(p);
+    if (rc) return rc;
+    if (split && split_refused(p, grad_faces, grad_textures)) return UMR_ERR_BAD_ARG;
+    if (raster_side(p) > GATHER_MAX_RASTER) return UMR_ERR_TOO_LARGE;  // as the forward
     if (!face_vertices || !textures || !soft_colors || !aggrs_info || !grad_images || !workspace) return UMR_ERR_BAD_ARG;
     if (!grad_faces && !grad_textures) return UMR_ERR_BAD_ARG;
-    if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
-    const bool gen = is_generic(p);
-    const bool nc4 = p->color_channels == 4;
-    if (nc4 && grad_textures) return UMR_ERR_UNSUPPORTED;  // part maps are constants (loss_utils.py:367-381)
-    cudaStream_t stream = (cudaStream_t)stream_;
-    const int B = p->batch_size, F = p->num_faces;
-    const Consts<float> K = make_consts(p);
-    const WorkspaceLayout L = ws_layout(B, F, K.S);
-    char* ws = (char*)workspace;
-    float* rec = (float*)(ws + L.rec_off);
-    float4* box = (float4*)(ws + L.box_off);
-    uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
-    const size_t n = (size_t)B * F;
-    cudaError_t e = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
-    if (e != cudaSuccess) return (int)e;
-    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr));
-    if (grad_textures) {
-        e = cudaMemsetAsync(grad_textures, 0, (n / K.tex_div) * p->texture_size * 3 * sizeof(float), stream);
-        if (e != cudaSuccess) return (int)e;
-    }
-    const dim3 grid((unsigned)((F + NWARP - 1) / NWARP), (unsigned)(B / K.tex_div));
-    const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
-    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-#define UMR_BWD_DET(RGBM, TG, NCH)                                                                                        \
-    do {                                                                                                                    \
-        if (gen) k_raster_bwd_det<float, RGBM, TG, NCH, true><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors,        \
-                                                                                      aggrs_info, grad_images, grad_faces, \
-                                                                                      grad_textures, K);                   \
-        else k_raster_bwd_det<float, RGBM, TG, NCH><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info,         \
-                                                                               grad_images, grad_faces, grad_textures, K); \
-    } while (0)
-    if (nc4) k_raster_bwd_det<float, 1, false, 4><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images,
-                                                                             grad_faces, grad_textures, K);
-    else if (split && softmax) k_raster_bwd_det<float, 1, true, 3, false, true><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors,
-                                                                                                          aggrs_info, grad_images,
-                                                                                                          grad_faces, grad_textures, K);
-    else if (softmax) { if (grad_textures) UMR_BWD_DET(1, true, 3); else UMR_BWD_DET(1, false, 3); }
-    else { if (grad_textures) UMR_BWD_DET(0, true, 3); else UMR_BWD_DET(0, false, 3); }  // hard: split == full
-#undef UMR_BWD_DET
-    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
-    count_launch(2);
+    if (misaligned(workspace, 256)) return UMR_ERR_BAD_ARG;
+    if (p->color_channels == 4 && grad_textures) return UMR_ERR_UNSUPPORTED;  // part maps are constants (loss_utils.py:367-381)
+    const RasterCall c = raster_call(p, workspace, stream_, false);
+    if ((rc = prep(c, face_vertices, nullptr)) || (rc = zero_grads(c, nullptr, grad_textures))) return rc;
+    // RGB x TEXGRAD x GEN with 3 channels; hard colours: the split backward is the full one
+    auto k = c.softmax ? (grad_textures ? (c.gen ? k_raster_bwd_det<float, 1, true, 3, true> : k_raster_bwd_det<float, 1, true, 3>)
+                                        : (c.gen ? k_raster_bwd_det<float, 1, false, 3, true> : k_raster_bwd_det<float, 1, false, 3>))
+                       : (grad_textures ? (c.gen ? k_raster_bwd_det<float, 0, true, 3, true> : k_raster_bwd_det<float, 0, true, 3>)
+                                        : (c.gen ? k_raster_bwd_det<float, 0, false, 3, true> : k_raster_bwd_det<float, 0, false, 3>));
+    if (c.nc4) k = k_raster_bwd_det<float, 1, false, 4>;
+    else if (split && c.softmax) k = k_raster_bwd_det<float, 1, true, 3, false, true>;
+    record(p->ev_kernel_start, c.stream);
+    launch(k, gather_grid(c.K, c.B), CTA, 0, c.stream, c.rec, textures, soft_colors, aggrs_info, grad_images, grad_faces,
+           grad_textures, c.K);
+    record(p->ev_kernel_stop, c.stream);
     return (int)cudaGetLastError();
 }
 
@@ -1784,8 +1684,6 @@ extern "C" int umr_raster_backward_deterministic(const float* face_vertices, con
                                                  const float* soft_colors, const float* aggrs_info,
                                                  const float* grad_images, float* grad_faces, float* grad_textures,
                                                  const UmrRasterParams* p, void* workspace, void* stream_) {
-    int rc = check_params(p);
-    if (rc) return rc;
     return raster_backward_det(face_vertices, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, p,
                                workspace, stream_, false);
 }
@@ -1794,9 +1692,6 @@ extern "C" int umr_raster_backward_split_deterministic(const float* face_vertice
                                                        const float* soft_colors, const float* aggrs_info,
                                                        const float* grad_images, float* grad_faces, float* grad_textures,
                                                        const UmrRasterParams* p, void* workspace, void* stream_) {
-    int rc = check_params(p);
-    if (rc) return rc;
-    if (split_refused(p, grad_faces, grad_textures)) return UMR_ERR_BAD_ARG;
     return raster_backward_det(face_vertices, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, p,
                                workspace, stream_, true);
 }
@@ -1804,65 +1699,42 @@ extern "C" int umr_raster_backward_split_deterministic(const float* face_vertice
 // =============================================================================================
 // Silhouette render (DESIGN.md §12): the alpha plane and its vertex gradient, UMR's configuration only
 // =============================================================================================
-// Refused before any device work: what check_params refuses, the generic modes and the 4-channel render (UMR_ERR_BAD_ARG).
-static int check_silhouette_params(const UmrRasterParams* p) {
-    int rc = check_params(p);
+// Refused before any device work: what check_params refuses, the generic modes and the 4-channel render (UMR_ERR_BAD_ARG),
+// and (det) a raster side past the deterministic limit.
+static int check_silhouette_params(const UmrRasterParams* p, bool det) {
+    int rc = check_params<float>(p);
     if (rc) return rc;
     if (is_generic(p) || p->color_channels == 4) return UMR_ERR_BAD_ARG;
+    if (det && raster_side(p) > GATHER_MAX_RASTER) return UMR_ERR_TOO_LARGE;
     return UMR_OK;
 }
-static bool misaligned_f32(const void* ptr) { return ((uintptr_t)ptr & (sizeof(float) - 1)) != 0; }
 
 // det: the deterministic twin -- the 16x16-tile forward whatever tile_mode says and no pair buffer (the silhouette forward
 // has no float atomics either way, so its planes are those of the default call)
 static int raster_forward_silhouette(const float* face_vertices, float* alpha, float* alpha_hi, const UmrRasterParams* p,
                                      void* workspace, void* stream_, bool det) {
-    int rc = check_silhouette_params(p);
+    int rc = check_silhouette_params(p, det);
     if (rc) return rc;
-    if (det && (int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;
     if (!face_vertices || !alpha || !workspace) return UMR_ERR_BAD_ARG;
-    if (misaligned_f32(face_vertices) || misaligned_f32(alpha) || misaligned_f32(alpha_hi) || ((uintptr_t)workspace & 255) != 0)
+    if (misaligned(face_vertices, 4) || misaligned(alpha, 4) || misaligned(alpha_hi, 4) || misaligned(workspace, 256))
         return UMR_ERR_BAD_ARG;
-    cudaStream_t stream = (cudaStream_t)stream_;
-    rc = ensure_smem_attrs();
-    if (rc) return rc;
-    const int B = p->batch_size, F = p->num_faces;
-    const Consts<float> K = make_consts(p);
-    if (!K.aa && alpha_hi == nullptr) alpha_hi = alpha;  // the raster is the image
-    const WorkspaceLayout L = ws_layout(B, F, K.S);
-    char* ws = (char*)workspace;
-    float* rec = (float*)(ws + L.rec_off);
-    float4* box = (float4*)(ws + L.box_off);
-    uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
-    int* ccount = (int*)(ws + L.ccount_off);
-    void* clist = ws + L.clist_off;
-    cudaError_t e = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
-    if (e != cudaSuccess) return (int)e;
-    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr));
-    count_launch();
-    const PairBuf pb = det ? PairBuf{nullptr, nullptr, nullptr, nullptr, nullptr, 0u} : make_pairbuf(p, K.S);
-    if (pb.cap > 0) {
-        e = cudaMemsetAsync(pb.ctrl, 0, 16, stream);
-        if (e != cudaSuccess) return (int)e;
-    }
-    count_launch(2);
-    rc = launch_bin_coarse(box, ubox, clist, ccount, B, F, K.S, L, stream);
-    if (rc) return rc;
-    const int ncb = (K.S + CB - 1) / CB;
-    const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
-    const dim3 grid32((K.S + T4 - 1) / T4, (K.S + T4 - 1) / T4, B);
-    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-#define UMR_SIL_ARGS(IDX) rec, box, (const IDX*)clist, ccount, /*textures*/ nullptr, alpha, alpha_hi, /*aggrs*/ nullptr, \
-                          /*p2f*/ nullptr, ubox, K, p->eps, 0.f, 0.f, 0.f, pb, ncb
-#define UMR_SIL_FWD(IDX)                                                                                                  \
-    if (det || forward_impl(p->tile_mode) == 3)                                                                           \
-        k_raster_fwd3<RGB_SIL, 3, IDX><<<grid, CTA, 0, stream>>>(UMR_SIL_ARGS(IDX));                                      \
-    else                                                                                                                  \
-        k_raster_fwd4<RGB_SIL, IDX><<<grid32, CTA, fwd4_dyn_smem(F, sizeof(IDX)), stream>>>(UMR_SIL_ARGS(IDX));
-    if (F > NARROW_MAX_FACES) { UMR_SIL_FWD(uint32_t) } else { UMR_SIL_FWD(uint16_t) }
-#undef UMR_SIL_FWD
-#undef UMR_SIL_ARGS
-    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+    if ((rc = ensure_smem_attrs())) return rc;
+    const RasterCall c = raster_call(p, workspace, stream_, !det);
+    if (!c.K.aa && alpha_hi == nullptr) alpha_hi = alpha;  // the raster is the image
+    if ((rc = prep(c, face_vertices, nullptr)) || (rc = bin_coarse(c))) return rc;
+    record(p->ev_kernel_start, c.stream);
+    with_index(c.wide, [&](auto idx) {
+        using IDX = decltype(idx);
+        if (det || forward_impl(p->tile_mode) == 3)
+            launch(k_raster_fwd3<RGB_SIL, 3, IDX>, c.grid16, CTA, 0, c.stream, c.rec, c.box, (const IDX*)c.clist, c.ccount,
+                   /*textures*/ nullptr, alpha, alpha_hi, /*aggrs*/ nullptr, /*p2f*/ nullptr, c.ubox, c.K, p->eps, 0.f, 0.f, 0.f,
+                   c.pb, c.ncb, 0.f, nullptr);
+        else
+            launch(k_raster_fwd4<RGB_SIL, IDX>, c.grid32, CTA, fwd4_dyn_smem(c.F, sizeof(IDX)), c.stream, c.rec, c.box,
+                   (const IDX*)c.clist, c.ccount, nullptr, alpha, alpha_hi, nullptr, nullptr, c.ubox, c.K, p->eps, 0.f, 0.f,
+                   0.f, c.pb, c.ncb);
+    });
+    record(p->ev_kernel_stop, c.stream);
     return (int)cudaGetLastError();
 }
 
@@ -1870,72 +1742,26 @@ static int raster_forward_silhouette(const float* face_vertices, float* alpha, f
 // forward saved and the recompute backward for the tiles it could not save (or for every tile without a pair buffer)
 static int raster_backward_silhouette(const float* face_vertices, const float* alpha_hi, const float* grad_alpha,
                                       float* grad_faces, const UmrRasterParams* p, void* workspace, void* stream_, bool det) {
-    int rc = check_silhouette_params(p);
+    int rc = check_silhouette_params(p, det);
     if (rc) return rc;
-    if (det && (int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > DET_MAX_RASTER) return UMR_ERR_TOO_LARGE;
     if (!face_vertices || !alpha_hi || !grad_alpha || !grad_faces || !workspace) return UMR_ERR_BAD_ARG;
-    if (misaligned_f32(face_vertices) || misaligned_f32(alpha_hi) || misaligned_f32(grad_alpha) || misaligned_f32(grad_faces) ||
-        ((uintptr_t)workspace & 255) != 0)
+    if (misaligned(face_vertices, 4) || misaligned(alpha_hi, 4) || misaligned(grad_alpha, 4) || misaligned(grad_faces, 4) ||
+        misaligned(workspace, 256))
         return UMR_ERR_BAD_ARG;
-    cudaStream_t stream = (cudaStream_t)stream_;
-    rc = ensure_smem_attrs();
-    if (rc) return rc;
-    const int B = p->batch_size, F = p->num_faces;
-    const Consts<float> K = make_consts(p);
-    const WorkspaceLayout L = ws_layout(B, F, K.S);
-    char* ws = (char*)workspace;
-    float* rec = (float*)(ws + L.rec_off);
-    float4* box = (float4*)(ws + L.box_off);
-    uint32_t* ubox = (uint32_t*)(ws + L.ubox_off);
-    // the workspace is scratch (another render may have used it since forward): rebuild the records
-    cudaError_t e = cudaMemsetAsync(ubox, 0, (size_t)B * 4 * sizeof(uint32_t), stream);
-    if (e != cudaSuccess) return (int)e;
-    if (det) {
-        k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr));
-        const dim3 grid((unsigned)((F + NWARP - 1) / NWARP), (unsigned)(B / K.tex_div));
-        if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-        k_raster_bwd_det<float, RGB_SIL, false><<<grid, CTA, 0, stream>>>(rec, nullptr, alpha_hi, nullptr, grad_alpha, grad_faces,
-                                                                         nullptr, K);
-        if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
-        count_launch(2);
-        return (int)cudaGetLastError();
-    }
-    const PairBuf pb = make_pairbuf(p, K.S);
+    if ((rc = ensure_smem_attrs())) return rc;
+    const RasterCall c = raster_call(p, workspace, stream_, !det);
     // the streamed silhouette backward reads no face record: with a pair buffer only the recompute fallback needs them, so
     // k_prep returns at once when no tile is unsaved
-    k_prep<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, ubox, F, sqrtf(K.thr),
-                                                         pb.cap > 0 ? pb.ctrl + 1 : nullptr);
-    count_launch();
-    e = cudaMemsetAsync(grad_faces, 0, (size_t)B * F * 9 * sizeof(float), stream);
-    if (e != cudaSuccess) return (int)e;
-    const size_t smem = raster_dyn_smem(F);
-    const dim3 grid_pairs((K.S + PT - 1) / PT, (K.S + PT - 1) / PT, B);
-    const dim3 grid32((K.S + T4 - 1) / T4, (K.S + T4 - 1) / T4, B);
-    const size_t ntiles = (size_t)grid_pairs.x * grid_pairs.y * B;
-    int sms = 0;
-    rc = sm_count(&sms);
-    if (rc) return rc;
-    const size_t list_max = (size_t)3 * sms;  // 3 resident CTAs per SM walk the unsaved-tile list
-    const unsigned list_grid = (unsigned)(ntiles < list_max ? ntiles : list_max);
-    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-    count_launch();
-    if (pb.cap > 0) {
-        count_launch();
-#define UMR_SIL_BWD2(TS, IDX, G)                                                                                          \
-        k_raster_bwd2<RGB_SIL, false, TS, 3, true, false, IDX><<<G, BWD2_THREADS, 0, stream>>>(                           \
-            nullptr, nullptr, alpha_hi, nullptr, grad_alpha, grad_faces, nullptr, K, pb)
-        const bool wide = F > NARROW_MAX_FACES;
-        if (forward_impl(p->tile_mode) == 4) { if (wide) UMR_SIL_BWD2(32, uint32_t, grid32); else UMR_SIL_BWD2(32, uint16_t, grid32); }
-        else { if (wide) UMR_SIL_BWD2(16, uint32_t, grid_pairs); else UMR_SIL_BWD2(16, uint16_t, grid_pairs); }
-#undef UMR_SIL_BWD2
-        k_raster_bwd_pairs_list<RGB_SIL, false><<<list_grid, CTA, smem, stream>>>(
-            rec, box, nullptr, alpha_hi, nullptr, grad_alpha, grad_faces, nullptr, ubox, K, pb.ctrl + 1, pb.ulist,
-            (int)grid_pairs.x, (int)grid_pairs.y);
-    } else {
-        k_raster_bwd_pairs<RGB_SIL, false><<<grid_pairs, CTA, smem, stream>>>(rec, box, nullptr, alpha_hi, nullptr, grad_alpha,
-                                                                              grad_faces, nullptr, ubox, K);
-    }
-    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
+    if ((rc = prep(c, face_vertices, c.pb.cap > 0 ? c.pb.ctrl + 1 : nullptr))) return rc;
+    unsigned lg = 0;
+    if (!det && ((rc = zero_grads(c, grad_faces, nullptr)) || (rc = list_grid(c, &lg)))) return rc;
+    record(p->ev_kernel_start, c.stream);
+    if (det)
+        launch(k_raster_bwd_det<float, RGB_SIL, false>, gather_grid(c.K, c.B), CTA, 0, c.stream, c.rec, nullptr, alpha_hi,
+               nullptr, grad_alpha, grad_faces, nullptr, c.K);
+    else
+        launch_pairs_backward<RGB_SIL, false, 3, false>(c, lg, false, BwdArgs{nullptr, alpha_hi, nullptr, grad_alpha, grad_faces, nullptr});
+    record(p->ev_kernel_stop, c.stream);
     return (int)cudaGetLastError();
 }
 

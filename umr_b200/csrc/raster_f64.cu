@@ -47,8 +47,6 @@ constexpr int P2F_LIMBS = 6;
 constexpr int P2F_LIMB_BITS = 26;
 constexpr int P2F_FRAC_BITS = 128;
 constexpr int P2F_WORDS = 3 * P2F_LIMBS + 1;  // x, y, w limbs, then a word set when a partial was not finite
-// the 16x16-tile grid (gridDim.y <= 65535) bounds the raster side, and with it the partials per face (see the header)
-constexpr int MAX_RASTER = 65535 * TILE;
 
 __host__ __device__ inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 struct Layout { size_t rec_off, box_off, acc_off, total; };
@@ -411,49 +409,13 @@ __global__ void __launch_bounds__(CTA, 2) k_raster_fwd_f64(const double* __restr
 }  // namespace f64
 }  // namespace umr
 
+#include "raster_host.cuh"
+
 // =============================================================================================
 // C ABI
 // =============================================================================================
 using namespace umr;
 using namespace umr::f64;
-
-// the checks of umr_raster_forward / umr_raster_backward, with 3 colour channels only
-static int check_params_f64(const UmrRasterParams* p) {
-    if (!p) return UMR_ERR_BAD_ARG;
-    if (p->batch_size <= 0 || p->num_faces <= 0 || p->texture_size <= 0 || p->image_size <= 0) return UMR_ERR_BAD_ARG;
-    if (p->num_faces > UMR_RASTER_MAX_FACES || p->batch_size > 65535) return UMR_ERR_TOO_LARGE;
-    if ((int64_t)p->image_size * (p->anti_aliasing ? 2 : 1) > MAX_RASTER) return UMR_ERR_TOO_LARGE;
-    if (p->func_id_dist < 0 || p->func_id_dist > 2 || p->func_id_alpha < 0 || p->func_id_alpha > 2 ||
-        p->texture_sample_type < 0 || p->texture_sample_type > 1)
-        return UMR_ERR_UNSUPPORTED;
-    if (p->texture_sample_type == UMR_TEX_VERTEX && p->texture_size != 3) return UMR_ERR_BAD_ARG;  // [B,F,3,3]
-    if (p->shared_textures > 1 && p->batch_size % p->shared_textures != 0) return UMR_ERR_BAD_ARG;
-    if (p->func_id_rgb != UMR_RGB_HARD && p->func_id_rgb != UMR_RGB_SOFTMAX) return UMR_ERR_UNSUPPORTED;
-    if (p->color_channels != 0 && p->color_channels != 3) return UMR_ERR_BAD_ARG;
-    return UMR_OK;
-}
-
-static Consts<double> make_consts_f64(const UmrRasterParams* p) {
-    Consts<double> K = {};
-    K.thr = (double)(p->dist_eps * p->sigma_val);  // kernel.cu:333: float * float, then scalar_t
-    K.sigma = p->sigma_val;
-    K.gamma = p->gamma_val;
-    K.near_ = p->near_plane;
-    K.far_ = p->far_plane;
-    K.F = p->num_faces;
-    K.T2 = p->texture_size;
-    K.R = (int)sqrt((double)p->texture_size);  // :685
-    K.IS = p->image_size;
-    K.aa = p->anti_aliasing ? 1 : 0;
-    K.S = p->image_size * (K.aa ? 2 : 1);
-    K.double_side = p->double_side ? 1 : 0;
-    K.dist = p->func_id_dist;
-    K.alpha = p->func_id_alpha;
-    K.tex = p->texture_sample_type;
-    K.tex_bs = (size_t)p->num_faces * p->texture_size * 3;
-    K.tex_div = p->shared_textures > 1 ? p->shared_textures : 1;
-    return K;
-}
 
 extern "C" size_t umr_raster_workspace_bytes_f64(int32_t B, int32_t F, int32_t image_size, int32_t anti_aliasing) {
     (void)anti_aliasing;
@@ -464,13 +426,13 @@ extern "C" size_t umr_raster_workspace_bytes_f64(int32_t B, int32_t F, int32_t i
 extern "C" int umr_raster_forward_f64(const double* face_vertices, const double* textures, double* images,
                                       double* soft_colors, double* aggrs_info, double* p2f_info,
                                       const UmrRasterParams* p, void* workspace, void* stream_) {
-    int rc = check_params_f64(p);
+    int rc = check_params<double>(p);
     if (rc) return rc;
     if (!face_vertices || !textures || !images || !aggrs_info || !workspace) return UMR_ERR_BAD_ARG;
-    if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
+    if (misaligned(workspace, 256)) return UMR_ERR_BAD_ARG;
     cudaStream_t stream = (cudaStream_t)stream_;
     const int B = p->batch_size, F = p->num_faces;
-    const Consts<double> K = make_consts_f64(p);
+    const Consts<double> K = make_consts<double>(p);
     if (!K.aa && soft_colors == nullptr) soft_colors = images;
     const f64::Layout L = f64::ws_layout(B, F);
     char* ws = (char*)workspace;
@@ -478,63 +440,49 @@ extern "C" int umr_raster_forward_f64(const double* face_vertices, const double*
     double* box = (double*)(ws + L.box_off);
     unsigned long long* acc = (unsigned long long*)(ws + L.acc_off);
     const size_t n = (size_t)B * F;
-    const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
-    const bool want_p2f = p2f_info != nullptr;
-    k_prep_f64<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, F, sqrt(K.thr));  // r: kernel.cu:355
-    if (want_p2f) {
+    const bool sums = p->func_id_rgb == UMR_RGB_SOFTMAX && p2f_info;  // p2f accumulated and finalized
+    launch(k_prep_f64, dim3((F + 255) / 256, B), 256, 0, stream, face_vertices, rec, box, F, sqrt(K.thr));  // r: kernel.cu:355
+    if (p2f_info) {
         // hard mode never accumulates p2f (kernel.cu:417-431 is softmax-only) -> zeros
-        cudaError_t e = softmax ? cudaMemsetAsync(acc, 0, n * P2F_WORDS * sizeof(unsigned long long), stream)
-                                : cudaMemsetAsync(p2f_info, 0, n * 2 * sizeof(double), stream);
+        cudaError_t e = sums ? cudaMemsetAsync(acc, 0, n * P2F_WORDS * sizeof(unsigned long long), stream)
+                             : cudaMemsetAsync(p2f_info, 0, n * 2 * sizeof(double), stream);
         if (e != cudaSuccess) return (int)e;
     }
-    const dim3 grid((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B);
-    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-    if (softmax)
-        k_raster_fwd_f64<1><<<grid, CTA, 0, stream>>>(rec, box, textures, images, soft_colors, aggrs_info,
-                                                     want_p2f ? acc : nullptr, K, p->eps, p->background_color[0],
-                                                     p->background_color[1], p->background_color[2]);
-    else
-        k_raster_fwd_f64<0><<<grid, CTA, 0, stream>>>(rec, box, textures, images, soft_colors, aggrs_info, nullptr, K, p->eps,
-                                                     p->background_color[0], p->background_color[1], p->background_color[2]);
-    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
-    count_launch(2);
-    if (want_p2f && softmax) {
-        k_p2f_finalize_f64<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(acc, p2f_info, n);
-        count_launch();
-    }
+    record(p->ev_kernel_start, stream);
+    launch(p->func_id_rgb == UMR_RGB_SOFTMAX ? k_raster_fwd_f64<1> : k_raster_fwd_f64<0>,
+           dim3((K.S + TILE - 1) / TILE, (K.S + TILE - 1) / TILE, B), CTA, 0, stream, rec, box, textures, images, soft_colors,
+           aggrs_info, sums ? acc : nullptr, K, p->eps, p->background_color[0], p->background_color[1], p->background_color[2]);
+    record(p->ev_kernel_stop, stream);
+    if (sums) launch(k_p2f_finalize_f64, (unsigned)((n + 255) / 256), 256, 0, stream, acc, p2f_info, n);
     return (int)cudaGetLastError();
 }
 
 extern "C" int umr_raster_backward_f64(const double* face_vertices, const double* textures, const double* soft_colors,
                                        const double* aggrs_info, const double* grad_images, double* grad_faces,
                                        double* grad_textures, const UmrRasterParams* p, void* workspace, void* stream_) {
-    int rc = check_params_f64(p);
+    int rc = check_params<double>(p);
     if (rc) return rc;
     if (!face_vertices || !textures || !soft_colors || !aggrs_info || !grad_images || !workspace) return UMR_ERR_BAD_ARG;
     if (!grad_faces && !grad_textures) return UMR_ERR_BAD_ARG;
-    if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
+    if (misaligned(workspace, 256)) return UMR_ERR_BAD_ARG;
     cudaStream_t stream = (cudaStream_t)stream_;
     const int B = p->batch_size, F = p->num_faces;
-    const Consts<double> K = make_consts_f64(p);
+    const Consts<double> K = make_consts<double>(p);
     const f64::Layout L = f64::ws_layout(B, F);
     char* ws = (char*)workspace;
     double* rec = (double*)(ws + L.rec_off);
     double* box = (double*)(ws + L.box_off);
     const size_t n = (size_t)B * F;
-    k_prep_f64<<<dim3((F + 255) / 256, B), 256, 0, stream>>>(face_vertices, rec, box, F, sqrt(K.thr));  // r: kernel.cu:355
+    launch(k_prep_f64, dim3((F + 255) / 256, B), 256, 0, stream, face_vertices, rec, box, F, sqrt(K.thr));  // r: kernel.cu:355
     if (grad_textures) {
         cudaError_t e = cudaMemsetAsync(grad_textures, 0, (n / K.tex_div) * p->texture_size * 3 * sizeof(double), stream);
         if (e != cudaSuccess) return (int)e;
     }
-    const dim3 grid((unsigned)((F + NWARP - 1) / NWARP), (unsigned)(B / K.tex_div));
     const bool softmax = p->func_id_rgb == UMR_RGB_SOFTMAX;
-    if (p->ev_kernel_start) cudaEventRecord((cudaEvent_t)p->ev_kernel_start, stream);
-#define UMR_BWD_F64(RGBM, TG) \
-    k_raster_bwd_det<double, RGBM, TG, 3, true><<<grid, CTA, 0, stream>>>(rec, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, K)
-    if (softmax) { if (grad_textures) UMR_BWD_F64(1, true); else UMR_BWD_F64(1, false); }
-    else { if (grad_textures) UMR_BWD_F64(0, true); else UMR_BWD_F64(0, false); }
-#undef UMR_BWD_F64
-    if (p->ev_kernel_stop) cudaEventRecord((cudaEvent_t)p->ev_kernel_stop, stream);
-    count_launch(2);
+    record(p->ev_kernel_start, stream);
+    launch(softmax ? (grad_textures ? k_raster_bwd_det<double, 1, true, 3, true> : k_raster_bwd_det<double, 1, false, 3, true>)
+                   : (grad_textures ? k_raster_bwd_det<double, 0, true, 3, true> : k_raster_bwd_det<double, 0, false, 3, true>),
+           gather_grid(K, B), CTA, 0, stream, rec, textures, soft_colors, aggrs_info, grad_images, grad_faces, grad_textures, K);
+    record(p->ev_kernel_stop, stream);
     return (int)cudaGetLastError();
 }
