@@ -1,6 +1,6 @@
-"""The harness of the rasteriser range tests (test_raster_gather_range_gpu.py, test_raster_fast_range_gpu.py): renders
-through the C entry points with every buffer between NaN guard bands, oracle B on the same inputs, and the tolerance
-gates.
+"""The harness of the rasteriser range tests (test_raster_gather_range_gpu.py, test_raster_fast_range_gpu.py,
+test_raster_part_map_range_gpu.py): renders through the C entry points with every buffer between NaN guard bands, oracle
+B on the same inputs (oracle4: the 4-channel part-map render composed from two of them), and the tolerance gates.
 
 Every input sits between guard bands and every output is prefilled with a NaN payload no kernel produces; after each
 call the bands are compared bit for bit and every output element must have been written.  Buffers start on 256-byte
@@ -290,9 +290,10 @@ def c_silhouette(path, fv, isz, aa, g_alpha, kw, blocks=0, tile=0):
     return out
 
 
-def oracle(path, fv, tex, isz, aa, g, kw, dt=None, alpha_only=False):
+def oracle(path, fv, tex, isz, aa, g, kw, dt=None, alpha_only=False, tex_abs=True):
     """oracle B in the path's precision (or dt); textures [G, ...] are expanded to the B renders and their gradient summed
-    back.  alpha_only: also the vertex gradient with the colour adjoints zeroed ("grad_faces_alpha")."""
+    back.  alpha_only: also the vertex gradient with the colour adjoints zeroed ("grad_faces_alpha"); tex_abs: the float32
+    texel gradient with absolute adjoints ("grad_tex_abs", the texel gates' floor)."""
     dt = dt or (np.float64 if path == "f64" else np.float32)
     k = dict(KW, **kw)
     k.pop("background_extra", None)
@@ -307,13 +308,39 @@ def oracle(path, fv, tex, isz, aa, g, kw, dt=None, alpha_only=False):
         ghi = softras.avg_pool2_backward(np.asarray(g, dt)) if aa else np.asarray(g, dt)
         gf, gt = softras.backward(fwd, ghi, cfg, impl="B")
         out["grad_faces"], out["grad_tex"] = gf, gt.reshape(G, B // G, *tex.shape[1:]).sum(1)
-        if dt == np.float32:
+        if dt == np.float32 and tex_abs:
             gta = softras.backward(fwd, np.abs(ghi), cfg, impl="B")[1]
             out["grad_tex_abs"] = np.abs(gta).reshape(G, B // G, *tex.shape[1:]).sum(1)
         if alpha_only:
             ga = np.zeros_like(ghi)
             ga[:, 3] = ghi[:, 3]
             out["grad_faces_alpha"] = softras.backward(fwd, ga, cfg, impl="B")[0]
+    return out
+
+
+def oracle4(fv, tex, isz, aa, g, kw):
+    """The 4-channel part-map render (float32, textures [G, F, T2, 4], images [B, 5, ...], kw's background_color (b0, b1,
+    b2) and background_extra bg3) composed from two 3-channel oracle B renders: A of channels 0-2 on (b0, b1, b2), and B of
+    channels (3, 0, 1) on (bg3, b0, b1).  Colour planes 0-2, alpha, aggrs and p2f are A's, plane 3 is B's plane 0.  Colour
+    channels do not interact in the rasteriser, so the vertex gradient is linear in the adjoint: A's for the adjoints of
+    planes 0-2 and alpha plus B's for plane 3's adjoint alone.  There is no texel gradient (part maps are constants).
+    Also returns the two renders ("A", "B")."""
+    k = dict(kw)
+    b0, b1, b2 = (float(c) for c in k.get("background_color", (0.0, 0.0, 0.0))[:3])
+    bg3 = float(k.pop("background_extra", 0.0))
+    ga = gb = None
+    if g is not None:
+        g = np.asarray(g, np.float32)
+        ga = np.ascontiguousarray(g[:, [0, 1, 2, 4]])
+        gb = np.zeros_like(ga)
+        gb[:, 0] = g[:, 3]
+    a = oracle("det", fv, tex[..., 0:3], isz, aa, ga, dict(k, background_color=(b0, b1, b2)), tex_abs=False)
+    b = oracle("det", fv, tex[..., [3, 0, 1]], isz, aa, gb, dict(k, background_color=(bg3, b0, b1)), tex_abs=False)
+    four = lambda x, y: np.concatenate([x[:, :3], y[:, :1], x[:, 3:]], 1)   # noqa: E731
+    out = dict(images=four(a["images"], b["images"]), colors=four(a["colors"], b["colors"]), aggrs=a["aggrs"], p2f=a["p2f"],
+               A=a, B=b)
+    if g is not None:
+        out["grad_faces"] = a["grad_faces"] + b["grad_faces"]
     return out
 
 

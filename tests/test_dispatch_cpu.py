@@ -174,6 +174,7 @@ ENTRIES = {
     "raster_generic": lambda dt: _raster(dt, dist_func="barycentric", aggr_func_alpha="sum"),
     "raster_hard": lambda dt: _raster(dt, aggr_func_rgb="hard"),
     "raster_part_map": lambda dt: _raster(dt, channels=4, tex=False, background_color=(0, 0, 0, 1)),
+    "raster_vertex_part_map": lambda dt: _raster(dt, channels=4, tex=False, texture_type="vertex"),
     "raster_aa": lambda dt: _raster(dt, anti_aliasing=True),
     "raster_texture_only": lambda dt: _raster(dt, geom=False),
     "raster_generic_texture_only": lambda dt: _raster(dt, geom=False, dist_func="barycentric"),
@@ -337,6 +338,10 @@ EXPECTED = {
             'umr_raster_workspace_bytes_deterministic:', 'umr_raster_forward_deterministic:111011p10',
             'umr_raster_workspace_bytes_deterministic:', 'umr_raster_backward_deterministic:1111110p10'
         ],
+        'f64': 'float64 rasterisation takes 3 colour channels, got 4 (part-map textures are float32 only)',
+    },
+    'raster_vertex_part_map': {
+        'f32 mixed half det': 'vertex textures take 3 colour channels, got 4 (4-channel part maps are surface textures only)',
         'f64': 'float64 rasterisation takes 3 colour channels, got 4 (part-map textures are float32 only)',
     },
     'raster_softmax': {

@@ -161,13 +161,10 @@ def test_backward(mode, wide):
 
 @pytest.mark.parametrize("wide", [False, True])
 def test_backward_four_channels(wide):
-    """(The default backward at 1280 faces only: its 4-channel recompute kernels are not opted into the large
-    shared-memory range, and their face list outgrows the default 48 KB at about 4000 faces.)"""
     for pairs in (False, True):
         r = Render(WIDE_F if wide else 1280, nc=4, tile=32, pairs=pairs)
         r.forward()
-        if not wide:
-            assert r.backward(tex=False) == (3 if pairs else 2), pairs
+        assert r.backward(tex=False) == (3 if pairs else 2), pairs
         assert r.backward(det=True, tex=False) == 2, pairs
 
 

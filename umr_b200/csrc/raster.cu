@@ -1257,7 +1257,10 @@ static PairBuf make_pairbuf(const UmrRasterParams* p, int S) {
 constexpr double TEXGRAD_PRE_RATIO_FULL = 160.0, TEXGRAD_PRE_RATIO_TEXONLY = 120.0;
 
 // Opt every raster kernel into the full dynamic shared-memory range ONCE per device (not per call:
-// the call may be inside a CUDA-graph capture).  A 65536-face window needs 8 KB + 32 KB + 128 KB.
+// the call may be inside a CUDA-graph capture).  A 65536-face window needs 8 KB + 32 KB + 128 KB.  Every kernel
+// launched with raster_dyn_smem (launch_pairs_backward's recompute kernels for each RGBM, TG, NC and SP it is called
+// with, the generic forward and backward) must be listed: without the opt-in, static plus dynamic shared memory is
+// capped at 48 KB, which the 4-channel recompute kernels pass from 1544 faces.
 static int ensure_smem_attrs() {
     static bool done[64] = {};
     int dev = 0;
@@ -1278,6 +1281,7 @@ static int ensure_smem_attrs() {
         (const void*)k_raster_bwd_pairs_list<0, false>, (const void*)k_raster_bwd_pairs_list<0, true>,
         (const void*)k_raster_bwd_pairs_list<1, false>, (const void*)k_raster_bwd_pairs_list<1, true>,
         (const void*)k_raster_bwd_pairs<1, true, 3, true>, (const void*)k_raster_bwd_pairs_list<1, true, 3, true>,
+        (const void*)k_raster_bwd_pairs<1, false, 4>, (const void*)k_raster_bwd_pairs_list<1, false, 4>,
         (const void*)k_raster_fwd4<RGB_SIL>, (const void*)k_raster_fwd4<RGB_SIL, uint32_t>,
         (const void*)k_raster_bwd_pairs<RGB_SIL, false>, (const void*)k_raster_bwd_pairs_list<RGB_SIL, false>,
     };

@@ -248,7 +248,10 @@ class SoftRasterizeFunction(torch.autograd.Function):
                              % int(tex.shape[-1]))
         # colour channels: 3, or 4 for the one-render part maps of part_matching_loss (SURVEY.md §8f-2); images then
         # carry NC + 1 planes (colours + alpha)
-        NC = int(tex.shape[-1]) if texture_type == "surface" and not mode.f64 else 3
+        NC = int(tex.shape[-1])
+        if texture_type != "surface" and NC != 3:   # the kernels would read it with a stride of 3
+            raise ValueError("%s textures take 3 colour channels, got %d (4-channel part maps are surface textures only)"
+                             % (texture_type, NC))
         if NC not in (3, 4):
             raise ValueError("textures must have 3 (or, surface textures only, 4) colour channels, got %d" % NC)
         S = int(image_size) * (2 if anti_aliasing else 1)
