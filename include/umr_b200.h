@@ -105,7 +105,8 @@ int umr_version(void);
 /* sizeof() of the parameter structs as compiled into the library (binding self-check). */
 size_t umr_sizeof_raster_params(void);
 size_t umr_sizeof_project_params(void);
-/* Number of kernels this library has launched in this process (all entry points, all threads). */
+/* Number of kernels this library has launched in this process (all entry points, all threads).  A call refused with an
+ * UMR_ERR_* code launches nothing and counts nothing. */
 uint64_t umr_launch_count(void);
 /* Thin event helpers so callers without a CUDA runtime binding can time on the launch stream. */
 int umr_event_create(void** event);

@@ -43,6 +43,7 @@ def test_workspace_formulas(B, N):
 
 def test_bad_arguments_refused():
     lib = _lib.load()
+    launches = lib.umr_launch_count()
     N0 = ctypes.c_void_p(0)
     assert lib.umr_bilinear_sample_forward_f64(N0, FAKE, FAKE, 1, 3, 4, 4, 10, None) == UMR_ERR_BAD_ARG
     assert lib.umr_bilinear_sample_forward_f64(FAKE, FAKE, FAKE, 0, 3, 4, 4, 10, None) == UMR_ERR_BAD_ARG
@@ -80,6 +81,7 @@ def test_bad_arguments_refused():
                                              N0, N0, FAKE, None) == UMR_ERR_BAD_ARG
     assert lib.umr_corr_chamfer_backward_f64(FAKE, 0, FAKE, FAKE, tp, tc, ends, wt, FAKE, FAKE, FAKE, N0, N0, FAKE, 65536, 4,
                                              9, N0, N0, N0, None) == UMR_ERR_TOO_LARGE
+    assert lib.umr_launch_count() == launches   # a refused call launches nothing
 
 
 def test_misaligned_vector_pointers_refused():
@@ -87,6 +89,7 @@ def test_misaligned_vector_pointers_refused():
     that is not a multiple of 2 * sizeof(element) is refused with UMR_ERR_BAD_ARG in every precision, before any launch
     (ops.py copies such an input to aligned storage first: test_dispatch_cpu.py::test_odd_offset_pairs_reach_the_library_aligned)."""
     lib = _lib.load()
+    launches = lib.umr_launch_count()
     N0 = ctypes.c_void_p(0)
     for suffix, step in (("", 4), ("_deterministic", 4), ("_f64", 8)):
         odd = ctypes.c_void_p(FAKE.value + step)   # aligned to the element, not to the pair
@@ -106,6 +109,7 @@ def test_misaligned_vector_pointers_refused():
             tbwd = getattr(lib, "umr_texcycle_backward" + suffix)
             for flow, prob, gflow in ((odd, FAKE, FAKE), (FAKE, odd, FAKE), (FAKE, FAKE, odd)):
                 assert tbwd(flow, prob, FAKE, FAKE, gflow, 2, 4, 9, None) == UMR_ERR_BAD_ARG, suffix
+    assert lib.umr_launch_count() == launches
 
 
 def test_texcycle_size_limit_in_every_precision():

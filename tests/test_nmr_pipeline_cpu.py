@@ -294,9 +294,11 @@ A = 4096  # a fake device address: every call below is refused before it touches
 ])
 def test_entry_point_refusals(kw, code):
     lib = _lib.load()
+    launches = lib.umr_launch_count()
     p = _p(**kw)
     assert lib.umr_nmr_lighting_forward(A, A, A, A, A, A, ctypes.byref(p), None) == code
     assert lib.umr_nmr_lighting_backward(A, A, A, A, A, A, A, A, A, ctypes.byref(p), A * 2, None) == code
+    assert lib.umr_launch_count() == launches   # a refused call launches nothing
 
 
 def test_entry_point_buffer_refusals():

@@ -152,14 +152,17 @@ SHAPE_REFUSALS = [
 
 @pytest.mark.parametrize("kw,code", SHAPE_REFUSALS, ids=[",".join("%s=%s" % i for i in k.items()) for k, _ in SHAPE_REFUSALS])
 def test_shapes_refused(kw, code):
+    launches = _lib.load().umr_launch_count()
     p = _params(**kw)
     assert _fwd(p) == code
     assert _bwd(p) == code and _bwd(p, det=True) == code
     if "T" in kw:   # without textures the texture size is ignored: the shape passes, the NULL workspace is refused
         assert _fwd(p, tex=N0, rgb=N0, ws=N0) == UMR_ERR_BAD_ARG
+    assert _lib.load().umr_launch_count() == launches   # a refused call launches nothing
 
 
 def test_pointers_and_alignment_refused():
+    launches = _lib.load().umr_launch_count()
     p = _params()
     for i in range(4):   # vertices, faces, face_index, raster_depth
         ptrs = [FAKE] * 4
@@ -178,6 +181,7 @@ def test_pointers_and_alignment_refused():
         for off in (1, 2, 3):
             assert _bwd(p, gt=ctypes.c_void_p(256 + off), det=det) == UMR_ERR_BAD_ARG   # grad_textures not 4-byte aligned
     assert _lib.load().umr_nmr_forward(FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, FAKE, None, FAKE, None) == UMR_ERR_BAD_ARG
+    assert _lib.load().umr_launch_count() == launches
 
 
 def _align256(x):

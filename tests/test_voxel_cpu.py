@@ -241,6 +241,7 @@ def test_refusals_without_gpu():
 def test_c_abi_refusals_without_gpu():
     """Argument checks return before any CUDA call."""
     lib = _lib.load()
+    launches = lib.umr_launch_count()
     p = ctypes.c_void_p(256)
     assert lib.umr_voxelize(p, 0, p, 1, 1, 0, 1.0, p, None) == -2          # size < 1: UMR_ERR_BAD_ARG
     assert lib.umr_voxelize(p, 2, p, 1, 1, 8, 1.0, p, None) == -2          # unknown dtype
@@ -248,6 +249,7 @@ def test_c_abi_refusals_without_gpu():
     vs = math.ceil(2 ** (31 / 3))                                           # B * vs^3 >= 2^31: UMR_ERR_TOO_LARGE
     assert lib.umr_voxelize(p, 0, p, 1, 1, vs, 1.0, p, None) == -3
     assert lib.umr_voxelize(p, 0, p, 2, 1, 1024, 1.0, p, None) == -3
+    assert lib.umr_launch_count() == launches   # a refused call launches nothing
     assert lib.umr_voxelize_workspace_bytes(1, vs) == 0
     assert lib.umr_voxelize_workspace_bytes(2, 64) >= 256 + 2 * 2 * 64 ** 3 // 8
     assert lib.umr_version() == 204

@@ -138,8 +138,7 @@ extern "C" int umr_p2p_allreduce(const void* peer_buffers_dev, float* out, int64
     unsigned grid = (unsigned)((n4 + 255) / 256);
     if (grid > (unsigned)sms) grid = (unsigned)sms;
     if (grid < 1) grid = 1;
-    count_launch();
-    k_p2p_allreduce<<<grid, 256, 0, st>>>((const uint64_t*)peer_buffers_dev, out, n4, (size_t)flag_offset_bytes,
-                                          (uint32_t*)local_state, rank, world, scale);
+    launch(k_p2p_allreduce, grid, 256, 0, st, (const uint64_t*)peer_buffers_dev, out, n4, (size_t)flag_offset_bytes,
+           (uint32_t*)local_state, rank, world, scale);
     return (int)cudaGetLastError();
 }

@@ -1,13 +1,22 @@
 // common.cuh -- small sm_90a device helpers shared by the kernels (mbarrier, TMA bulk copy,
-// warp reductions).  Inline PTX.
+// warp reductions; inline PTX), and the counted kernel launch of every C entry point.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <atomic>
+#include <utility>
 namespace umr {
 extern std::atomic<unsigned long long> g_launches;  // c_api.cu; read through umr_launch_count()
-inline void count_launch(int n = 1) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
+
+// Launches kernel(args...) with the given grid, block, dynamic shared memory and stream, counted in umr_launch_count().
+// Every kernel of the library is launched here, so the count is one per kernel launch by construction; memsets and event
+// records are not counted.
+template <typename... P, typename... A>
+inline void launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, A&&... args) {
+    kernel<<<grid, block, smem, stream>>>(std::forward<A>(args)...);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);

@@ -83,25 +83,9 @@ __global__ void __launch_bounds__(256) k_visible(const float* __restrict__ ids, 
 
 using namespace umr;
 
-#define UMR_RET_LAST() return (int)cudaGetLastError()
-
 extern "C" int umr_bilinear_sample_forward(const float* image, const float* flow, float* out, int32_t B,
                                            int32_t C, int32_t H, int32_t W, int32_t N, void* stream_) {
-    if (!image || !flow || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 || vec2_misaligned(flow))
-        return UMR_ERR_BAD_ARG;
-    if (B > 65535) return UMR_ERR_TOO_LARGE;
-    cudaStream_t st = (cudaStream_t)stream_;
-    const dim3 grid((N + 255) / 256, B);
-    const float2* fl = reinterpret_cast<const float2*>(flow);
-    count_launch();
-    switch (C) {
-        case 1: k_sample_fwd<float, 1><<<grid, 256, 0, st>>>(image, fl, out, H, W, N); break;
-        case 2: k_sample_fwd<float, 2><<<grid, 256, 0, st>>>(image, fl, out, H, W, N); break;
-        case 3: k_sample_fwd<float, 3><<<grid, 256, 0, st>>>(image, fl, out, H, W, N); break;
-        case 4: k_sample_fwd<float, 4><<<grid, 256, 0, st>>>(image, fl, out, H, W, N); break;
-        default: return UMR_ERR_UNSUPPORTED;
-    }
-    UMR_RET_LAST();
+    return sample_forward(image, flow, out, B, C, H, W, N, stream_);
 }
 
 extern "C" int umr_bilinear_sample_backward(const float* image, const float* flow, const float* grad_out,
@@ -111,23 +95,17 @@ extern "C" int umr_bilinear_sample_backward(const float* image, const float* flo
         vec2_misaligned(flow) || vec2_misaligned(grad_flow))
         return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
+    if (C > 4) return UMR_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream_;
     if (grad_image) {
         cudaError_t e = cudaMemsetAsync(grad_image, 0, (size_t)B * C * H * W * sizeof(float), st);
         if (e != cudaSuccess) return (int)e;
     }
-    const dim3 grid((N + 255) / 256, B);
-    const float2* fl = reinterpret_cast<const float2*>(flow);
-    float2* gf = reinterpret_cast<float2*>(grad_flow);
-    count_launch();
-    switch (C) {
-        case 1: k_sample_bwd<float, 1><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, grad_image, H, W, N); break;
-        case 2: k_sample_bwd<float, 2><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, grad_image, H, W, N); break;
-        case 3: k_sample_bwd<float, 3><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, grad_image, H, W, N); break;
-        case 4: k_sample_bwd<float, 4><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, grad_image, H, W, N); break;
-        default: return UMR_ERR_UNSUPPORTED;
-    }
-    UMR_RET_LAST();
+    with_channels(C, [&](auto c) {
+        launch(k_sample_bwd<float, c>, dim3((N + 255) / 256, B), 256, 0, st, image, reinterpret_cast<const float2*>(flow),
+               grad_out, reinterpret_cast<float2*>(grad_flow), grad_image, H, W, N);
+    });
+    return (int)cudaGetLastError();
 }
 
 extern "C" int umr_iou_forward(const float* predict, int64_t predict_bstride, const float* target, float* inter,
@@ -140,9 +118,9 @@ extern "C" int umr_iou_forward(const float* predict, int64_t predict_bstride, co
     e = cudaMemsetAsync(uni, 0, (size_t)B * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     const dim3 grid(iou_slots<float>(N), B);
-    count_launch(); k_iou_partial<float, false><<<grid, IOU_THREADS<float>, 0, st>>>(predict, target, inter, uni, N, predict_bstride);
-    count_launch(); k_iou_finalize<<<(B + 127) / 128, 128, 0, st>>>(inter, uni, loss, B);
-    UMR_RET_LAST();
+    launch(k_iou_partial<float, false>, grid, IOU_THREADS<float>, 0, st, predict, target, inter, uni, N, predict_bstride);
+    launch(k_iou_finalize, (B + 127) / 128, 128, 0, st, inter, uni, loss, B);
+    return (int)cudaGetLastError();
 }
 
 extern "C" int umr_iou_backward(const float* target, const float* inter, const float* uni, const float* grad_loss,
@@ -161,25 +139,16 @@ extern "C" int umr_chamfer_backward(const float* a, const float* b, const int32_
     if (!a || !b || !grad_a || !grad_b || B <= 0 || N <= 0 || M <= 0) return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     if (D != 2 && D != 3) return UMR_ERR_UNSUPPORTED;
+    if ((grad_dist_ab && !idx_ab) || (grad_dist_ba && !idx_ba)) return UMR_ERR_BAD_ARG;
     cudaStream_t st = (cudaStream_t)stream_;
     cudaError_t e = cudaMemsetAsync(grad_a, 0, (size_t)B * N * D * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
     e = cudaMemsetAsync(grad_b, 0, (size_t)B * M * D * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
-    const dim3 g1((N + 255) / 256, B), g2((M + 255) / 256, B);
-    if (grad_dist_ab) {
-        if (!idx_ab) return UMR_ERR_BAD_ARG;
-        count_launch();
-        if (D == 2) k_chamfer_bwd<2><<<g1, 256, 0, st>>>(a, b, idx_ab, grad_dist_ab, grad_a, grad_b, N, M);
-        else k_chamfer_bwd<3><<<g1, 256, 0, st>>>(a, b, idx_ab, grad_dist_ab, grad_a, grad_b, N, M);
-    }
-    if (grad_dist_ba) {
-        if (!idx_ba) return UMR_ERR_BAD_ARG;
-        count_launch();
-        if (D == 2) k_chamfer_bwd<2><<<g2, 256, 0, st>>>(b, a, idx_ba, grad_dist_ba, grad_b, grad_a, M, N);
-        else k_chamfer_bwd<3><<<g2, 256, 0, st>>>(b, a, idx_ba, grad_dist_ba, grad_b, grad_a, M, N);
-    }
-    UMR_RET_LAST();
+    auto bwd = D == 2 ? k_chamfer_bwd<2> : k_chamfer_bwd<3>;
+    if (grad_dist_ab) launch(bwd, dim3((N + 255) / 256, B), 256, 0, st, a, b, idx_ab, grad_dist_ab, grad_a, grad_b, N, M);
+    if (grad_dist_ba) launch(bwd, dim3((M + 255) / 256, B), 256, 0, st, b, a, idx_ba, grad_dist_ba, grad_b, grad_a, M, N);
+    return (int)cudaGetLastError();
 }
 
 extern "C" int umr_texcycle_forward(const float* flow, const float* prob, const float* face_ids, uint8_t* visible,
@@ -196,13 +165,13 @@ extern "C" int umr_texcycle_forward(const float* flow, const float* prob, const 
         e = cudaMemsetAsync(visible, 0, (size_t)B * F, st);
         if (e != cudaSuccess) return (int)e;
         const int64_t blocks = (P / 4 + 255) / 256 + 1;
-        count_launch(); k_visible<<<dim3((unsigned)(blocks > 1024 ? 1024 : blocks), B), 256, 0, st>>>(face_ids, visible, F, P);
+        launch(k_visible, dim3((unsigned)(blocks > 1024 ? 1024 : blocks), B), 256, 0, st, face_ids, visible, F, P);
     }
     const int n = B * F;
     const float scale = 1.f / ((float)n * 2.f);  // MSELoss mean over B*F*2 elements
-    count_launch(); k_texcycle_fwd<float, false><<<(n + 255) / 256, 256, 0, st>>>(reinterpret_cast<const float2*>(flow),
-                                                    reinterpret_cast<const float2*>(prob), visible, loss, n, T2, scale);
-    UMR_RET_LAST();
+    launch(k_texcycle_fwd<float, false>, (n + 255) / 256, 256, 0, st, reinterpret_cast<const float2*>(flow),
+           reinterpret_cast<const float2*>(prob), visible, loss, n, T2, scale);
+    return (int)cudaGetLastError();
 }
 
 extern "C" int umr_texcycle_backward(const float* flow, const float* prob, const uint8_t* visible, const float* grad_loss,
@@ -225,10 +194,9 @@ extern "C" int umr_masked_l1_forward(const float* pred, int64_t pred_bstride, co
     if (e != cudaSuccess) return (int)e;
     const dim3 grid(ml1_slots(HW), B);
     const float inv_n = 1.f / ((float)C * (float)HW);
-    count_launch();
-    if (C == 3) k_masked_l1_fwd<float, 3, false><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, loss, HW, inv_n);
-    else k_masked_l1_fwd<float, 1, false><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, loss, HW, inv_n);
-    UMR_RET_LAST();
+    launch(C == 3 ? k_masked_l1_fwd<float, 3, false> : k_masked_l1_fwd<float, 1, false>, grid, ML1_THREADS, 0, st, pred,
+           pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, loss, HW, inv_n);
+    return (int)cudaGetLastError();
 }
 
 extern "C" int umr_masked_l1_backward(const float* pred, int64_t pred_bstride, const float* mask_pred,
@@ -247,9 +215,8 @@ extern "C" int umr_loss_head_forward(const float* rgba, const float* gt, const f
     cudaStream_t st = (cudaStream_t)stream_;
     cudaError_t e = cudaMemsetAsync(stats, 0, (size_t)B * 3 * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
-    count_launch(2);
-    k_losshead_partial<float, false><<<dim3(lh_slots(HW), B), LH_THREADS, 0, st>>>(rgba, gt, mask_gt, stats, HW);
-    k_losshead_finalize<float><<<1, 32, 0, st>>>(stats, per_image, loss, B, 1.f / (3.f * (float)HW), w_iou, w_tex);
+    launch(k_losshead_partial<float, false>, dim3(lh_slots(HW), B), LH_THREADS, 0, st, rgba, gt, mask_gt, stats, HW);
+    launch(k_losshead_finalize<float>, 1, 32, 0, st, stats, per_image, loss, B, 1.f / (3.f * (float)HW), w_iou, w_tex);
     return (int)cudaGetLastError();
 }
 
@@ -281,10 +248,6 @@ extern "C" size_t umr_texcycle_workspace_bytes_deterministic(int32_t B, int32_t 
 extern "C" int umr_texcycle_forward_deterministic(const float* flow, const float* prob, const float* face_ids, uint8_t* visible,
                                                   float* loss, int32_t B, int32_t F, int32_t T2, int64_t P, void* workspace,
                                                   void* stream_) {
-    if (!flow || !prob || !visible || !loss || !workspace || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0) ||
-        vec2_misaligned(flow) || vec2_misaligned(prob))
-        return UMR_ERR_BAD_ARG;
-    if (B > 65535 || (int64_t)B * F > INT_MAX) return UMR_ERR_TOO_LARGE;
     return texcycle_forward_slots(flow, prob, face_ids, visible, loss, B, F, T2, P, workspace, stream_);
 }
 
@@ -313,12 +276,6 @@ extern "C" int umr_bilinear_sample_backward_deterministic(const float* image, co
                                                           float* grad_flow, float* grad_image, int32_t B, int32_t C, int32_t H,
                                                           int32_t W, int32_t N, const int32_t* cell_rowptr,
                                                           const int32_t* cell_samples, void* stream_) {
-    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 ||
-        vec2_misaligned(flow) || vec2_misaligned(grad_flow))
-        return UMR_ERR_BAD_ARG;
-    if (grad_image && (!cell_rowptr || !cell_samples)) return UMR_ERR_BAD_ARG;
-    if (cells_too_large(B, H, W)) return UMR_ERR_TOO_LARGE;
-    if (C < 1 || C > 4) return UMR_ERR_UNSUPPORTED;
     return sample_backward_gather(image, flow, grad_out, grad_flow, grad_image, B, C, H, W, N, cell_rowptr, cell_samples,
                                   stream_);
 }

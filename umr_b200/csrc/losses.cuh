@@ -904,40 +904,60 @@ static inline bool vec2_misaligned(const T* p) {
     return ((uintptr_t)p & (2 * sizeof(T) - 1)) != 0;
 }
 
+// f(std::integral_constant<int, C>{}) for the channel count C of the sampler kernels; 1 <= C <= 4
+template <typename Fn>
+static void with_channels(int32_t C, Fn&& f) {
+    switch (C) {
+        case 1: f(std::integral_constant<int, 1>{}); break;
+        case 2: f(std::integral_constant<int, 2>{}); break;
+        case 3: f(std::integral_constant<int, 3>{}); break;
+        default: f(std::integral_constant<int, 4>{}); break;
+    }
+}
+
+template <typename T>
+static int sample_forward(const T* image, const T* flow, T* out, int32_t B, int32_t C, int32_t H, int32_t W, int32_t N,
+                          void* stream_) {
+    if (!image || !flow || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 || vec2_misaligned(flow))
+        return UMR_ERR_BAD_ARG;
+    if (B > 65535) return UMR_ERR_TOO_LARGE;
+    if (C > 4) return UMR_ERR_UNSUPPORTED;
+    with_channels(C, [&](auto c) {
+        launch(k_sample_fwd<T, c>, dim3((N + 255) / 256, B), 256, 0, (cudaStream_t)stream_, image,
+               reinterpret_cast<const vec2_t<T>*>(flow), out, H, W, N);
+    });
+    return (int)cudaGetLastError();
+}
+
 template <typename T>
 static int sample_cells(const T* flow, int32_t* cells, int32_t B, int32_t H, int32_t W, int32_t N, void* stream_) {
     if (!flow || !cells || B <= 0 || H <= 0 || W <= 0 || N <= 0 || vec2_misaligned(flow)) return UMR_ERR_BAD_ARG;
     if (cells_too_large(B, H, W)) return UMR_ERR_TOO_LARGE;
-    count_launch();
-    k_sample_cells<T><<<dim3((N + 255) / 256, B), 256, 0, (cudaStream_t)stream_>>>(
-        reinterpret_cast<const vec2_t<T>*>(flow), cells, B, H, W, N);
+    launch(k_sample_cells<T>, dim3((N + 255) / 256, B), 256, 0, (cudaStream_t)stream_,
+           reinterpret_cast<const vec2_t<T>*>(flow), cells, B, H, W, N);
     return (int)cudaGetLastError();
 }
 
-// grad_flow from k_sample_bwd (no image gradient there), the image gradient from the per-pixel gather; 1 <= C <= 4
+// grad_flow from k_sample_bwd (no image gradient there), the image gradient from the per-pixel gather over the cell table
 template <typename T>
 static int sample_backward_gather(const T* image, const T* flow, const T* grad_out, T* grad_flow, T* grad_image, int32_t B,
                                   int32_t C, int32_t H, int32_t W, int32_t N, const int32_t* cell_rowptr,
                                   const int32_t* cell_samples, void* stream_) {
+    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 ||
+        vec2_misaligned(flow) || vec2_misaligned(grad_flow))
+        return UMR_ERR_BAD_ARG;
+    if (grad_image && (!cell_rowptr || !cell_samples)) return UMR_ERR_BAD_ARG;
+    if (cells_too_large(B, H, W)) return UMR_ERR_TOO_LARGE;
+    if (C > 4) return UMR_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream_;
-    const dim3 grid((N + 255) / 256, B), gpix((H * W + 255) / 256, B);
     const vec2_t<T>* fl = reinterpret_cast<const vec2_t<T>*>(flow);
-    vec2_t<T>* gf = reinterpret_cast<vec2_t<T>*>(grad_flow);
-    count_launch(grad_image ? 2 : 1);
-    switch (C) {
-        case 1: k_sample_bwd<T, 1><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, nullptr, H, W, N); break;
-        case 2: k_sample_bwd<T, 2><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, nullptr, H, W, N); break;
-        case 3: k_sample_bwd<T, 3><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, nullptr, H, W, N); break;
-        default: k_sample_bwd<T, 4><<<grid, 256, 0, st>>>(image, fl, grad_out, gf, nullptr, H, W, N); break;
-    }
-    if (grad_image) {
-        switch (C) {
-            case 1: k_sample_bwd_image_gather<T, 1><<<gpix, 256, 0, st>>>(fl, grad_out, cell_rowptr, cell_samples, grad_image, H, W); break;
-            case 2: k_sample_bwd_image_gather<T, 2><<<gpix, 256, 0, st>>>(fl, grad_out, cell_rowptr, cell_samples, grad_image, H, W); break;
-            case 3: k_sample_bwd_image_gather<T, 3><<<gpix, 256, 0, st>>>(fl, grad_out, cell_rowptr, cell_samples, grad_image, H, W); break;
-            default: k_sample_bwd_image_gather<T, 4><<<gpix, 256, 0, st>>>(fl, grad_out, cell_rowptr, cell_samples, grad_image, H, W); break;
-        }
-    }
+    with_channels(C, [&](auto c) {
+        launch(k_sample_bwd<T, c>, dim3((N + 255) / 256, B), 256, 0, st, image, fl, grad_out,
+               reinterpret_cast<vec2_t<T>*>(grad_flow), nullptr, H, W, N);
+        if (grad_image)
+            launch(k_sample_bwd_image_gather<T, c>, dim3((H * W + 255) / 256, B), 256, 0, st, fl, grad_out, cell_rowptr,
+                   cell_samples, grad_image, H, W);
+    });
     return (int)cudaGetLastError();
 }
 
@@ -955,9 +975,8 @@ static int iou_forward_slots(const T* predict, int64_t predict_bstride, const T*
     const unsigned gx = iou_slots<T>(N);
     T* si = (T*)workspace;
     T* su = si + (size_t)B * gx;
-    count_launch(2);
-    k_iou_partial<T, true><<<dim3(gx, B), IOU_THREADS<T>, 0, st>>>(predict, target, si, su, N, predict_bstride);
-    k_iou_finalize_det<T><<<(B + 127) / 128, 128, 0, st>>>(si, su, inter, uni, loss, B, (int)gx);
+    launch(k_iou_partial<T, true>, dim3(gx, B), IOU_THREADS<T>, 0, st, predict, target, si, su, N, predict_bstride);
+    launch(k_iou_finalize_det<T>, (B + 127) / 128, 128, 0, st, si, su, inter, uni, loss, B, (int)gx);
     return (int)cudaGetLastError();
 }
 template <typename T>
@@ -966,8 +985,7 @@ static int iou_backward(const T* target, const T* inter, const T* uni, const T* 
     if (!target || !inter || !uni || !grad_loss || !grad_predict || B <= 0 || N <= 0) return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     const unsigned gx = (unsigned)std::min<int64_t>((N + 1023) / 1024, 1024);
-    count_launch();
-    k_iou_bwd<T><<<dim3(gx, B), 256, 0, (cudaStream_t)stream_>>>(target, inter, uni, grad_loss, grad_predict, N);
+    launch(k_iou_bwd<T>, dim3(gx, B), 256, 0, (cudaStream_t)stream_, target, inter, uni, grad_loss, grad_predict, N);
     return (int)cudaGetLastError();
 }
 
@@ -979,14 +997,9 @@ static int chamfer_forward(const T* a, const T* b, T* dist_ab, T* dist_ba, int32
     if (D != 2 && D != 3) return UMR_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream_;
     const dim3 g1((N + 7) / 8, B), g2((M + 7) / 8, B);
-    count_launch(2);
-    if (D == 2) {
-        k_chamfer_nn<T, 2><<<g1, 256, 0, st>>>(a, b, dist_ab, idx_ab, N, M);
-        k_chamfer_nn<T, 2><<<g2, 256, 0, st>>>(b, a, dist_ba, idx_ba, M, N);
-    } else {
-        k_chamfer_nn<T, 3><<<g1, 256, 0, st>>>(a, b, dist_ab, idx_ab, N, M);
-        k_chamfer_nn<T, 3><<<g2, 256, 0, st>>>(b, a, dist_ba, idx_ba, M, N);
-    }
+    auto nn = D == 2 ? k_chamfer_nn<T, 2> : k_chamfer_nn<T, 3>;
+    launch(nn, g1, 256, 0, st, a, b, dist_ab, idx_ab, N, M);
+    launch(nn, g2, 256, 0, st, b, a, dist_ba, idx_ba, M, N);
     return (int)cudaGetLastError();
 }
 template <typename T>
@@ -999,14 +1012,9 @@ static int chamfer_backward_gather(const T* a, const T* b, const int32_t* idx_ab
     if (D != 2 && D != 3) return UMR_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream_;
     const dim3 g1((N + 7) / 8, B), g2((M + 7) / 8, B);  // one warp per output point
-    count_launch(2);
-    if (D == 2) {
-        k_chamfer_bwd_gather<T, 2><<<g1, 256, 0, st>>>(a, b, idx_ab, idx_ba, grad_dist_ab, grad_dist_ba, grad_a, N, M);
-        k_chamfer_bwd_gather<T, 2><<<g2, 256, 0, st>>>(b, a, idx_ba, idx_ab, grad_dist_ba, grad_dist_ab, grad_b, M, N);
-    } else {
-        k_chamfer_bwd_gather<T, 3><<<g1, 256, 0, st>>>(a, b, idx_ab, idx_ba, grad_dist_ab, grad_dist_ba, grad_a, N, M);
-        k_chamfer_bwd_gather<T, 3><<<g2, 256, 0, st>>>(b, a, idx_ba, idx_ab, grad_dist_ba, grad_dist_ab, grad_b, M, N);
-    }
+    auto gather = D == 2 ? k_chamfer_bwd_gather<T, 2> : k_chamfer_bwd_gather<T, 3>;
+    launch(gather, g1, 256, 0, st, a, b, idx_ab, idx_ba, grad_dist_ab, grad_dist_ba, grad_a, N, M);
+    launch(gather, g2, 256, 0, st, b, a, idx_ba, idx_ab, grad_dist_ba, grad_dist_ab, grad_b, M, N);
     return (int)cudaGetLastError();
 }
 
@@ -1015,24 +1023,28 @@ static size_t texcycle_workspace_bytes(int32_t B, int32_t F) {
     if (B <= 0 || F <= 0) return 0;
     return (size_t)(((int64_t)B * F + 255) / 256) * sizeof(T);
 }
-// after the entry point's checks: the bitmap of the face-id plane (if given), the per-CTA slots and their sum
+// the bitmap of the face-id plane (if given; NULL: `visible` was already filled by umr_raster_visibility), the per-CTA
+// slots and their sum
 template <typename T>
 static int texcycle_forward_slots(const T* flow, const T* prob, const float* face_ids, uint8_t* visible, T* loss, int32_t B,
                                   int32_t F, int32_t T2, int64_t P, void* workspace, void* stream_) {
+    if (!flow || !prob || !visible || !loss || !workspace || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0) ||
+        vec2_misaligned(flow) || vec2_misaligned(prob))
+        return UMR_ERR_BAD_ARG;
+    if (B > 65535 || (int64_t)B * F > INT_MAX) return UMR_ERR_TOO_LARGE;
     cudaStream_t st = (cudaStream_t)stream_;
     if (face_ids) {   // the bitmap only ever receives 1s: its bytes do not depend on the order of the stores
         cudaError_t e = cudaMemsetAsync(visible, 0, (size_t)B * F, st);
         if (e != cudaSuccess) return (int)e;
         const int64_t blocks = (P / 4 + 255) / 256 + 1;
-        count_launch(); k_visible<<<dim3((unsigned)(blocks > 1024 ? 1024 : blocks), B), 256, 0, st>>>(face_ids, visible, F, P);
+        launch(k_visible, dim3((unsigned)(blocks > 1024 ? 1024 : blocks), B), 256, 0, st, face_ids, visible, F, P);
     }
     const int n = B * F;
     const int gx = (n + 255) / 256;
     T* slots = (T*)workspace;
-    count_launch(2);
-    k_texcycle_fwd<T, true><<<gx, 256, 0, st>>>(reinterpret_cast<const vec2_t<T>*>(flow), reinterpret_cast<const vec2_t<T>*>(prob),
-                                                visible, slots, n, T2, T(1) / ((T)n * T(2)));  // MSELoss mean over B*F*2
-    k_sum_slot_rows<T><<<1, 32, 0, st>>>(slots, loss, 1, gx);
+    launch(k_texcycle_fwd<T, true>, gx, 256, 0, st, reinterpret_cast<const vec2_t<T>*>(flow),
+           reinterpret_cast<const vec2_t<T>*>(prob), visible, slots, n, T2, T(1) / ((T)n * T(2)));  // MSELoss mean over B*F*2
+    launch(k_sum_slot_rows<T>, 1, 32, 0, st, slots, loss, 1, gx);
     return (int)cudaGetLastError();
 }
 // after the entry point's checks
@@ -1040,10 +1052,9 @@ template <typename T>
 static int texcycle_backward(const T* flow, const T* prob, const uint8_t* visible, const T* grad_loss, T* grad_flow, int32_t B,
                              int32_t F, int32_t T2, void* stream_) {
     const int n = B * F;
-    count_launch();
-    k_texcycle_bwd<T><<<(n + 255) / 256, 256, 0, (cudaStream_t)stream_>>>(
-        reinterpret_cast<const vec2_t<T>*>(flow), reinterpret_cast<const vec2_t<T>*>(prob), visible, grad_loss,
-        reinterpret_cast<vec2_t<T>*>(grad_flow), n, T2, T(1) / ((T)n * T(2)));
+    launch(k_texcycle_bwd<T>, (n + 255) / 256, 256, 0, (cudaStream_t)stream_, reinterpret_cast<const vec2_t<T>*>(flow),
+           reinterpret_cast<const vec2_t<T>*>(prob), visible, grad_loss, reinterpret_cast<vec2_t<T>*>(grad_flow), n, T2,
+           T(1) / ((T)n * T(2)));
     return (int)cudaGetLastError();
 }
 
@@ -1064,10 +1075,9 @@ static int masked_l1_forward_slots(const T* pred, int64_t pred_bstride, const T*
     const dim3 grid(gx, B);
     const T inv_n = T(1) / ((T)C * (T)HW);
     T* slots = (T*)workspace;
-    count_launch(2);
-    if (C == 3) k_masked_l1_fwd<T, 3, true><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, slots, HW, inv_n);
-    else k_masked_l1_fwd<T, 1, true><<<grid, ML1_THREADS, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, slots, HW, inv_n);
-    k_sum_slot_rows<T><<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, (int)gx);
+    launch(C == 3 ? k_masked_l1_fwd<T, 3, true> : k_masked_l1_fwd<T, 1, true>, grid, ML1_THREADS, 0, st, pred, pred_bstride,
+           mask_pred, mask_pred_bstride, gt, mask_gt, slots, HW, inv_n);
+    launch(k_sum_slot_rows<T>, (B + 127) / 128, 128, 0, st, slots, loss, B, (int)gx);
     return (int)cudaGetLastError();
 }
 template <typename T>
@@ -1080,9 +1090,8 @@ static int masked_l1_backward(const T* pred, int64_t pred_bstride, const T* mask
     cudaStream_t st = (cudaStream_t)stream_;
     const dim3 grid((unsigned)std::min<int64_t>((HW + 1023) / 1024, 1024), B);
     const T inv_n = T(1) / ((T)C * (T)HW);
-    count_launch();
-    if (C == 3) k_masked_l1_bwd<T, 3><<<grid, 256, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, grad_loss, grad_pred, grad_mask_pred, HW, inv_n);
-    else k_masked_l1_bwd<T, 1><<<grid, 256, 0, st>>>(pred, pred_bstride, mask_pred, mask_pred_bstride, gt, mask_gt, grad_loss, grad_pred, grad_mask_pred, HW, inv_n);
+    launch(C == 3 ? k_masked_l1_bwd<T, 3> : k_masked_l1_bwd<T, 1>, grid, 256, 0, st, pred, pred_bstride, mask_pred,
+           mask_pred_bstride, gt, mask_gt, grad_loss, grad_pred, grad_mask_pred, HW, inv_n);
     return (int)cudaGetLastError();
 }
 
@@ -1099,10 +1108,9 @@ static int loss_head_forward_slots(const T* rgba, const T* gt, const T* mask_gt,
     cudaStream_t st = (cudaStream_t)stream_;
     const unsigned gx = lh_slots(HW);
     T* slots = (T*)workspace;
-    count_launch(3);
-    k_losshead_partial<T, true><<<dim3(gx, B), LH_THREADS, 0, st>>>(rgba, gt, mask_gt, slots, HW);
-    k_losshead_sum<T><<<(3 * B + 127) / 128, 128, 0, st>>>(slots, stats, B, (int)gx);
-    k_losshead_finalize<T><<<1, 32, 0, st>>>(stats, per_image, loss, B, T(1) / (T(3) * (T)HW), w_iou, w_tex);
+    launch(k_losshead_partial<T, true>, dim3(gx, B), LH_THREADS, 0, st, rgba, gt, mask_gt, slots, HW);
+    launch(k_losshead_sum<T>, (3 * B + 127) / 128, 128, 0, st, slots, stats, B, (int)gx);
+    launch(k_losshead_finalize<T>, 1, 32, 0, st, stats, per_image, loss, B, T(1) / (T(3) * (T)HW), w_iou, w_tex);
     return (int)cudaGetLastError();
 }
 template <typename T>
@@ -1111,9 +1119,8 @@ static int loss_head_backward(const T* rgba, const T* gt, const T* mask_gt, cons
     if (!rgba || !gt || !mask_gt || !stats || !grad_loss || !grad_rgba || B <= 0 || HW <= 0) return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     const unsigned gx = (unsigned)std::min<int64_t>((HW + 255) / 256, 1024);
-    count_launch();
-    k_losshead_bwd<T><<<dim3(gx, B), 256, 0, (cudaStream_t)stream_>>>(rgba, gt, mask_gt, stats, grad_loss, grad_rgba, HW, B,
-                                                                      T(1) / (T(3) * (T)HW), w_iou, w_tex);
+    launch(k_losshead_bwd<T>, dim3(gx, B), 256, 0, (cudaStream_t)stream_, rgba, gt, mask_gt, stats, grad_loss, grad_rgba, HW,
+           B, T(1) / (T(3) * (T)HW), w_iou, w_tex);
     return (int)cudaGetLastError();
 }
 
@@ -1165,12 +1172,11 @@ static int part_head_forward(const T* const* maps, const int64_t* map_bstrides, 
     T* slots = stats + (size_t)B * PH_STATS;
     int32_t* idx = (int32_t*)(slots + (size_t)B * ns * PH_SLOT);
     int32_t* slot_idx = idx + (size_t)B * PH_IDX;
-    count_launch(kld ? 2 : 4);
-    k_part_head_partial<T><<<dim3(ns, B), PH_THREADS, 0, st>>>(in, slots, slot_idx, H, kld);
-    k_part_head_finalize<T><<<B, 64, 0, st>>>(slots, slot_idx, stats, idx, terms, ns, kld);
+    launch(k_part_head_partial<T>, dim3(ns, B), PH_THREADS, 0, st, in, slots, slot_idx, H, kld);
+    launch(k_part_head_finalize<T>, B, 64, 0, st, slots, slot_idx, stats, idx, terms, ns, kld);
     if (!kld) {
-        k_part_head_mse<T><<<dim3(ns, B), PH_THREADS, 0, st>>>(in, weights, stats, slots, H);
-        k_part_head_mse_finalize<T><<<B, 32, 0, st>>>(slots, stats, terms, ns);
+        launch(k_part_head_mse<T>, dim3(ns, B), PH_THREADS, 0, st, in, weights, stats, slots, H);
+        launch(k_part_head_mse_finalize<T>, B, 32, 0, st, slots, stats, terms, ns);
     }
     return (int)cudaGetLastError();
 }
@@ -1187,8 +1193,8 @@ static int part_head_backward(const T* const* maps, const int64_t* map_bstrides,
     const T* stats = (const T*)workspace;
     const int32_t* idx = (const int32_t*)(stats + (size_t)B * PH_STATS + (size_t)B * ph_slots(H) * PH_SLOT);
     const unsigned gx = (unsigned)std::min<int64_t>((HW + 255) / 256, 1024);
-    count_launch();
-    k_part_head_bwd<T><<<dim3(gx, B), 256, 0, (cudaStream_t)stream_>>>(in, weights, stats, idx, grad_terms, grad_maps, H, kld);
+    launch(k_part_head_bwd<T>, dim3(gx, B), 256, 0, (cudaStream_t)stream_, in, weights, stats, idx, grad_terms, grad_maps, H,
+           kld);
     return (int)cudaGetLastError();
 }
 // losses_f64.cu: the double instantiations, reached through the dtype argument of the entry points in losses.cu

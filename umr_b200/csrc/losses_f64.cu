@@ -20,25 +20,9 @@
 
 using namespace umr;
 
-#define UMR_RET_LAST() return (int)cudaGetLastError()
-
 extern "C" int umr_bilinear_sample_forward_f64(const double* image, const double* flow, double* out, int32_t B, int32_t C,
                                                int32_t H, int32_t W, int32_t N, void* stream_) {
-    if (!image || !flow || !out || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 || vec2_misaligned(flow))
-        return UMR_ERR_BAD_ARG;
-    if (B > 65535) return UMR_ERR_TOO_LARGE;
-    if (C > 4) return UMR_ERR_UNSUPPORTED;
-    cudaStream_t st = (cudaStream_t)stream_;
-    const dim3 grid((N + 255) / 256, B);
-    const double2* fl = reinterpret_cast<const double2*>(flow);
-    count_launch();
-    switch (C) {
-        case 1: k_sample_fwd<double, 1><<<grid, 256, 0, st>>>(image, fl, out, H, W, N); break;
-        case 2: k_sample_fwd<double, 2><<<grid, 256, 0, st>>>(image, fl, out, H, W, N); break;
-        case 3: k_sample_fwd<double, 3><<<grid, 256, 0, st>>>(image, fl, out, H, W, N); break;
-        default: k_sample_fwd<double, 4><<<grid, 256, 0, st>>>(image, fl, out, H, W, N); break;
-    }
-    UMR_RET_LAST();
+    return sample_forward(image, flow, out, B, C, H, W, N, stream_);
 }
 
 extern "C" int umr_bilinear_sample_cells_f64(const double* flow, int32_t* cells, int32_t B, int32_t H, int32_t W, int32_t N,
@@ -50,12 +34,6 @@ extern "C" int umr_bilinear_sample_backward_f64(const double* image, const doubl
                                                 double* grad_flow, double* grad_image, int32_t B, int32_t C, int32_t H,
                                                 int32_t W, int32_t N, const int32_t* cell_rowptr,
                                                 const int32_t* cell_samples, void* stream_) {
-    if (!image || !flow || !grad_out || !grad_flow || B <= 0 || C <= 0 || H <= 0 || W <= 0 || N <= 0 ||
-        vec2_misaligned(flow) || vec2_misaligned(grad_flow))
-        return UMR_ERR_BAD_ARG;
-    if (grad_image && (!cell_rowptr || !cell_samples)) return UMR_ERR_BAD_ARG;
-    if (cells_too_large(B, H, W)) return UMR_ERR_TOO_LARGE;
-    if (C > 4) return UMR_ERR_UNSUPPORTED;
     return sample_backward_gather(image, flow, grad_out, grad_flow, grad_image, B, C, H, W, N, cell_rowptr, cell_samples,
                                   stream_);
 }
@@ -111,10 +89,6 @@ extern "C" size_t umr_texcycle_workspace_bytes_f64(int32_t B, int32_t F) { retur
 extern "C" int umr_texcycle_forward_f64(const double* flow, const double* prob, const float* face_ids, uint8_t* visible,
                                         double* loss, int32_t B, int32_t F, int32_t T2, int64_t P, void* workspace,
                                         void* stream_) {
-    if (!flow || !prob || !visible || !loss || !workspace || B <= 0 || F <= 0 || T2 <= 0 || (face_ids && P <= 0) ||
-        vec2_misaligned(flow) || vec2_misaligned(prob))
-        return UMR_ERR_BAD_ARG;
-    if (B > 65535 || (int64_t)B * F > INT_MAX) return UMR_ERR_TOO_LARGE;
     return texcycle_forward_slots(flow, prob, face_ids, visible, loss, B, F, T2, P, workspace, stream_);
 }
 extern "C" int umr_texcycle_backward_f64(const double* flow, const double* prob, const uint8_t* visible, const double* grad_loss,

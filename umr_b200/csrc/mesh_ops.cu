@@ -369,8 +369,6 @@ __global__ void __launch_bounds__(256) k_edt_rows(const int32_t* __restrict__ g_
 
 using namespace umr;
 
-#define UMR_RET() return (int)cudaGetLastError()
-
 extern "C" int umr_create_texture_image(const float* faces_uv, const float* textures, float* image, int32_t num_faces,
                                         int32_t texture_res_in, int32_t image_height, int32_t image_width, float eps,
                                         void* stream_) {
@@ -380,10 +378,9 @@ extern "C" int umr_create_texture_image(const float* faces_uv, const float* text
     const int R_out = image_width / tile_width;                       // :82 (image.size(1) / tile_width)
     if (R_out <= 0) return UMR_ERR_BAD_ARG;
     const int64_t npix = (int64_t)image_height * image_width;
-    count_launch();
-    k_create_texture_image<<<(unsigned)((npix + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(
-        faces_uv, textures, image, npix, num_faces, texture_res_in, R_out, tile_width, eps);
-    UMR_RET();
+    launch(k_create_texture_image, (unsigned)((npix + 255) / 256), 256, 0, (cudaStream_t)stream_, faces_uv, textures, image,
+           npix, num_faces, texture_res_in, R_out, tile_width, eps);
+    return (int)cudaGetLastError();
 }
 
 extern "C" int umr_load_textures(const float* image, const float* faces_uv, const int32_t* is_update, float* textures,
@@ -392,11 +389,9 @@ extern "C" int umr_load_textures(const float* image, const float* faces_uv, cons
     if (!image || !faces_uv || !is_update || !textures || num_faces <= 0 || texture_res <= 0 || image_height <= 1 || image_width <= 1)
         return UMR_ERR_BAD_ARG;
     const int64_t ntexel = (int64_t)num_faces * texture_res * texture_res;
-    count_launch();
-    k_load_textures<<<(unsigned)((ntexel + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(image, faces_uv, is_update, textures,
-                                                                                         ntexel, texture_res, image_height,
-                                                                                         image_width);
-    UMR_RET();
+    launch(k_load_textures, (unsigned)((ntexel + 255) / 256), 256, 0, (cudaStream_t)stream_, image, faces_uv, is_update,
+           textures, ntexel, texture_res, image_height, image_width);
+    return (int)cudaGetLastError();
 }
 
 extern "C" int umr_laplacian_forward(const float* x, const int32_t* rowptr, const int32_t* col, const float* coef, float* y,
@@ -406,9 +401,8 @@ extern "C" int umr_laplacian_forward(const float* x, const int32_t* rowptr, cons
     cudaStream_t st = (cudaStream_t)stream_;
     cudaError_t e = cudaMemsetAsync(loss, 0, (size_t)B * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
-    count_launch();
-    k_laplacian_fwd<float, false><<<dim3((V + 255) / 256, B), 256, 0, st>>>(x, rowptr, col, coef, y, loss, V);
-    UMR_RET();
+    launch(k_laplacian_fwd<float, false>, dim3((V + 255) / 256, B), 256, 0, st, x, rowptr, col, coef, y, loss, V);
+    return (int)cudaGetLastError();
 }
 // float32 (default and deterministic mode: one writer per element) and float64
 template <typename T>
@@ -416,9 +410,9 @@ static int laplacian_backward(const T* y, const int32_t* rowptr, const int32_t* 
                               T* grad_x, int32_t B, int32_t V, void* stream_) {
     if (!y || !rowptr || !col || !tcoef || !grad_loss || !grad_x || B <= 0 || V <= 0) return UMR_ERR_BAD_ARG;
     if (B > 65535) return UMR_ERR_TOO_LARGE;
-    count_launch();
-    k_laplacian_bwd<T><<<dim3((V + 255) / 256, B), 256, 0, (cudaStream_t)stream_>>>(y, rowptr, col, tcoef, grad_loss, grad_x, V);
-    UMR_RET();
+    launch(k_laplacian_bwd<T>, dim3((V + 255) / 256, B), 256, 0, (cudaStream_t)stream_, y, rowptr, col, tcoef, grad_loss,
+           grad_x, V);
+    return (int)cudaGetLastError();
 }
 extern "C" int umr_laplacian_backward(const float* y, const int32_t* rowptr, const int32_t* col, const float* tcoef,
                                       const float* grad_loss, float* grad_x, int32_t B, int32_t V, void* stream_) {
@@ -432,9 +426,9 @@ extern "C" int umr_flatten_forward(const float* vertices, const int32_t* edges, 
     cudaStream_t st = (cudaStream_t)stream_;
     cudaError_t e = cudaMemsetAsync(loss, 0, (size_t)B * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
-    count_launch();
-    k_flatten<float, false, false><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, loss, nullptr, nullptr, V, E, eps);
-    UMR_RET();
+    launch(k_flatten<float, false, false>, dim3((E + 127) / 128, B), 128, 0, st, vertices, edges, loss, nullptr, nullptr, V, E,
+           eps);
+    return (int)cudaGetLastError();
 }
 extern "C" int umr_flatten_backward(const float* vertices, const int32_t* edges, const float* grad_loss, float* grad_vertices,
                                     int32_t B, int32_t V, int32_t E, float eps, void* stream_) {
@@ -443,9 +437,9 @@ extern "C" int umr_flatten_backward(const float* vertices, const int32_t* edges,
     cudaStream_t st = (cudaStream_t)stream_;
     cudaError_t e = cudaMemsetAsync(grad_vertices, 0, (size_t)B * V * 3 * sizeof(float), st);
     if (e != cudaSuccess) return (int)e;
-    count_launch();
-    k_flatten<float, true, false><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, nullptr, grad_loss, grad_vertices, V, E, eps);
-    UMR_RET();
+    launch(k_flatten<float, true, false>, dim3((E + 127) / 128, B), 128, 0, st, vertices, edges, nullptr, grad_loss,
+           grad_vertices, V, E, eps);
+    return (int)cudaGetLastError();
 }
 
 extern "C" size_t umr_dt_barrier_workspace_bytes(int32_t B, int32_t H, int32_t W) {
@@ -459,10 +453,10 @@ extern "C" int umr_dt_barrier(const float* mask, float* dt, void* workspace, int
     cudaStream_t st = (cudaStream_t)stream_;
     int32_t* g_out = (int32_t*)workspace;
     int32_t* g_in = g_out + (size_t)B * H * W;
-    count_launch(2);
-    k_edt_columns<<<dim3((W + 255) / 256, B), 256, 0, st>>>(mask, g_out, g_in, H, W);
-    k_edt_rows<<<dim3(H, B), 256, (size_t)2 * W * sizeof(int32_t), st>>>(g_out, g_in, dt, H, W, k, 1.f / (float)std::max(H, W));
-    UMR_RET();
+    launch(k_edt_columns, dim3((W + 255) / 256, B), 256, 0, st, mask, g_out, g_in, H, W);
+    launch(k_edt_rows, dim3(H, B), 256, (size_t)2 * W * sizeof(int32_t), st, g_out, g_in, dt, H, W, k,
+           1.f / (float)std::max(H, W));
+    return (int)cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -483,10 +477,9 @@ static int laplacian_forward_slots(const T* x, const int32_t* rowptr, const int3
     cudaStream_t st = (cudaStream_t)stream_;
     const int gx = (V + 255) / 256;
     T* slots = (T*)workspace;
-    count_launch(2);
-    k_laplacian_fwd<T, true><<<dim3(gx, B), 256, 0, st>>>(x, rowptr, col, coef, y, slots, V);
-    k_sum_slot_rows<T><<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, gx);
-    UMR_RET();
+    launch(k_laplacian_fwd<T, true>, dim3(gx, B), 256, 0, st, x, rowptr, col, coef, y, slots, V);
+    launch(k_sum_slot_rows<T>, (B + 127) / 128, 128, 0, st, slots, loss, B, gx);
+    return (int)cudaGetLastError();
 }
 template <typename T>
 static size_t flatten_forward_workspace_bytes(int32_t B, int32_t E) {
@@ -501,10 +494,9 @@ static int flatten_forward_slots(const T* vertices, const int32_t* edges, T* los
     cudaStream_t st = (cudaStream_t)stream_;
     const int gx = (E + 127) / 128;
     T* slots = (T*)workspace;
-    count_launch(2);
-    k_flatten<T, false, true><<<dim3(gx, B), 128, 0, st>>>(vertices, edges, slots, nullptr, nullptr, V, E, eps);
-    k_sum_slot_rows<T><<<(B + 127) / 128, 128, 0, st>>>(slots, loss, B, gx);
-    UMR_RET();
+    launch(k_flatten<T, false, true>, dim3(gx, B), 128, 0, st, vertices, edges, slots, nullptr, nullptr, V, E, eps);
+    launch(k_sum_slot_rows<T>, (B + 127) / 128, 128, 0, st, slots, loss, B, gx);
+    return (int)cudaGetLastError();
 }
 template <typename T>
 static size_t flatten_backward_workspace_bytes(int32_t B, int32_t E) {
@@ -521,10 +513,11 @@ static int flatten_backward_gather(const T* vertices, const int32_t* edges, cons
     if (B > 65535) return UMR_ERR_TOO_LARGE;
     cudaStream_t st = (cudaStream_t)stream_;
     T* terms = (T*)workspace;
-    count_launch(2);
-    k_flatten<T, true, true><<<dim3((E + 127) / 128, B), 128, 0, st>>>(vertices, edges, nullptr, grad_loss, terms, V, E, eps);
-    k_gather3<T><<<dim3((V + 255) / 256, B), 256, 0, st>>>(terms, vert_rowptr, vert_incidence, grad_vertices, V, (int64_t)E * 4);
-    UMR_RET();
+    launch(k_flatten<T, true, true>, dim3((E + 127) / 128, B), 128, 0, st, vertices, edges, nullptr, grad_loss, terms, V, E,
+           eps);
+    launch(k_gather3<T>, dim3((V + 255) / 256, B), 256, 0, st, terms, vert_rowptr, vert_incidence, grad_vertices, V,
+           (int64_t)E * 4);
+    return (int)cudaGetLastError();
 }
 
 extern "C" size_t umr_laplacian_workspace_bytes_deterministic(int32_t B, int32_t V) { return laplacian_workspace_bytes<float>(B, V); }

@@ -1033,16 +1033,47 @@ static Consts make_consts(const UmrNmrParams* p) {
     return K;
 }
 
-static void launch_prep(const float* vertices, const int32_t* faces, float* rec, int4* box, const Consts& K,
-                        cudaStream_t stream) {
-    k_nmr_prep<<<dim3((K.Fc + 127) / 128, K.B), 128, 0, stream>>>(vertices, faces, rec, box, K);
-    count_launch();
+// the record and box arrays at the start of every NMR workspace (umr_nmr_workspace_bytes), filled by k_nmr_prep
+struct Prepared {
+    float* rec;
+    int4* box;
+};
+static Prepared prep(const float* vertices, const int32_t* faces, void* workspace, const Consts& K, cudaStream_t stream) {
+    const Prepared w{(float*)workspace, (int4*)((char*)workspace + rec_bytes(K.B, K.Fc))};
+    launch(k_nmr_prep, dim3((K.Fc + 127) / 128, K.B), 128, 0, stream, vertices, faces, w.rec, w.box, K);
+    return w;
+}
+
+// the default and deterministic texture gradients: the same arguments and workspace, k_nmr_bwd_tex_det in place of
+// k_nmr_bwd_tex
+static int backward_textures(const float* vertices, const int32_t* faces, const int32_t* face_index, const float* grad_rgb,
+                             float* grad_textures, const UmrNmrParams* p, void* workspace, void* stream_, bool det) {
+    int rc = check(p, true);
+    if (rc) return rc;
+    if (!vertices || !faces || !face_index || !grad_rgb || !grad_textures || !workspace) return UMR_ERR_BAD_ARG;
+    if (((uintptr_t)workspace & 255) != 0 || ((uintptr_t)grad_textures & 3) != 0) return UMR_ERR_BAD_ARG;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const Consts K = make_consts(p);
+    const size_t gbytes = (size_t)(K.B / K.tex_div) * K.F * K.T * K.T * K.T * 3 * sizeof(float);
+    cudaError_t e = cudaMemsetAsync(grad_textures, 0, gbytes, stream);
+    if (e != cudaSuccess) return (int)e;
+    const Prepared w = prep(vertices, faces, workspace, K, stream);
+    if (det) {
+        const long long nwarp = (long long)(K.B / K.tex_div) * K.F;
+        launch(k_nmr_bwd_tex_det, (unsigned)((nwarp + DET_WARPS - 1) / DET_WARPS), DET_WARPS * 32, 0, stream, w.rec, w.box,
+               face_index, grad_rgb, grad_textures, K);
+    } else {
+        const size_t nthr = (size_t)K.B * K.IS * K.IS;
+        launch(k_nmr_bwd_tex, (unsigned)((nthr + 255) / 256), 256, 0, stream, w.rec, face_index, grad_rgb, grad_textures, K);
+    }
+    return (int)cudaGetLastError();
 }
 
 }  // namespace nmr
 }  // namespace umr
 
 using namespace umr::nmr;
+using umr::launch;
 
 extern "C" size_t umr_nmr_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t fill_back) {
     // 0 for the shapes check() refuses, like B <= 0
@@ -1064,20 +1095,14 @@ extern "C" int umr_nmr_forward(const float* vertices, const int32_t* faces, cons
     if (((uintptr_t)workspace & 255) != 0) return UMR_ERR_BAD_ARG;
     cudaStream_t stream = (cudaStream_t)stream_;
     const Consts K = make_consts(p);
-    char* ws = (char*)workspace;
-    float* rec = (float*)ws;
-    int4* box = (int4*)(ws + rec_bytes(K.B, K.Fc));
-    launch_prep(vertices, faces, rec, box, K, stream);
+    const Prepared w = prep(vertices, faces, workspace, K, stream);
     const int nb = (K.S + BIN - 1) / BIN;
-    k_nmr_zbuf<<<dim3(nb, nb, K.B), CTA, 0, stream>>>(rec, box, face_index, raster_depth, K);
-    umr::count_launch();
+    launch(k_nmr_zbuf, dim3(nb, nb, K.B), CTA, 0, stream, w.rec, w.box, face_index, raster_depth, K);
     if (rgb || alpha || depth) {
         const bool vec = (K.IS % 4) == 0 && (((uintptr_t)rgb | (uintptr_t)alpha | (uintptr_t)depth) & 15) == 0;
         const size_t nthr = (size_t)K.B * K.IS * (vec ? K.IS / 4 : K.IS);
-        const unsigned grid = (unsigned)((nthr + 255) / 256);
-        if (vec) k_nmr_shade<4><<<grid, 256, 0, stream>>>(rec, face_index, raster_depth, textures, rgb, alpha, depth, K);
-        else k_nmr_shade<1><<<grid, 256, 0, stream>>>(rec, face_index, raster_depth, textures, rgb, alpha, depth, K);
-        umr::count_launch();
+        launch(vec ? k_nmr_shade<4> : k_nmr_shade<1>, (unsigned)((nthr + 255) / 256), 256, 0, stream, w.rec, face_index,
+               raster_depth, textures, rgb, alpha, depth, K);
     }
     return (int)cudaGetLastError();
 }
@@ -1085,48 +1110,14 @@ extern "C" int umr_nmr_forward(const float* vertices, const int32_t* faces, cons
 extern "C" int umr_nmr_backward_textures(const float* vertices, const int32_t* faces, const int32_t* face_index,
                                          const float* grad_rgb, float* grad_textures, const UmrNmrParams* p,
                                          void* workspace, void* stream_) {
-    int rc = check(p, true);
-    if (rc) return rc;
-    if (!vertices || !faces || !face_index || !grad_rgb || !grad_textures || !workspace) return UMR_ERR_BAD_ARG;
-    if (((uintptr_t)workspace & 255) != 0 || ((uintptr_t)grad_textures & 3) != 0) return UMR_ERR_BAD_ARG;
-    cudaStream_t stream = (cudaStream_t)stream_;
-    const Consts K = make_consts(p);
-    const size_t gbytes = (size_t)(K.B / K.tex_div) * K.F * K.T * K.T * K.T * 3 * sizeof(float);
-    cudaError_t e = cudaMemsetAsync(grad_textures, 0, gbytes, stream);
-    if (e != cudaSuccess) return (int)e;
-    char* ws = (char*)workspace;
-    float* rec = (float*)ws;
-    int4* box = (int4*)(ws + rec_bytes(K.B, K.Fc));
-    launch_prep(vertices, faces, rec, box, K, stream);
-    const size_t nthr = (size_t)K.B * K.IS * K.IS;
-    k_nmr_bwd_tex<<<(unsigned)((nthr + 255) / 256), 256, 0, stream>>>(rec, face_index, grad_rgb, grad_textures, K);
-    umr::count_launch();
-    return (int)cudaGetLastError();
+    return backward_textures(vertices, faces, face_index, grad_rgb, grad_textures, p, workspace, stream_, false);
 }
 
-// Deterministic texture gradient (include/umr_b200.h): the default call's arguments and workspace; k_nmr_bwd_tex_det in
-// place of k_nmr_bwd_tex.
+// Deterministic texture gradient (include/umr_b200.h)
 extern "C" int umr_nmr_backward_textures_deterministic(const float* vertices, const int32_t* faces, const int32_t* face_index,
                                                        const float* grad_rgb, float* grad_textures, const UmrNmrParams* p,
                                                        void* workspace, void* stream_) {
-    int rc = check(p, true);
-    if (rc) return rc;
-    if (!vertices || !faces || !face_index || !grad_rgb || !grad_textures || !workspace) return UMR_ERR_BAD_ARG;
-    if (((uintptr_t)workspace & 255) != 0 || ((uintptr_t)grad_textures & 3) != 0) return UMR_ERR_BAD_ARG;
-    cudaStream_t stream = (cudaStream_t)stream_;
-    const Consts K = make_consts(p);
-    const size_t gbytes = (size_t)(K.B / K.tex_div) * K.F * K.T * K.T * K.T * 3 * sizeof(float);
-    cudaError_t e = cudaMemsetAsync(grad_textures, 0, gbytes, stream);
-    if (e != cudaSuccess) return (int)e;
-    char* ws = (char*)workspace;
-    float* rec = (float*)ws;
-    int4* box = (int4*)(ws + rec_bytes(K.B, K.Fc));
-    launch_prep(vertices, faces, rec, box, K, stream);
-    const long long nwarp = (long long)(K.B / K.tex_div) * K.F;
-    k_nmr_bwd_tex_det<<<(unsigned)((nwarp + DET_WARPS - 1) / DET_WARPS), DET_WARPS * 32, 0, stream>>>(rec, box, face_index,
-                                                                                                      grad_rgb, grad_textures, K);
-    umr::count_launch();
-    return (int)cudaGetLastError();
+    return backward_textures(vertices, faces, face_index, grad_rgb, grad_textures, p, workspace, stream_, true);
 }
 
 // Geometry gradient (include/umr_b200.h, DESIGN.md §14).  Workspace: the forward's record and box arrays, then the
@@ -1154,20 +1145,15 @@ extern "C" int umr_nmr_backward_faces(const float* vertices, const int32_t* face
     if (p->fill_back || p->light_intensity_directional != 0.f) return UMR_ERR_UNSUPPORTED;
     cudaStream_t stream = (cudaStream_t)stream_;
     const Consts K = make_consts(p);
-    char* ws = (char*)workspace;
-    float* rec = (float*)ws;
-    int4* box = (int4*)(ws + rec_bytes(K.B, K.Fc));
-    float* color = (float*)(ws + rec_bytes(K.B, K.Fc) + box_bytes(K.B, K.Fc));
-    launch_prep(vertices, faces, rec, box, K, stream);
+    float* color = (float*)((char*)workspace + rec_bytes(K.B, K.Fc) + box_bytes(K.B, K.Fc));
+    const Prepared w = prep(vertices, faces, workspace, K, stream);
     if (grad_rgb) {
         const size_t n = (size_t)K.B * K.S * K.S;
-        k_nmr_shade_raster<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(rec, face_index, textures, color, K);
-        umr::count_launch();
+        launch(k_nmr_shade_raster, (unsigned)((n + 255) / 256), 256, 0, stream, w.rec, face_index, textures, color, K);
     }
     GradPlanes G{grad_rgb, grad_alpha, grad_depth, color, face_index};
     const long long nthr = (long long)K.B * K.F * 32;
-    k_nmr_grad_faces<<<(unsigned)((nthr + 255) / 256), 256, 0, stream>>>(rec, box, G, grad_face_vertices, eps, K);
-    umr::count_launch();
+    launch(k_nmr_grad_faces, (unsigned)((nthr + 255) / 256), 256, 0, stream, w.rec, w.box, G, grad_face_vertices, eps, K);
     return (int)cudaGetLastError();
 }
 
@@ -1215,9 +1201,8 @@ static LightArgs<T> light_args(const void* faces, const void* textures, const vo
 template <typename T>
 static int light_forward(const LightArgs<T>& A, T* out, cudaStream_t stream) {
     const unsigned grid = (unsigned)((A.N + lt_elems<T>() - 1) / lt_elems<T>());
-    if (aligned(A.tex, 16) && aligned(out, 16)) k_nmr_light_fwd<T, true><<<grid, LT_CTA, 0, stream>>>(A, out);
-    else k_nmr_light_fwd<T, false><<<grid, LT_CTA, 0, stream>>>(A, out);
-    umr::count_launch();
+    launch(aligned(A.tex, 16) && aligned(out, 16) ? k_nmr_light_fwd<T, true> : k_nmr_light_fwd<T, false>, grid, LT_CTA, 0,
+           stream, A, out);
     return (int)cudaGetLastError();
 }
 
@@ -1225,13 +1210,11 @@ template <typename T>
 static int light_backward(const LightArgs<T>& A, int B, const T* g, T* grad_faces, T* grad_tex, T* grad_light, T* part,
                           cudaStream_t stream) {
     const long long nface = (long long)B * A.F;
-    k_nmr_light_bwd<T><<<(unsigned)((nface * 32 + 255) / 256), 256, 0, stream>>>(A, nface, g, grad_tex, grad_faces,
-                                                                                  grad_light ? part : nullptr);
-    umr::count_launch();
-    if (grad_light) {
-        k_nmr_light_reduce<T><<<(unsigned)(((long long)B * 9 * 32 + 127) / 128), 128, 0, stream>>>(part, grad_light, B, A.F);
-        umr::count_launch();
-    }
+    launch(k_nmr_light_bwd<T>, (unsigned)((nface * 32 + 255) / 256), 256, 0, stream, A, nface, g, grad_tex, grad_faces,
+           grad_light ? part : nullptr);
+    if (grad_light)
+        launch(k_nmr_light_reduce<T>, (unsigned)(((long long)B * 9 * 32 + 127) / 128), 128, 0, stream, part, grad_light, B,
+               A.F);
     return (int)cudaGetLastError();
 }
 

@@ -1,26 +1,17 @@
-// raster_host.cuh -- host side shared by the rasteriser's C entry points (raster.cu, raster_f64.cu): the parameter checks,
-// the kernel constants and the counted kernel launch.
+// raster_host.cuh -- host side shared by the rasteriser's C entry points (raster.cu, raster_f64.cu): the parameter checks
+// and the kernel constants.  Kernels are launched through launch() (common.cuh).
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
 
 #include <type_traits>
-#include <utility>
 
 #include "common.cuh"
 #include "raster_generic.cuh"
 #include "umr_b200.h"
 
 namespace umr {
-
-// kernel<<<grid, block, smem, stream>>>(args...), counted in umr_launch_count().  Every raster kernel is launched here, so
-// the count is one per kernel launch by construction; memsets and event records are not counted.
-template <typename... P, typename... A>
-inline void launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, A&&... args) {
-    kernel<<<grid, block, smem, stream>>>(std::forward<A>(args)...);
-    count_launch();
-}
 
 // one of the profiling events of UmrRasterParams (NULL: off)
 inline void record(void* event, cudaStream_t stream) {

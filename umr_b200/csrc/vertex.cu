@@ -510,13 +510,10 @@ extern "C" int umr_project_faces_forward(const float* vertices, const float* cam
     if (!vertices || !cams || !faces || !face_vertices || !p) return UMR_ERR_BAD_ARG;
     if (p->batch_size <= 0 || p->num_vertices <= 0 || p->num_faces <= 0) return UMR_ERR_BAD_ARG;
     if (p->batch_size > 65535) return UMR_ERR_TOO_LARGE;
-    cudaStream_t st = (cudaStream_t)stream_;
-    const dim3 grid((p->num_faces + 255) / 256, p->batch_size);
-    count_launch();
     const int H = p->num_hypotheses > 1 ? p->num_hypotheses : 1;
     if (p->batch_size % H != 0) return UMR_ERR_BAD_ARG;
-    k_project_faces<<<grid, 256, 0, st>>>(vertices, cams, faces, face_vertices, light, p->num_vertices, p->num_faces, H,
-                                          p->faces_batch_stride, make_pc(p), make_lc(p));
+    launch(k_project_faces, dim3((p->num_faces + 255) / 256, p->batch_size), 256, 0, (cudaStream_t)stream_, vertices, cams,
+           faces, face_vertices, light, p->num_vertices, p->num_faces, H, p->faces_batch_stride, make_pc(p), make_lc(p));
     return (int)cudaGetLastError();
 }
 
@@ -539,12 +536,10 @@ extern "C" int umr_project_faces_backward(const float* vertices, const float* ca
         e = cudaMemsetAsync(grad_cams, 0, (size_t)B * 7 * sizeof(float), st);
         if (e != cudaSuccess) return (int)e;
     }
-    count_launch(2);
-    k_scatter_face_grads<false><<<dim3((F + 255) / 256, B), 256, 0, st>>>(vertices, cams, faces, grad_face_vertices,
-                                                                          grad_light, grad_proj, V, F, H,
-                                                                          p->faces_batch_stride, make_pc(p), make_lc(p));
-    k_project_backward<false><<<dim3((V + 255) / 256, B), 256, 0, st>>>(vertices, cams, grad_proj, grad_vertices, grad_cams,
-                                                                        V, H, make_pc(p));
+    launch(k_scatter_face_grads<false>, dim3((F + 255) / 256, B), 256, 0, st, vertices, cams, faces, grad_face_vertices,
+           grad_light, grad_proj, V, F, H, p->faces_batch_stride, make_pc(p), make_lc(p));
+    launch(k_project_backward<false>, dim3((V + 255) / 256, B), 256, 0, st, vertices, cams, grad_proj, grad_vertices, grad_cams,
+           V, H, make_pc(p));
     return (int)cudaGetLastError();
 }
 
@@ -574,16 +569,14 @@ extern "C" int umr_project_faces_backward_deterministic(const float* vertices, c
     float* vterms = terms + (size_t)B * F * 9;
     float* slots = vterms + (size_t)B * V * 3;
     float* gv = (grad_vertices && H > 1) ? vterms : grad_vertices;
-    count_launch(3 + (grad_vertices && H > 1 ? 1 : 0) + (grad_cams ? 1 : 0));
-    k_scatter_face_grads<true><<<dim3((F + 255) / 256, B), 256, 0, st>>>(vertices, cams, faces, grad_face_vertices, grad_light,
-                                                                         terms, V, F, H, p->faces_batch_stride, make_pc(p),
-                                                                         make_lc(p));
-    k_vertex_gather<<<dim3(nslot, B), 256, 0, st>>>(terms, vert_rowptr, vert_incidence, grad_proj, V, F, H,
-                                                    p->faces_batch_stride != 0 ? 1 : 0);
-    k_project_backward<true><<<dim3(nslot, B), 256, 0, st>>>(vertices, cams, grad_proj, gv, grad_cams ? slots : nullptr, V, H,
-                                                             make_pc(p));
-    if (grad_vertices && H > 1) k_hypothesis_sum<<<dim3(nslot, B / H), 256, 0, st>>>(vterms, grad_vertices, V, H);
-    if (grad_cams) k_cam_finalize<<<(B * 7 + 255) / 256, 256, 0, st>>>(slots, grad_cams, B, (int)nslot);
+    launch(k_scatter_face_grads<true>, dim3((F + 255) / 256, B), 256, 0, st, vertices, cams, faces, grad_face_vertices,
+           grad_light, terms, V, F, H, p->faces_batch_stride, make_pc(p), make_lc(p));
+    launch(k_vertex_gather, dim3(nslot, B), 256, 0, st, terms, vert_rowptr, vert_incidence, grad_proj, V, F, H,
+           p->faces_batch_stride != 0 ? 1 : 0);
+    launch(k_project_backward<true>, dim3(nslot, B), 256, 0, st, vertices, cams, grad_proj, gv, grad_cams ? slots : nullptr, V,
+           H, make_pc(p));
+    if (grad_vertices && H > 1) launch(k_hypothesis_sum, dim3(nslot, B / H), 256, 0, st, vterms, grad_vertices, V, H);
+    if (grad_cams) launch(k_cam_finalize, (B * 7 + 255) / 256, 256, 0, st, slots, grad_cams, B, (int)nslot);
     return (int)cudaGetLastError();
 }
 
@@ -610,9 +603,8 @@ static int corr_chamfer_forward(const T* vertices, int64_t vertices_batch_stride
     CorrCfg<T> c;
     const int rc = make_corr_cfg(c, targets, target_counts, part_ends, weights, NS);
     if (rc) return rc;
-    count_launch();
-    k_corr_fwd<T><<<B, 256, 0, (cudaStream_t)stream_>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest,
-                                                        loss, NS);
+    launch(k_corr_fwd<T>, B, 256, 0, (cudaStream_t)stream_, vertices, vertices_batch_stride, cams, selection, c, vert2d,
+           nearest, loss, NS);
     return (int)cudaGetLastError();
 }
 
@@ -640,9 +632,8 @@ extern "C" int umr_corr_chamfer_backward(const float* vertices, int64_t vertices
         cudaError_t e = cudaMemsetAsync(grad_vertices, 0, (size_t)B * V * 3 * sizeof(float), st);
         if (e != cudaSuccess) return (int)e;
     }
-    count_launch();
-    k_corr_bwd<float, false><<<B, 256, 0, st>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss,
-                                                grad_vert2d, grad_vertices, grad_cams, NS, V);
+    launch(k_corr_bwd<float, false>, B, 256, 0, st, vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest,
+           grad_loss, grad_vert2d, grad_vertices, grad_cams, NS, V);
     return (int)cudaGetLastError();
 }
 
@@ -670,11 +661,11 @@ static int corr_chamfer_backward_gather(const T* vertices, int64_t vertices_batc
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream_;
     T* terms = grad_vertices ? (T*)workspace : nullptr;
-    count_launch(grad_vertices ? 2 : 1);
-    k_corr_bwd<T, true><<<B, 256, 0, st>>>(vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss,
-                                           grad_vert2d, terms, grad_cams, NS, V);
+    launch(k_corr_bwd<T, true>, B, 256, 0, st, vertices, vertices_batch_stride, cams, selection, c, vert2d, nearest, grad_loss,
+           grad_vert2d, terms, grad_cams, NS, V);
     if (grad_vertices)
-        k_gather3<T><<<dim3((V + 255) / 256, B), 256, 0, st>>>(terms, vert_rowptr, vert_selection, grad_vertices, V, (int64_t)NS);
+        launch(k_gather3<T>, dim3((V + 255) / 256, B), 256, 0, st, terms, vert_rowptr, vert_selection, grad_vertices, V,
+               (int64_t)NS);
     return (int)cudaGetLastError();
 }
 

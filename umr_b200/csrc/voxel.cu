@@ -250,23 +250,21 @@ extern "C" int umr_voxelize(const void* faces, int32_t dtype, int32_t* voxels, i
     if (e != cudaSuccess) return (int)e;
     const int64_t nf = (int64_t)B * F;
     if (nf > 0) {
-        count_launch();
         const unsigned blocks = (unsigned)((nf + VOX_SURF_WARPS - 1) / VOX_SURF_WARPS);
         if (dtype == UMR_DTYPE_FLOAT32)
-            k_vox_surface<float><<<blocks, VOX_SURF_WARPS * 32, 0, st>>>((const float*)faces, occ, nf, F, vs, W, (float)scale);
+            launch(k_vox_surface<float>, blocks, VOX_SURF_WARPS * 32, 0, st, (const float*)faces, occ, nf, F, vs, W, (float)scale);
         else
-            k_vox_surface<double><<<blocks, VOX_SURF_WARPS * 32, 0, st>>>((const double*)faces, occ, nf, F, vs, W, scale);
+            launch(k_vox_surface<double>, blocks, VOX_SURF_WARPS * 32, 0, st, (const double*)faces, occ, nf, F, vs, W, scale);
     }
-    count_launch(2);
     if (vs <= VOX_SMEM_MAX_VS) {
         const size_t smem = 2 * (size_t)vs * vs * W * sizeof(uint32_t);
         e = cudaFuncSetAttribute(k_vox_fill<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return (int)e;
-        k_vox_fill<true><<<B, VOX_FILL_THREADS, smem, st>>>(occ, vis, status, vs, W);
+        launch(k_vox_fill<true>, B, VOX_FILL_THREADS, smem, st, occ, vis, status, vs, W);
     } else {
-        k_vox_fill<false><<<B, VOX_FILL_THREADS, 0, st>>>(occ, vis, status, vs, W);
+        launch(k_vox_fill<false>, B, VOX_FILL_THREADS, 0, st, occ, vis, status, vs, W);
     }
     const int64_t n = (int64_t)B * vs * vs * ((vs + 3) / 4);
-    k_vox_unpack<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(vis, voxels, (int64_t)B * vs * vs, vs, W);
+    launch(k_vox_unpack, (unsigned)((n + 255) / 256), 256, 0, st, vis, voxels, (int64_t)B * vs * vs, vs, W);
     return (int)cudaGetLastError();
 }
