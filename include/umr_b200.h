@@ -733,4 +733,8 @@ int umr_part_head_backward(const void* const* maps, const int64_t* map_bstrides,
 #ifdef __cplusplus
 }
 #endif
+
+/* keypoint transfer of the keypoint evaluation (umr_kp_transfer_flow / _cam) */
+#include "umr_kp_transfer.h"
+
 #endif /* UMR_B200_H_ */

@@ -252,6 +252,15 @@ EXPORTS = {
                                [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
 }
 
+# Keypoint transfer of the keypoint evaluation (include/umr_kp_transfer.h), bound by load() like EXPORTS.  A table of its
+# own, as the header is: EXPORTS lists umr_b200.h's own declarations.
+KP_EXPORTS = {
+    # kps, flow_src, flow_tgt, gauss, grid, out, P, K, F, T2, S, sigma, stream
+    "umr_kp_transfer_flow": (ctypes.c_int, [c_f32p] * 6 + [ctypes.c_int32] * 6 + [ctypes.c_void_p]),
+    # kps, proj_src, proj_tgt, mask_tgt, grid, out, P, K, V, S, stream
+    "umr_kp_transfer_cam": (ctypes.c_int, [c_f32p] * 6 + [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
+}
+
 _lock = threading.Lock()
 _lib = None
 
@@ -272,7 +281,7 @@ def load():
                     "libumr_b200.so is not built (%s). Run `python -m umr_b200.build` "
                     "(or __graft_entry__.build()). There is no CPU fallback." % LIB_PATH)
             lib = ctypes.CDLL(LIB_PATH)
-            for name, (res, args) in EXPORTS.items():
+            for name, (res, args) in list(EXPORTS.items()) + list(KP_EXPORTS.items()):
                 fn = getattr(lib, name)  # AttributeError if the symbol is missing
                 fn.restype = res
                 fn.argtypes = args

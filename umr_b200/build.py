@@ -22,7 +22,8 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-I", os.path
 # raster.cu must not contract a*b+c into FMA: its per-(pixel,face) arithmetic is an exact IEEE twin
 # of the reference (DESIGN.md §4).  The loss kernels have no such constraint.
 PER_FILE = {"raster.cu": ["-fmad=false"], "raster_f64.cu": ["-fmad=false"], "losses_f64.cu": ["-fmad=false"],
-            "vertex.cu": ["-fmad=false"], "mesh_ops.cu": ["-fmad=false"], "nmr.cu": ["-fmad=false"], "voxel.cu": ["-fmad=false"]}
+            "vertex.cu": ["-fmad=false"], "mesh_ops.cu": ["-fmad=false"], "nmr.cu": ["-fmad=false"], "voxel.cu": ["-fmad=false"],
+            "kp_transfer.cu": ["-fmad=false"]}
 
 
 def sources():
@@ -40,7 +41,7 @@ def build(force=False, verbose=False):
     nvcc = os.environ.get("NVCC", "nvcc")
     os.makedirs(OBJ, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    headers.append(os.path.join(ROOT, "include", "umr_b200.h"))
+    headers += [os.path.join(ROOT, "include", f) for f in os.listdir(os.path.join(ROOT, "include")) if f.endswith(".h")]
     objs = []
     for src in sources():
         s = os.path.join(CSRC, src)

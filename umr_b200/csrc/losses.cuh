@@ -26,31 +26,58 @@ namespace umr {
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool inb(int x, int y, int W, int H) { return x >= 0 && x < W && y >= 0 && y < H; }
 
+// One sample's bilinear tap: its top-left corner (x0, y0), the weights of the corners nw = (x0, y0), ne = (x0+1, y0),
+// sw = (x0, y0+1), se = (x0+1, y0+1), and which of them lie in the H x W image.  Shared with kp_transfer.cu, which
+// samples its keypoint heat maps and the identity grid in exactly this arithmetic.
+template <typename T>
+struct BilinearTap {
+    int x0, y0;
+    T nw, ne, sw, se;
+    bool v00, v10, v01, v11;
+};
+template <typename T>
+__device__ __forceinline__ BilinearTap<T> bilinear_tap(vec2_t<T> xy, int H, int W) {
+    BilinearTap<T> t;
+    const T ix = ((xy.x + T(1)) / T(2)) * (T)(W - 1);
+    const T iy = ((xy.y + T(1)) / T(2)) * (T)(H - 1);
+    const T fx = floor(ix), fy = floor(iy);
+    t.x0 = (int)fx;
+    t.y0 = (int)fy;
+    const int x1 = t.x0 + 1, y1 = t.y0 + 1;
+    t.nw = ((T)x1 - ix) * ((T)y1 - iy);
+    t.ne = (ix - (T)t.x0) * ((T)y1 - iy);
+    t.sw = ((T)x1 - ix) * (iy - (T)t.y0);
+    t.se = (ix - (T)t.x0) * (iy - (T)t.y0);
+    t.v00 = inb(t.x0, t.y0, W, H);
+    t.v10 = inb(x1, t.y0, W, H);
+    t.v01 = inb(t.x0, y1, W, H);
+    t.v11 = inb(x1, y1, W, H);
+    return t;
+}
+// The sampled value: pixel(x, y) times its weight, summed over the in-image corners in the order nw, ne, sw, se
+template <typename T, typename Pixel>
+__device__ __forceinline__ T bilinear_value(const BilinearTap<T>& t, Pixel pixel) {
+    T acc = 0;
+    if (t.v00) acc += pixel(t.x0, t.y0) * t.nw;
+    if (t.v10) acc += pixel(t.x0 + 1, t.y0) * t.ne;
+    if (t.v01) acc += pixel(t.x0, t.y0 + 1) * t.sw;
+    if (t.v11) acc += pixel(t.x0 + 1, t.y0 + 1) * t.se;
+    return acc;
+}
+
 template <typename T, int C>
 __global__ void __launch_bounds__(256) k_sample_fwd(const T* __restrict__ image, const vec2_t<T>* __restrict__ flow,
                                                     T* __restrict__ out, int H, int W, int N) {
     const int n = blockIdx.x * blockDim.x + threadIdx.x;
     const int b = blockIdx.y;
     if (n >= N) return;
-    const vec2_t<T> xy = __ldg(flow + (size_t)b * N + n);
-    const T ix = ((xy.x + T(1)) / T(2)) * (T)(W - 1);
-    const T iy = ((xy.y + T(1)) / T(2)) * (T)(H - 1);
-    const T fx = floor(ix), fy = floor(iy);
-    const int x0 = (int)fx, y0 = (int)fy, x1 = x0 + 1, y1 = y0 + 1;
-    const T nw = ((T)x1 - ix) * ((T)y1 - iy), ne = (ix - (T)x0) * ((T)y1 - iy);
-    const T sw = ((T)x1 - ix) * (iy - (T)y0), se = (ix - (T)x0) * (iy - (T)y0);
-    const bool v00 = inb(x0, y0, W, H), v10 = inb(x1, y0, W, H), v01 = inb(x0, y1, W, H), v11 = inb(x1, y1, W, H);
+    const BilinearTap<T> tap = bilinear_tap<T>(__ldg(flow + (size_t)b * N + n), H, W);
     const T* img = image + (size_t)b * C * H * W;
     T* o = out + ((size_t)b * N + n) * C;
 #pragma unroll
     for (int c = 0; c < C; ++c) {
         const T* p = img + (size_t)c * H * W;
-        T acc = 0;
-        if (v00) acc += __ldg(p + (size_t)y0 * W + x0) * nw;
-        if (v10) acc += __ldg(p + (size_t)y0 * W + x1) * ne;
-        if (v01) acc += __ldg(p + (size_t)y1 * W + x0) * sw;
-        if (v11) acc += __ldg(p + (size_t)y1 * W + x1) * se;
-        o[c] = acc;
+        o[c] = bilinear_value(tap, [&](int x, int y) { return __ldg(p + (size_t)y * W + x); });
     }
 }
 
@@ -243,6 +270,40 @@ __global__ void __launch_bounds__(256) k_iou_bwd(const T* __restrict__ t, const 
 // chamfer: one warp per query point, lanes stride over the key set; lexicographic (value, index)
 // minimum => lowest index wins ties, like torch.min.
 // ---------------------------------------------------------------------------------------------
+// Defined operation order (never contracted to FMA, whatever the compile flags):
+//   |p|^2 = ((p0*p0 + p1*p1) + p2*p2),  a.b = ((a0*b0 + a1*b1) + a2*b2),  P = (|q|^2 + |k|^2) - 2*(q.k)
+// -- chamfer_python.py:58-63 with every product and sum rounded once.  oracle/losses.py::dist_chamfer_np
+// restates exactly this sequence, so distances AND argmins are bit-exact against it.  kp_transfer.cu's nearest-vertex
+// and nearest-pixel searches use the same distance and the same warp minimum.
+template <typename T, int D>
+__device__ __forceinline__ T chamfer_sqnorm(const T (&v)[D]) {
+    T s = mul_rn(v[0], v[0]);
+#pragma unroll
+    for (int d = 1; d < D; ++d) s = add_rn(s, mul_rn(v[d], v[d]));
+    return s;
+}
+// P between a query qv (|q|^2 = qq) and a key kv
+template <typename T, int D>
+__device__ __forceinline__ T chamfer_dist(const T (&qv)[D], T qq, const T (&kv)[D]) {
+    T kk = mul_rn(kv[0], kv[0]), zz = mul_rn(qv[0], kv[0]);
+#pragma unroll
+    for (int d = 1; d < D; ++d) {
+        kk = add_rn(kk, mul_rn(kv[d], kv[d]));
+        zz = add_rn(zz, mul_rn(qv[d], kv[d]));
+    }
+    return sub_rn(add_rn(qq, kk), mul_rn(T(2), zz));  // chamfer_python.py:63 expanded form
+}
+// every lane of the warp ends with the lexicographic (value, index) minimum of the lanes' (best, bi)
+template <typename T>
+__device__ __forceinline__ void warp_argmin(T& best, int& bi) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const T ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+    }
+}
+
 template <typename T, int D>
 __global__ void __launch_bounds__(256) k_chamfer_nn(const T* __restrict__ q, const T* __restrict__ k,
                                                     T* __restrict__ dist, int32_t* __restrict__ idx, int NQ, int NK) {
@@ -251,16 +312,10 @@ __global__ void __launch_bounds__(256) k_chamfer_nn(const T* __restrict__ q, con
     const int b = blockIdx.y;
     if (qi >= NQ) return;
     const T* qp = q + ((size_t)b * NQ + qi) * D;
-    // Defined operation order (never contracted to FMA, whatever the compile flags):
-    //   |p|^2 = ((p0*p0 + p1*p1) + p2*p2),  a.b = ((a0*b0 + a1*b1) + a2*b2),  P = (|q|^2 + |k|^2) - 2*(q.k)
-    // -- chamfer_python.py:58-63 with every product and sum rounded once.  oracle/losses.py::dist_chamfer_np
-    // restates exactly this sequence, so distances AND argmins are bit-exact against it.
     T qv[D];
 #pragma unroll
     for (int d = 0; d < D; ++d) { qv[d] = __ldg(qp + d); }
-    T qq = mul_rn(qv[0], qv[0]);
-#pragma unroll
-    for (int d = 1; d < D; ++d) qq = add_rn(qq, mul_rn(qv[d], qv[d]));
+    const T qq = chamfer_sqnorm(qv);
     T best = (T)INFINITY;
     int bi = 0x7fffffff;
     const T* kb = k + (size_t)b * NK * D;
@@ -268,21 +323,10 @@ __global__ void __launch_bounds__(256) k_chamfer_nn(const T* __restrict__ q, con
         T kv[D];
 #pragma unroll
         for (int d = 0; d < D; ++d) kv[d] = __ldg(kb + (size_t)j * D + d);
-        T kk = mul_rn(kv[0], kv[0]), zz = mul_rn(qv[0], kv[0]);
-#pragma unroll
-        for (int d = 1; d < D; ++d) {
-            kk = add_rn(kk, mul_rn(kv[d], kv[d]));
-            zz = add_rn(zz, mul_rn(qv[d], kv[d]));
-        }
-        const T P = sub_rn(add_rn(qq, kk), mul_rn(T(2), zz));  // chamfer_python.py:63 expanded form
+        const T P = chamfer_dist(qv, qq, kv);
         if (P < best) { best = P; bi = j; }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const T ob = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-    }
+    warp_argmin(best, bi);
     if (lane == 0) {
         dist[(size_t)b * NQ + qi] = best;
         idx[(size_t)b * NQ + qi] = bi;

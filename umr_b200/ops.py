@@ -90,9 +90,21 @@ def _pairs(t):
 # -------------------------------------------------------------------------------------------------
 # bilinear texture-flow sampler
 # -------------------------------------------------------------------------------------------------
+SAMPLE_MAX_CHANNELS = 4   # channels one sampler kernel call takes; wider images are sampled in groups of this many
+
+
+def _channel_groups(C):
+    """[(first channel, count)] of the sampler calls for C channels: one call for C <= 4, else groups of at most 4."""
+    return [(c, min(SAMPLE_MAX_CHANNELS, C - c)) for c in range(0, C, SAMPLE_MAX_CHANNELS)]
+
+
 class BilinearSampleFunction(torch.autograd.Function):
     """images [B,C,H,W], flow [B,N,2] -> out [B,N,C]; bilinear, zeros padding, align_corners=True
-    (the torch-1.1 semantics the reference was written for: geom_utils.py:55, loss_utils.py:64)."""
+    (the torch-1.1 semantics the reference was written for: geom_utils.py:55, loss_utils.py:64).
+
+    The kernels take at most 4 channels.  A wider image (SCOPS's 5 part probabilities in avg_uv.py, K keypoint heat maps)
+    runs them on channel groups of at most 4: the forward concatenates the groups' outputs, each group gets its own image
+    gradient, and the flow gradient is the groups' flow gradients summed in ascending group order."""
 
     @staticmethod
     def forward(ctx, images, flow):
@@ -101,14 +113,19 @@ class BilinearSampleFunction(torch.autograd.Function):
         img, fl = _as(images, m), _pairs(_as(flow, m))
         B, C, H, W = img.shape
         N = fl.shape[1]
+        groups = _channel_groups(C)
         with torch.cuda.device(img.device):
-            out = torch.empty(B, N, C, device=img.device, dtype=m.dtype)
-            m.call("umr_bilinear_sample_forward", False, _ptr(img), _ptr(fl), _ptr(out), B, C, H, W, N,
-                   _stream_ptr(img.device))
+            outs = []
+            for c0, c in groups:
+                part = img if len(groups) == 1 else img[:, c0:c0 + c].contiguous()
+                out = torch.empty(B, N, c, device=img.device, dtype=m.dtype)
+                m.call("umr_bilinear_sample_forward", False, _ptr(part), _ptr(fl), _ptr(out), B, c, H, W, N,
+                       _stream_ptr(img.device))
+                outs.append(out)
         ctx.save_for_backward(img, fl)
         ctx.img_grad = images.requires_grad
         ctx.mode = m
-        return out
+        return outs[0] if len(outs) == 1 else torch.cat(outs, dim=2)
 
     @staticmethod
     def backward(ctx, grad_out):
@@ -117,19 +134,27 @@ class BilinearSampleFunction(torch.autograd.Function):
         B, C, H, W = img.shape
         N = fl.shape[1]
         g = grad_out.contiguous().to(m.dtype)
+        groups = _channel_groups(C)
         with torch.cuda.device(img.device):
-            gflow = torch.empty_like(fl)
-            gimg = torch.empty_like(img) if ctx.img_grad else None
             tables = ()
             if m.gather:   # the image gradient gathers over samples keyed by their top-left cell: the cell -> samples table
                 rowptr = samples = None
-                if gimg is not None:
+                if ctx.img_grad:
                     cells = torch.empty(B, N, device=img.device, dtype=torch.int32)
                     m.call("umr_bilinear_sample_cells", False, _ptr(fl), _ptr(cells), B, H, W, N, _stream_ptr(img.device))
                     rowptr, samples = device_incidence(cells, B * (H + 1) * (W + 1))
                 tables = (_ptr(rowptr), _ptr(samples))
-            m.call("umr_bilinear_sample_backward", True, _ptr(img), _ptr(fl), _ptr(g), _ptr(gflow), _ptr(gimg),
-                   B, C, H, W, N, *tables, _stream_ptr(img.device))
+            gflow, gimgs = None, []
+            for c0, c in groups:
+                part, gpart = (img, g) if len(groups) == 1 else (img[:, c0:c0 + c].contiguous(), g[:, :, c0:c0 + c].contiguous())
+                gf = torch.empty_like(fl)
+                gi = torch.empty_like(part) if ctx.img_grad else None
+                m.call("umr_bilinear_sample_backward", True, _ptr(part), _ptr(fl), _ptr(gpart), _ptr(gf), _ptr(gi),
+                       B, c, H, W, N, *tables, _stream_ptr(img.device))
+                gflow = gf if gflow is None else gflow.add_(gf)
+                if gi is not None:
+                    gimgs.append(gi)
+            gimg = (gimgs[0] if len(gimgs) == 1 else torch.cat(gimgs, dim=1)) if gimgs else None
         return gimg, gflow
 
 
