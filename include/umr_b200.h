@@ -737,4 +737,7 @@ int umr_part_head_backward(const void* const* maps, const int64_t* map_bstrides,
 /* keypoint transfer of the keypoint evaluation (umr_kp_transfer_flow / _cam) */
 #include "umr_kp_transfer.h"
 
+/* SCOPS part centres and part points of CorrLossChamfer's targets (umr_part_points) */
+#include "umr_part_points.h"
+
 #endif /* UMR_B200_H_ */

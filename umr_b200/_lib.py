@@ -261,6 +261,16 @@ KP_EXPORTS = {
     "umr_kp_transfer_cam": (ctypes.c_int, [c_f32p] * 6 + [ctypes.c_int32] * 4 + [ctypes.c_void_p]),
 }
 
+# SCOPS part centres and part points (include/umr_part_points.h), bound by load() like EXPORTS, in a table of its own as
+# KP_EXPORTS is.
+PP_EXPORTS = {
+    # part_prob, mask, uniforms, B, S, C, K, channels, num_samples (host int32 [K]), dtype, centers_in, centers,
+    # points, drawn (host pointer arrays [K]), status, stream
+    "umr_part_points": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 4 +
+                        [ctypes.POINTER(ctypes.c_int32)] * 2 + [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p] +
+                        [ctypes.POINTER(ctypes.c_void_p)] * 2 + [ctypes.c_void_p, ctypes.c_void_p]),
+}
+
 _lock = threading.Lock()
 _lib = None
 
@@ -281,7 +291,7 @@ def load():
                     "libumr_b200.so is not built (%s). Run `python -m umr_b200.build` "
                     "(or __graft_entry__.build()). There is no CPU fallback." % LIB_PATH)
             lib = ctypes.CDLL(LIB_PATH)
-            for name, (res, args) in list(EXPORTS.items()) + list(KP_EXPORTS.items()):
+            for name, (res, args) in list(EXPORTS.items()) + list(KP_EXPORTS.items()) + list(PP_EXPORTS.items()):
                 fn = getattr(lib, name)  # AttributeError if the symbol is missing
                 fn.restype = res
                 fn.argtypes = args
