@@ -740,4 +740,7 @@ int umr_part_head_backward(const void* const* maps, const int64_t* map_bstrides,
 /* SCOPS part centres and part points of CorrLossChamfer's targets (umr_part_points) */
 #include "umr_part_points.h"
 
+/* SCOPS semantic template of avg_uv.py: UV part average and part labels (umr_st_*) */
+#include "umr_semantic_template.h"
+
 #endif /* UMR_B200_H_ */

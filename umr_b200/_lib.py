@@ -271,6 +271,22 @@ PP_EXPORTS = {
                         [ctypes.POINTER(ctypes.c_void_p)] * 2 + [ctypes.c_void_p, ctypes.c_void_p]),
 }
 
+# SCOPS semantic template (include/umr_semantic_template.h), bound by load() like EXPORTS, in a table of its own as
+# KP_EXPORTS is.
+ST_EXPORTS = {
+    # B, H, W
+    "umr_st_average_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 3),
+    # part_segs, uvimage_pred, exemplar, B, C, S, H, W, k, workspace, dist, selected, acc, stream
+    "umr_st_average_add": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 6 + [ctypes.c_void_p] * 5),
+    # acc, C, H, W, count, avg_prob, stream
+    "umr_st_average_mean": (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_int64, ctypes.c_void_p,
+                                                                                       ctypes.c_void_p]),
+    # avg_prob, H, W, C, uv_sampler, F_src, T2, num_sym_faces, vertex_rowptr, vertex_corners, V, label_image,
+    # texel_labels, face_labels, vertex_labels, stream
+    "umr_st_labels": (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_void_p] + [ctypes.c_int32] * 3 +
+                      [ctypes.c_void_p] * 2 + [ctypes.c_int32] + [ctypes.c_void_p] * 5),
+}
+
 _lock = threading.Lock()
 _lib = None
 
@@ -291,7 +307,8 @@ def load():
                     "libumr_b200.so is not built (%s). Run `python -m umr_b200.build` "
                     "(or __graft_entry__.build()). There is no CPU fallback." % LIB_PATH)
             lib = ctypes.CDLL(LIB_PATH)
-            for name, (res, args) in list(EXPORTS.items()) + list(KP_EXPORTS.items()) + list(PP_EXPORTS.items()):
+            for name, (res, args) in list(EXPORTS.items()) + list(KP_EXPORTS.items()) + list(PP_EXPORTS.items()) + \
+                    list(ST_EXPORTS.items()):
                 fn = getattr(lib, name)  # AttributeError if the symbol is missing
                 fn.restype = res
                 fn.argtypes = args

@@ -418,6 +418,21 @@ def batch_get_centers(pred_softmax, epsilon=1e-3):
     return torch.stack((xc, yc), dim=2)
 
 
+def label_image_one_hot(uv_img, uv_sampler, num_sym_faces, tex_size, num_labels=5):
+    """The per-texel one-hot part ids of a UV label image (loss_utils.py:341-356): uv_img [1,1,H,W] float labels sampled
+    at uv_sampler [1,F',T2,2] (grid_sample, align_corners=True), the last num_sym_faces faces appended again, rounded
+    and one-hot encoded -> [1,F'+num_sym_faces,T2,num_labels].  `part_matching_loss` builds its `stex_one_hot` from
+    `semantic_seg.png` with it, and `utils.semantic_template` from the label image it computes."""
+    tex = torch.nn.functional.grid_sample(uv_img, uv_sampler, align_corners=True)
+    tex = tex.view(tex.size(0), -1, tex.size(2), tex_size, tex_size).permute(0, 2, 3, 4, 1)
+    tex = torch.cat([tex, tex[:, -num_sym_faces:]], 1)
+    stex = torch.round(tex.reshape(tex.size(1), -1))
+    nf, nt = stex.size()
+    one_hot = torch.zeros(nf * nt, num_labels, device=stex.device)
+    one_hot.scatter_(1, stex.view(-1, 1).long(), 1)
+    return one_hot.view(1, nf, nt, num_labels)
+
+
 class part_matching_loss(nn.Module):
     """loss_utils.py:333-440.  `stex_one_hot` [1,F,T2,5] (one-hot semantic part id per texel) replaces
     the `semantic_seg.png` + `uv_sampler` lookup of :341-356; when it is None the reference's file
@@ -430,14 +445,7 @@ class part_matching_loss(nn.Module):
             from PIL import Image
             uv_img = np.asarray(Image.open(osp.join(scops_path, "semantic_seg.png"))).astype(np.float32)
             uv_img = torch.from_numpy(uv_img).view(1, 1, 128, 256).float().to(uv_sampler.device)
-            tex = torch.nn.functional.grid_sample(uv_img, uv_sampler, align_corners=True)
-            tex = tex.view(tex.size(0), -1, tex.size(2), tex_size, tex_size).permute(0, 2, 3, 4, 1)
-            tex = torch.cat([tex, tex[:, -num_sym_faces:]], 1)
-            stex = torch.round(tex.reshape(tex.size(1), -1))
-            nf, nt = stex.size()
-            one_hot = torch.zeros(nf * nt, 5, device=stex.device)
-            one_hot.scatter_(1, stex.view(-1, 1).long(), 1)
-            stex_one_hot = one_hot.view(1, nf, nt, 5)
+            stex_one_hot = label_image_one_hot(uv_img, uv_sampler, num_sym_faces, tex_size)
         n = batch_size * num_cam
         for k in (1, 2, 3, 4):
             self.register_buffer("stex%d" % k, stex_one_hot[:, :, :, k].unsqueeze(-1).repeat(n, 1, 1, 3))
