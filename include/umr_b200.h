@@ -743,4 +743,7 @@ int umr_part_head_backward(const void* const* maps, const int64_t* map_bstrides,
 /* SCOPS semantic template of avg_uv.py: UV part average and part labels (umr_st_*) */
 #include "umr_semantic_template.h"
 
+/* training batch crop, resize, mirror and normalisation of forward_img / set_input (umr_crop_batch) */
+#include "umr_crop.h"
+
 #endif /* UMR_B200_H_ */

@@ -96,6 +96,15 @@ def main():
     tex_edge = ops.load_textures(torch.rand(5, 4, 3, device=dev), uv_edge, torch.zeros(3, 9, 3, device=dev),
                                  torch.ones(3, dtype=torch.int32, device=dev))
     assert torch.isfinite(tex_edge).all()
+    # batch crop / resize / mirror / normalisation (both launches), then the part points on its outputs
+    from umr_b200.utils import crop_loader, image
+    wins = [crop_loader.CropWindow(rng.integers(0, 256, (9, 7, 3), dtype=np.uint8), np.ones((9, 7), np.uint8), 2, 1, 11, True),
+            crop_loader.CropWindow(rng.integers(0, 256, (5, 6, 1), dtype=np.uint8), np.ones((5, 6), np.uint8), 0, 3, 8, False)]
+    cb = crop_loader.collate([{"crop": w} for w in wins])
+    c_imgs, c_inp, c_masks, c_prob, c_segs = image.crop_batch(cb["crop_pack"].to(dev), cb["crop_table"], IS,
+                                                              torch.rand(2, IS, IS, 5, device=dev) + 0.1)
+    assert torch.isfinite(c_inp).all() and torch.isfinite(c_segs).all()
+    image.part_points(c_prob, c_masks, num_samples=(2, 2, 2, 2))
     total.backward()
     torch.cuda.synchronize()
     assert torch.isfinite(verts.grad).all() and torch.isfinite(cams.grad).all() and torch.isfinite(flow.grad).all()

@@ -287,6 +287,16 @@ ST_EXPORTS = {
                       [ctypes.c_void_p] * 2 + [ctypes.c_int32] + [ctypes.c_void_p] * 5),
 }
 
+# Training batch crop / resize / mirror / normalisation (include/umr_crop.h), bound by load() like EXPORTS, in a table
+# of its own as KP_EXPORTS is.
+CROP_EXPORTS = {
+    # pack, pack_bytes, table_dev, table_host, B, S, part_prob, C, imgs, input_imgs, masks, part_prob_out, part_segs,
+    # stream
+    "umr_crop_batch": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32),
+                                      ctypes.c_int32, ctypes.c_int32, ctypes.c_void_p, ctypes.c_int32] +
+                       [ctypes.c_void_p] * 6),
+}
+
 _lock = threading.Lock()
 _lib = None
 
@@ -308,7 +318,7 @@ def load():
                     "(or __graft_entry__.build()). There is no CPU fallback." % LIB_PATH)
             lib = ctypes.CDLL(LIB_PATH)
             for name, (res, args) in list(EXPORTS.items()) + list(KP_EXPORTS.items()) + list(PP_EXPORTS.items()) + \
-                    list(ST_EXPORTS.items()):
+                    list(ST_EXPORTS.items()) + list(CROP_EXPORTS.items()):
                 fn = getattr(lib, name)  # AttributeError if the symbol is missing
                 fn.restype = res
                 fn.argtypes = args

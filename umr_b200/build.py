@@ -23,7 +23,8 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-I", os.path
 # of the reference (DESIGN.md §4).  The loss kernels have no such constraint.
 PER_FILE = {"raster.cu": ["-fmad=false"], "raster_f64.cu": ["-fmad=false"], "losses_f64.cu": ["-fmad=false"],
             "vertex.cu": ["-fmad=false"], "mesh_ops.cu": ["-fmad=false"], "nmr.cu": ["-fmad=false"], "voxel.cu": ["-fmad=false"],
-            "kp_transfer.cu": ["-fmad=false"], "part_points.cu": ["-fmad=false"], "semantic_template.cu": ["-fmad=false"]}
+            "kp_transfer.cu": ["-fmad=false"], "part_points.cu": ["-fmad=false"], "semantic_template.cu": ["-fmad=false"],
+            "crop.cu": ["-fmad=false"]}
 
 
 def sources():

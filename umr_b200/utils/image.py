@@ -7,6 +7,10 @@
 loader, four channels per image on the CPU (data/base.py:155-166).  `part_points` does every channel of a whole batch in
 two kernel launches (csrc/part_points.cu, DESIGN.md §17); `prob2center` and `sample_prob` keep the reference's
 single-image signatures on top of it.
+
+`crop_batch` is the pixel half of the loader's `forward_img` (crop, cv2.resize, mirror: data/base.py:88-186) and of
+`set_input`'s ResNet normalisation and part-map normalisation (experiments/train_s2.py:166-192), for a whole batch in two
+kernel launches (csrc/crop.cu, DESIGN.md §19); the loader's half is `umr_b200.utils.crop_loader`.
 """
 import ctypes
 
@@ -136,3 +140,63 @@ def sample_prob(part_prob, mask, center, num_samples=10, ch=1, generator=None):
     c = torch.as_tensor(center, device=part_prob.device).reshape(1, 1, 2)
     _, points, _ = _part_points(part_prob[None], mask[None], u, (num_samples,), (ch,), centers_in=c)
     return points[0][0]
+
+
+CROP_TABLE_COLS = 8       # UMR_CROP_TABLE_COLS
+CROP_MAX_CHANNELS = 8     # UMR_CROP_MAX_CHANNELS
+
+
+def crop_batch(pack, table, size, part_prob=None):
+    """The batch `crop_loader.collate` packed, cropped, resized to size x size, mirrored and normalised on the GPU.
+
+    pack: uint8 [bytes] ('crop_pack'), on a CUDA device or pinned on the host; table: int32 [B,8] on the host
+    ('crop_table': offset, h, w, ch, x0, y0, L, flip per image), validated there and copied to the device without a
+    host synchronisation; part_prob: optional float32 [B,size,size,C] CUDA tensor, C <= 8, the SCOPS maps as loaded.
+    Returns (imgs [B,3,S,S], input_imgs [B,3,S,S], masks [B,S,S], part_prob [B,S,S,C] mirrored, part_segs [B,C,S,S]),
+    float32, the last two None without part_prob: cv2.resize INTER_LINEAR on the float64 crop frame rounded once to
+    float32, torchvision's ImageNet Normalize, and q / max(q) per (image, channel) for q = part_prob * masks.  One kernel
+    launch, two with part_prob; bitwise reproducible."""
+    if not isinstance(table, torch.Tensor) or table.is_cuda or table.dtype != torch.int32 or table.dim() != 2 \
+            or table.shape[1] != CROP_TABLE_COLS or table.shape[0] < 1:
+        raise ValueError("crop_batch: table must be a host int32 [B,%d] tensor" % CROP_TABLE_COLS)
+    if not isinstance(pack, torch.Tensor) or pack.dtype != torch.uint8 or pack.dim() != 1 or pack.numel() < 1:
+        raise ValueError("crop_batch: pack must be a non-empty uint8 [bytes] tensor")
+    if isinstance(size, bool) or int(size) != size or size < 1:
+        raise ValueError("crop_batch: size must be a positive integer, got %r" % (size,))
+    B, S = table.shape[0], int(size)
+    if part_prob is not None:
+        if not isinstance(part_prob, torch.Tensor) or not part_prob.is_cuda:
+            raise TypeError("crop_batch: part_prob must be a CUDA tensor")
+        if part_prob.dtype != torch.float32:
+            raise TypeError("crop_batch: part_prob must be float32, got %s" % part_prob.dtype)
+        if part_prob.dim() != 4 or tuple(part_prob.shape[:3]) != (B, S, S) or not 1 <= part_prob.shape[3] <= CROP_MAX_CHANNELS:
+            raise ValueError("crop_batch: part_prob must be [%d,%d,%d,C] with 1 <= C <= %d, got %s"
+                             % (B, S, S, CROP_MAX_CHANNELS, tuple(part_prob.shape)))
+        if pack.is_cuda and pack.device != part_prob.device:
+            raise ValueError("crop_batch: pack and part_prob must be on one device, got %s and %s"
+                             % (pack.device, part_prob.device))
+    if pack.is_cuda:
+        dev = pack.device
+    elif part_prob is not None:
+        dev = part_prob.device
+    else:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    tab = table.contiguous()
+    with torch.cuda.device(dev):
+        pk = pack.to(dev, non_blocking=True).contiguous()
+        tab_dev = tab.to(dev, non_blocking=True)
+        imgs = torch.empty(B, 3, S, S, device=dev)
+        input_imgs = torch.empty(B, 3, S, S, device=dev)
+        masks = torch.empty(B, S, S, device=dev)
+        prob = segs = None
+        C = 0
+        if part_prob is not None:
+            C = part_prob.shape[3]
+            part_prob = part_prob.detach().contiguous()
+            prob = torch.empty_like(part_prob)
+            segs = torch.empty(B, C, S, S, device=dev)
+        host = ctypes.cast(tab.data_ptr(), ctypes.POINTER(ctypes.c_int32))
+        _lib.check(_lib.load().umr_crop_batch(_ptr(pk), pk.numel(), _ptr(tab_dev), host, B, S, _ptr(part_prob), C,
+                                              _ptr(imgs), _ptr(input_imgs), _ptr(masks), _ptr(prob), _ptr(segs),
+                                              _stream_ptr(dev)), "umr_crop_batch")
+    return imgs, input_imgs, masks, prob, segs
